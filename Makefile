@@ -1,4 +1,4 @@
-# hpc-patterns-b200 — native build (sm_100a only).
+# hpc-patterns-b200 — native build (sm_90a only).
 #
 #   make            everything: static lib, CLIs in bin/, torch extension (_C.so)
 #   make cli        native CLIs only            make ext   torch extension only
@@ -15,7 +15,7 @@ NVCC      ?= nvcc
 HOSTCXX   ?= $(shell command -v /usr/bin/g++ || echo g++)
 override CXX := $(HOSTCXX)
 PYTHON    ?= python
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := -ccbin $(HOSTCXX) $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-fopenmp,-Wall -Icsrc
 CXXFLAGS  := -O2 -std=c++17 -fPIC -fopenmp -Wall -Wextra -Icsrc -I/usr/local/cuda/include
 BUILD     := build

@@ -1,63 +1,29 @@
-"""The one part of the reference that builds in this image, run UNMODIFIED: its OpenMP concurrency bench.
+"""The one part of the reference that builds with a host compiler, run UNMODIFIED: its OpenMP concurrency bench.
 
-argonne-lcf/HPC-Patterns has no Python package (``pip install /root/reference`` -> "not installable: neither
-setup.py nor pyproject.toml"), its GPU programs need icpx/SYCL, Level-Zero and a GPU-aware MPICH, none of which
-exist here — so the GPU headline has no reference arm (``bench.py --impl reference`` says so).  What does build
-is BASELINE.json's config #1, "concurency/bench compute+copy overlap on CPU host (OpenMP, no GPU)":
-``concurency/main.cpp`` + ``concurency/bench_omp.cpp`` with plain ``g++ -fopenmp`` (target regions fall back
-to the host).  ``baseline/_ref`` is a verbatim copy of ``/root/reference`` (git-ignored, travels to the GPU box);
-the only build-line addition is ``-Domp_target_alloc_host=omp_target_alloc`` (an Intel extension mapped to the
-standard call on the command line; the sources are untouched), the same two builds as concurency/run_omp.sh:6-7.
+argonne-lcf/HPC-Patterns has no Python package, its GPU programs need icpx/SYCL, Level-Zero and a GPU-aware MPICH —
+so the GPU headline has no reference arm (``bench.py --impl reference`` says so).  What does build is BASELINE.json's
+config #1, "concurency/bench compute+copy overlap on CPU host (OpenMP, no GPU)": ``concurency/main.cpp`` +
+``concurency/bench_omp.cpp`` with plain ``g++ -fopenmp``, compiled by ``build()`` into ``oracle/_ref/``
+(recipe: oracle/build_ref.py).
 
 Both arms run the reference's five command groups (run_omp.sh:9) through each program's stock ``main()`` and
 report the same numbers, parsed from the same stdout contract (main.cpp:284-319).
 """
 from __future__ import annotations
 
-import math
 import os
 import re
-import shutil
 import subprocess
 from typing import Dict, List, Optional
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
-REF_SRC = os.environ.get("HPCP_REFERENCE", "/root/reference")
 GROUPS = ["C C", "C M2D", "C D2M", "M2D D2M", "H2D D2H"]          # concurency/run_omp.sh:9
-MODES = {"nowait": "NOWAIT", "host_threads": "HOST_THREADS"}       # run_omp.sh:6-7
 
 
-def host_cxx() -> str:
-    return os.environ.get("HOSTCXX") or ("/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++")
+def reference_binary(mode: str = "nowait") -> Optional[str]:
+    from oracle import build_ref
 
-
-def ensure_ref() -> Optional[str]:
-    """Verbatim copy of the reference under baseline/_ref (made once, where /root/reference is mounted)."""
-    if os.path.exists(os.path.join(REF_DIR, "concurency", "main.cpp")):
-        return REF_DIR
-    if not os.path.exists(os.path.join(REF_SRC, "concurency", "main.cpp")):
-        return None
-    if os.path.isdir(REF_DIR):
-        shutil.rmtree(REF_DIR)
-    shutil.copytree(REF_SRC, REF_DIR)
-    return REF_DIR
-
-
-def build_reference(mode: str = "nowait") -> Optional[str]:
-    ref = ensure_ref()
-    if ref is None or mode not in MODES:
-        return None
-    out_dir = os.path.join(ref, "_build")
-    exe = os.path.join(out_dir, f"omp_{mode}")
-    srcs = [os.path.join(ref, "concurency", f) for f in ("main.cpp", "bench_omp.cpp")]
-    if os.path.exists(exe) and all(os.path.getmtime(exe) >= os.path.getmtime(s) for s in srcs):
-        return exe
-    os.makedirs(out_dir, exist_ok=True)
-    p = subprocess.run([host_cxx(), "-O2", "-std=c++17", "-fopenmp", f"-D{MODES[mode]}",
-                        "-Domp_target_alloc_host=omp_target_alloc", *srcs, "-o", exe],
-                       capture_output=True, text=True, timeout=900)
-    return exe if p.returncode == 0 else None
+    return build_ref.binary(mode)
 
 
 def ours_binary() -> Optional[str]:
@@ -100,32 +66,28 @@ def parse_concurency(text: str) -> List[Dict]:
     return [g for g in groups if "speedup" in g]
 
 
-def run_cpu_concurency(impl: str, mode: str = "nowait", repetitions: int = 5, elements: int = 8_000_000,
-                       tripcount: int = 40000, threads: Optional[int] = None) -> Dict:
-    """Run the five reference command groups through the stock main() of `impl` ('reference' or 'ours').
-
-    Every tunable is given on the command line (``--tripcount_C``, ``--globalsize_<copy>``: public flags of both
-    programs, main.cpp:143-196) so that neither program autotunes: on a host-only build the reference's copies
-    (``#pragma omp target update``, bench_omp.cpp:83-95) are no-ops that take 0 us, its autotuner then scales every
-    size to zero and the program aborts on ``omp_target_alloc(0)`` ("Wrong Allocation").  For the same reason only the
-    ``C C`` group does real work in the reference arm; it is the headline of this config, the other groups are listed.
-    """
-    exe = build_reference(mode) if impl == "reference" else ours_binary()
-    if exe is None:
-        return {"impl": impl, "unavailable": "reference tree / binary not present"}
+def cpu_concurency_command(exe: str, mode: str = "nowait", repetitions: int = 5, elements: int = 8_000_000,
+                           tripcount: int = 40000) -> List[str]:
+    """The command line both arms run: every tunable given explicitly (``--tripcount_C``, ``--globalsize_<copy>``:
+    public flags of both programs, main.cpp:143-196) so that neither program autotunes: on a host-only build the
+    reference's copies (``#pragma omp target update``, bench_omp.cpp:83-95) are no-ops that take 0 us, its autotuner
+    then scales every size to zero and the program aborts on ``omp_target_alloc(0)`` ("Wrong Allocation").  For the
+    same reason only the ``C C`` group does real work in the reference arm; it is the headline of this config, the
+    other groups are listed."""
     cmd = [exe, mode, "--repetitions", str(repetitions), "--tripcount_C", str(tripcount)]
     for c in ("MD", "DM", "HD", "DH"):
         cmd += [f"--globalsize_{c}", str(elements)]
     for g in GROUPS:
         cmd += ["--commands"] + g.split()
-    env = dict(os.environ)
-    env["OMP_NUM_THREADS"] = str(threads or min(os.cpu_count() or 1, 8))
-    env.pop("OMP_PROC_BIND", None)
-    p = subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=env)
-    groups = parse_concurency(p.stdout)
+    return cmd
+
+
+def summarize(impl: str, stdout: str, stderr: str = "", rc: int = 0, mode: str = "nowait", tripcount: int = 40000) -> Dict:
+    """The config's JSON result from one program's stdout."""
+    groups = parse_concurency(stdout)
     cc = next((g for g in groups if g["commands"].split() == ["C", "C"]), None)
     if cc is None:
-        return {"impl": impl, "unavailable": f"unexpected output (rc {p.returncode}): {p.stdout[-300:]} {p.stderr[-300:]}"}
+        return {"impl": impl, "unavailable": f"unexpected output (rc {rc}): {stdout[-300:]} {stderr[-300:]}"}
 
     def num(x):
         return None if x is None or x != x or x in (float("inf"), float("-inf")) else x
@@ -142,6 +104,24 @@ def run_cpu_concurency(impl: str, mode: str = "nowait", repetitions: int = 5, el
                        "concurrent_us": num(g.get("concurrent_us")), "verdict": g.get("verdict")} for g in groups],
         "note": "host-only build: the reference's copy commands are no-op target updates (0 us), so only 'C C' "
                 "compares like with like; ours executes real host memcpys for M/D/H",
-        "omp_threads": int(env["OMP_NUM_THREADS"]), "repetitions": repetitions, "elements": elements,
-        "binary": os.path.relpath(exe, ROOT), "rc": p.returncode,
+        "rc": rc,
     }
+
+
+def run_cpu_concurency(impl: str, mode: str = "nowait", repetitions: int = 5, elements: int = 8_000_000,
+                       tripcount: int = 40000, threads: Optional[int] = None) -> Dict:
+    """Run the five reference command groups through the stock main() of `impl` ('reference' or 'ours')."""
+    exe = reference_binary(mode) if impl == "reference" else ours_binary()
+    if exe is None:
+        return {"impl": impl, "unavailable": "binary not built (reference: oracle/build_ref.py needs the reference "
+                                             "checkout)"}
+    env = dict(os.environ)
+    env["OMP_NUM_THREADS"] = str(threads or min(os.cpu_count() or 1, 8))
+    env.pop("OMP_PROC_BIND", None)
+    p = subprocess.run(cpu_concurency_command(exe, mode, repetitions, elements, tripcount), capture_output=True,
+                       text=True, timeout=900, env=env)
+    out = summarize(impl, p.stdout, p.stderr, p.returncode, mode, tripcount)
+    if "unavailable" not in out:
+        out.update(omp_threads=int(env["OMP_NUM_THREADS"]), repetitions=repetitions, elements=elements,
+                   binary=os.path.relpath(exe, ROOT))
+    return out

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Flagship benchmark: slab stencil fused with its halo exchange over NVLink, ring of N B200s.
+"""Flagship benchmark: slab stencil fused with its halo exchange over NVLink, ring of N H100s.
 
 Metric (BASELINE.json): P2P bus GB/s at the reference's message size (188 743 680 B = 47 185 920 floats,
 p2p/peer2pear.cpp:115-116) and compute/comm overlap %, device-timed, max over ranks, whole-job aggregate.
@@ -11,14 +11,20 @@ the previous step produced on the neighbours, the dependency structure of the re
 (compute; Send/Recv with both ring neighbours; swap; compute — allreduce-mpi-sycl.cpp:167-181).  The exchange is
 inside the stencil kernel (pull: TMA bulk loads from the neighbours' fields; push: TMA bulk stores into their halo
 buffers), K steps are ONE persistent launch, no NCCL / cudaMemcpy / host sync on the path.  Per step a rank moves one
-message to (or from) each neighbour: value = N x 2 x message / time.  `rows` balances the step's HBM time against its
-NVLink time, the rule of the reference's autotuner (concurency/main.cpp:219-258).  N=1: the rank is its own neighbour.
+message to (or from) each neighbour: value = N x 2 x message / time.  `rows` (8 by default) sets the step's HBM work
+next to its two NVLink messages, as the reference's autotuner sizes commands against each other
+(concurency/main.cpp:219-258).  N=1: the rank is its own neighbour.
 
 Contract: `python bench.py --gpus N --steps K --warmup W`; for N>1 launched by torchrun (one rank per GPU).
-Rank 0 prints ONE JSON line.  Timing: W>=3 untimed warm-up steps, a time-based pre-heat, then `--blocks` blocks of
-EXACTLY K steps, each behind an in-kernel cross-GPU barrier, CUDA events on the launching stream, max over ranks;
-`value` is the best block (the reference reports the minimum over 10 iterations, peer2pear.cpp:23,52), all blocks are
-listed.  `--impl reference`: the reference's GPU programs cannot be built here (no SYCL / Level-Zero / MPI) -> prints
+Rank 0 prints ONE JSON line.  Timing: W>=3 untimed warm-up steps, a time-based pre-heat (a number of K-step blocks
+that depends on how long a block takes), then `--blocks` timed blocks of EXACTLY K steps (blocks x K timed steps in
+all), each behind an in-kernel cross-GPU barrier, CUDA events on the launching stream, max over ranks; `value` is the
+best block (the reference reports the minimum over 10 iterations, peer2pear.cpp:23,52), all blocks are listed.
+`--dump-outputs DIR` writes what a timed block computes: because the number of pre-heat blocks varies, the field after
+the series is not reproducible, so the field is reset to the closed-form initial field and ONE block of K steps (the
+same single launch the series times) is run again; a fixed sample of that field goes to .npy files, so two builds can
+be compared output for output.
+`--impl reference`: the reference's GPU programs cannot be built here (no SYCL / Level-Zero / MPI) -> prints
 {"impl": "reference", "unavailable": ...}; `--config cpu_concurency` runs the one part that does build (its OpenMP
 concurrency bench, unmodified, baseline/reference_arm.py) for either impl.
 """
@@ -39,22 +45,9 @@ REFERENCE_UNAVAILABLE = ("argonne-lcf/HPC-Patterns is C++17 SYCL/OpenMP-offload/
                          "GPU-aware MPICH, none of which exists in this image.  Only its host OpenMP concurrency bench "
                          "builds (g++ -fopenmp): see the cpu_concurency field / --config cpu_concurency")
 MESSAGE_BYTES = 1179648 * 40 * 4
-HBM_GBS_MEASURED = 6567.4     # MEASURED_PEAKS.json hbm_gbs (copy, read+write bytes)
-NVLINK_GBS_MEASURED = 770.0   # measured peer copy, ONE direction busy (B200_PROFILING.md); 900 nominal
-NVLINK_BIDIR_GBS_MEASURED = 706.1   # copy engines with BOTH directions of a pair busy: 1412.2 GB/s per pair
-                                    # (profiles/r2_call3_2gpu/p2p_tune.jsonl) — what a neighbour exchange can get
-
-
-def measured_hbm_gbs() -> float:
-    """Roofline denominator: the driver-written copy bandwidth of THIS box generation (MEASURED_PEAKS.json), the
-    committed value when the file is missing or unreadable.  `rows` keeps using the committed constant so that the
-    benchmark's configuration does not move with a re-measurement."""
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            v = float(json.load(f)["hbm_gbs"])
-        return v if v > 0 else HBM_GBS_MEASURED
-    except Exception:
-        return HBM_GBS_MEASURED
+HBM_GBS_DATASHEET = 3350.0    # H100 SXM HBM3, NVIDIA data sheet (not a measurement)
+NVLINK_GBS_NOMINAL = 450.0    # H100 SXM NVLink 4 per direction (900 GB/s bidirectional, data sheet)
+DUMP_SAMPLE = 1 << 22         # field values written by --dump-outputs (a fixed, seeded sample of the whole field)
 
 
 def env_int(name: str, default: int) -> int:
@@ -70,7 +63,7 @@ def parse_args():
     ap.add_argument("--config", default="halo", choices=("halo", "cpu_concurency"))
     ap.add_argument("--bytes", type=int, default=MESSAGE_BYTES, help="one message = one row of the slab")
     ap.add_argument("--rows", type=int, default=env_int("HPCP_BENCH_ROWS", 0),
-                    help="rows per slab; 0 -> balanced (HBM time = NVLink time at the measured peaks)")
+                    help="rows per slab; 0 -> 8")
     ap.add_argument("--mode", default=os.environ.get("HPCP_BENCH_MODE", "pull"), choices=("pull", "push"))
     ap.add_argument("--ctas", type=int, default=env_int("HPCP_BENCH_CTAS", 0))
     ap.add_argument("--tile-kb", type=int, default=env_int("HPCP_BENCH_TILE_KB", 0))
@@ -79,6 +72,8 @@ def parse_args():
     ap.add_argument("--preheat-ms", type=float, default=float(os.environ.get("HPCP_BENCH_PREHEAT_MS", "300")))
     ap.add_argument("--e2e-steps", type=int, default=4)
     ap.add_argument("--no-extras", action="store_true", help="skip the unfused / stock / legacy comparison runs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the field after one timed block (K steps from the initial field) as DIR/*.npy")
     return ap.parse_args()
 
 
@@ -86,6 +81,30 @@ def cpu_concurency(impl: str) -> dict:
     from baseline import reference_arm
 
     return reference_arm.run_cpu_concurency(impl)
+
+
+def dump_field(hs, steps: int, out_dir: str, comm) -> None:
+    """The timed path's result, reproducibly: the field after ONE timed block (``steps`` steps in one persistent launch)
+    from the closed-form initial field — the timed series itself runs a time-based number of blocks.  Every rank writes
+    the same seeded sample positions of its slab (field_rank<r>.npy, float32) and rank 0 the flat positions
+    (field_index.npy, float64); the sample is split over the ranks so all files together stay below 64 MB."""
+    import numpy as np
+    import torch
+
+    hs.reset()
+    hs.step(steps)
+    torch.cuda.synchronize(hs.device)
+    u = hs.u_tensor().reshape(-1)
+    n = min(u.numel(), max(1, DUMP_SAMPLE // comm.world))
+    idx = np.sort(np.random.default_rng(0).choice(u.numel(), size=n, replace=False)) if n < u.numel() \
+        else np.arange(u.numel())
+    sample = u[torch.from_numpy(idx).to(u.device)].cpu().numpy().astype(np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"field_rank{comm.rank}.npy"), sample)
+    if comm.rank == 0:
+        np.save(os.path.join(out_dir, "field_index.npy"), idx.astype(np.float64))
+    hs.check()
+    comm.barrier()
 
 
 def main() -> int:
@@ -107,13 +126,13 @@ def main() -> int:
 
     import torch
 
-    from hpc_patterns_b200.models.halo import HaloStencil, balanced_rows
+    from hpc_patterns_b200.models.halo import DEFAULT_ROWS, HaloStencil
     from hpc_patterns_b200.parallel.comm import Comm
     from hpc_patterns_b200.utils.clocks import ClockSampler
     from hpc_patterns_b200.utils.timing import BlockTimer
 
     if not torch.cuda.is_available():
-        print(json.dumps({"error": "no CUDA device: bench.py measures sm_100a kernels"}))
+        print(json.dumps({"error": "no CUDA device: bench.py measures sm_90a kernels"}))
         return 1
 
     comm = Comm()
@@ -132,7 +151,7 @@ def main() -> int:
             uuid = None
         sampler = ClockSampler(gpu_index=device, period_ms=1.0, uuid=uuid).start(paused=True)
 
-    rows = args.rows if args.rows > 0 else balanced_rows(HBM_GBS_MEASURED, NVLINK_BIDIR_GBS_MEASURED)
+    rows = args.rows if args.rows > 0 else DEFAULT_ROWS
     tune = {k: v for k, v in (("ctas", args.ctas), ("tile_kb", args.tile_kb), ("stages", args.stages)) if v}
     K, W = args.steps, max(args.warmup, 3)
     hs = HaloStencil(comm, device, args.bytes, rows, args.mode, tune=tune)
@@ -155,13 +174,15 @@ def main() -> int:
                                         # barrier is enqueued before the start event, i.e. outside the region)
     total_fused_launches = hs.launches - launches0
     wrong_last = int(comm.sum(hs.verify_last_step()))
+    if args.dump_outputs:
+        dump_field(hs, K, args.dump_outputs, comm)
     ms_per_step = fused["ms"]
     msg = args.bytes
     value = world * 2 * msg / (ms_per_step * 1e-3) / 1e9          # aggregate GB/s over all GPUs, both neighbours
     per_gpu_dir = msg * 2 / (ms_per_step * 1e-3) / 1e9            # per GPU per direction
-    hbm_peak = measured_hbm_gbs()
+    hbm_peak = HBM_GBS_DATASHEET
     hbm_ms = hs.hbm_bytes_per_step() / hbm_peak / 1e6
-    nvl_ms = (hs.nvlink_bytes_per_step() / NVLINK_BIDIR_GBS_MEASURED / 1e6) if world > 1 else 0.0
+    nvl_ms = (hs.nvlink_bytes_per_step() / NVLINK_GBS_NOMINAL / 1e6) if world > 1 else 0.0
     roof_ms = max(hbm_ms, nvl_ms)
 
     extras = {}
@@ -189,7 +210,7 @@ def main() -> int:
         stock_nowait = timer.measure(lambda: [hs.stock_step("memcpy", host_wait=False) for _ in range(k)], k, blocks=3,
                                      preheat_ms=0)
         # share of the shorter piece that the fused step hides; the raw value exceeds 100 when the fused kernel is also
-        # faster than the LONGER piece run alone (N=8: the stand-alone exchange to two different peers takes 0.71 ms)
+        # faster than the LONGER piece run alone
         overlap_raw = (t_compute["ms"] + t_xchg["ms"] - ms_per_step) / min(t_compute["ms"], t_xchg["ms"]) * 100.0
         overlap = min(overlap_raw, 100.0)
         extras.update({
@@ -215,8 +236,8 @@ def main() -> int:
             bad1 = int(comm.sum(hs1.verify_last_step()))
             extras["rows_1"] = {"ms_per_step": round(t1["ms"], 5),
                                 "per_gpu_per_direction_GBps": round(2 * msg / (t1["ms"] * 1e-3) / 1e9, 1),
-                                "frac_of_nvlink_770_measured": round(2 * msg / (t1["ms"] * 1e-3) / 1e9 / 770.0, 3)
-                                if world > 1 else None,
+                                "frac_of_nvlink_450_nominal": round(2 * msg / (t1["ms"] * 1e-3) / 1e9 / NVLINK_GBS_NOMINAL,
+                                                                    3) if world > 1 else None,
                                 "wrong_words": bad1}
             hs1.close()
         # round-1 flagship (unidirectional ring put of a triad, no dependency between steps) under THIS harness
@@ -281,9 +302,7 @@ def main() -> int:
                 "global_batch": world, "seq_len": msg // 4, "parallelism": f"ring{world}",
                 "message_bytes": msg, "messages_per_step_per_gpu": 2, "rows": rows, "mode": args.mode,
                 "ctas": hs.ctas, "steps_per_launch": K,
-                "rows_rule": "rows such that the step's HBM time ~ its NVLink time at stock measured rates (HBM copy "
-                             "6567 GB/s; copy engines with both directions busy 706 GB/s/dir) — the balancing rule of "
-                             "the reference's autotuner",
+                "rows_rule": "8 rows of one message per slab unless --rows is given",
                 "peer": "self (no NVLink at N=1)" if world == 1 else "rank-1 and rank+1 over NVLink/NVSwitch",
                 "l2": f"inputs larger than L2: {(2 * rows + 2)} x 180 MiB streamed per step, no reuse between steps",
                 "timing": "in-kernel cross-GPU barrier, then cuda events on the launching stream; max over ranks; "
@@ -305,15 +324,13 @@ def main() -> int:
                                  "one_launch_per_step_ms is the same kernel launched K times",
             "wrong_words": wrong_init + wrong_last,
             "per_gpu_per_direction_GBps": round(per_gpu_dir, 1),
-            "frac_of_nvlink_706_measured_bidirectional": round(per_gpu_dir / NVLINK_BIDIR_GBS_MEASURED, 3) if world > 1 else None,
-            "frac_of_nvlink_770_measured": round(per_gpu_dir / 770.0, 3) if world > 1 else None,
-            "frac_of_nvlink_900_nominal": round(per_gpu_dir / 900.0, 3) if world > 1 else None,
+            "frac_of_nvlink_450_nominal": round(per_gpu_dir / NVLINK_GBS_NOMINAL, 3) if world > 1 else None,
             "hbm_traffic_GBps": round(hs.hbm_bytes_per_step() / (ms_per_step * 1e-3) / 1e9, 1),
             "roofline": {"hbm_ms": round(hbm_ms, 4), "nvlink_ms": round(nvl_ms, 4), "bound_ms": round(roof_ms, 4),
                          "frac": round(roof_ms / ms_per_step, 3),
-                         "hbm_gbs": hbm_peak, "nvlink_gbs_per_dir": NVLINK_BIDIR_GBS_MEASURED,
-                         "of": "max(HBM bytes / MEASURED_PEAKS.json hbm_gbs (copy peak), NVLink bytes per direction / "
-                               "706.1 GB/s measured with both directions busy)"},
+                         "hbm_gbs": hbm_peak, "nvlink_gbs_per_dir": NVLINK_GBS_NOMINAL,
+                         "of": "max(HBM bytes / 3350 GB/s (HBM3, data sheet), NVLink bytes per direction / 450 GB/s "
+                               "nominal)"},
             **extras,
         }
         if not args.no_extras:

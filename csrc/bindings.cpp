@@ -108,7 +108,7 @@ std::unique_ptr<con::Backend> backend_from(const std::string& choice) {
 }  // namespace
 
 PYBIND11_MODULE(_C, m) {
-  m.doc() = "hpc-patterns-b200 native extension (sm_100a kernels + peer memory + topology)";
+  m.doc() = "hpc-patterns-b200 native extension (sm_90a kernels + peer memory + topology)";
 
   // ------------------------------------------------------------ constants ----
   m.attr("PAD_WORDS") = kPadWords;
@@ -262,7 +262,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("dst"), py::arg("src"), py::arg("bytes"), py::arg("src_is_peer") = false,
       py::arg("engine") = "ldst", py::arg("tune") = py::dict(), py::arg("sync") = py::dict(),
       py::arg("device") = 0, py::arg("stream") = 0,
-      "dst[0:bytes] = src[0:bytes] with an sm_100a kernel; either side may be a peer pointer. "
+      "dst[0:bytes] = src[0:bytes] with an sm_90a kernel; either side may be a peer pointer. "
       "Returns the number of CTAs launched (advance the ticket counter by it).");
   m.def("fill_pattern", [](uintptr_t dst, size_t n_words, uint32_t seed, uintptr_t stream) {
     launch_fill_pattern(as_ptr<uint32_t>(dst), n_words, seed, as_stream(stream));
@@ -418,7 +418,7 @@ PYBIND11_MODULE(_C, m) {
     launch_tc_busy(as_ptr<const void>(operands), as_ptr<float>(out), ctas, tripcount, as_stream(stream), cluster);
   }, py::arg("operands"), py::arg("out"), py::arg("ctas"), py::arg("tripcount"), py::arg("stream") = 0,
   py::arg("cluster") = 1,
-  "tcgen05 tile loop: out[cta] = tripcount * (A[128x64] . B[256x64]^T), operands via TMA, accumulator in TMEM.");
+  "wgmma tile loop: out[cta] = tripcount * (A[128x64] . B[256x64]^T), operands via TMA, accumulator in registers.");
 
   m.def(
       "gemm_put",
@@ -431,7 +431,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("a"), py::arg("b"), py::arg("c_local"), py::arg("c_peer"), py::arg("m"), py::arg("n"), py::arg("k"),
       py::arg("out_bf16") = false, py::arg("sync") = py::dict(), py::arg("ctas") = 0, py::arg("device") = 0,
       py::arg("stream") = 0, py::arg("cluster") = 0, py::arg("tma_epilogue") = false,
-      "tcgen05 GEMM C = A . B^T (bf16 in, fp32 out) whose epilogue stores to c_local and/or the peer-mapped c_peer.");
+      "wgmma GEMM C = A . B^T (bf16 in, fp32 out) whose epilogue stores to c_local and/or the peer-mapped c_peer.");
 
   m.def(
       "gemm_reduce_scatter",
@@ -467,7 +467,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("n"), py::arg("k"), py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0,
       py::arg("cluster") = 0, py::arg("c_multicast") = 0, py::arg("out_bf16") = false,
       py::arg("tma_epilogue") = false,
-      "tcgen05 GEMM whose epilogue adds every tile into the owner's fp32 shard over NVLink (GEMM -> reduce-scatter), "
+      "wgmma GEMM whose epilogue adds every tile into the owner's fp32 shard over NVLink (GEMM -> reduce-scatter), "
       "or, with c_multicast, into every rank's copy through the NVSwitch (GEMM -> all-reduce).");
   m.def(
       "gemm_all_to_all",
@@ -500,7 +500,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("done_flags") = std::vector<uintptr_t>(), py::arg("done_epoch") = 0, py::arg("ticket") = 0,
       py::arg("ticket_base") = 0, py::arg("rank") = 0, py::arg("m"), py::arg("n"), py::arg("k"), py::arg("ctas") = 0,
       py::arg("device") = 0, py::arg("stream") = 0, py::arg("cluster") = 0,
-      "tcgen05 GEMM whose epilogue stores row block q of the result into rank q's receive buffer (GEMM -> all-to-all).");
+      "wgmma GEMM whose epilogue stores row block q of the result into rank q's receive buffer (GEMM -> all-to-all).");
   // Tile / gather orderings of the tensor-core kernels (kernels/tile_order.h), exposed for the CPU tests.
   m.def("gemm_tile_coords", [](int tile, int tiles_m, int tiles_n) {
     int mb = 0, nb = 0;
@@ -559,7 +559,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("done_epoch") = 0, py::arg("ticket") = 0, py::arg("ticket_base") = 0, py::arg("timeout_ns") = 0,
       py::arg("status") = 0, py::arg("rank") = 0, py::arg("m"), py::arg("n"), py::arg("k"), py::arg("ctas") = 0,
       py::arg("device") = 0, py::arg("stream") = 0, py::arg("cluster") = 0, py::arg("activation") = 0,
-      "tcgen05 GEMM over row-sharded A: one gather thread per CTA pulls the peers' rows (TMA bulk, NVLink) while "
+      "wgmma GEMM over row-sharded A: one gather thread per CTA pulls the peers' rows (TMA bulk, NVLink) while "
       "the tiles of the rows that are already here are computed (all-gather -> GEMM).");
   m.def(
       "wait_flags",

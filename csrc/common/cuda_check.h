@@ -40,8 +40,7 @@ inline void cuda_check(cudaError_t e, const char* expr, const char* file, int li
 // Opt a kernel into `bytes` of dynamic shared memory AND ask for the maximum shared-memory
 // carveout.  The carveout matters for co-residency: an SM configured for a small carveout by an
 // earlier launch cannot host a CTA of a later kernel that needs more until it drains, which
-// serialises kernels that were meant to overlap (measured: `fused | T C` 1.04x before, see
-// profiles/r1_call4_1gpu/call4_concurency.txt).
+// serialises kernels that were meant to overlap.
 template <typename Kernel>
 inline void enable_dynamic_smem(Kernel kernel, size_t bytes, const char* file, int line) {
   cuda_check(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -56,8 +55,8 @@ inline void enable_dynamic_smem(Kernel kernel, size_t bytes, const char* file, i
 // its module, and that load cannot complete while another kernel is running on the device.  This suite runs kernels
 // that spin on words a peer's kernel will write; when two ranks share a GPU (more ranks than devices) the peer's
 // FIRST launch of e.g. `signal_kernel` then waits for the spinning kernel, which waits for that signal: a deadlock
-// that only the 30 s device-side deadline breaks (found in round 2: every >= 3-ranks-per-GPU run and the
-// rendezvous / copy-engine transports of peer2pear on one GPU timed out; profiles/r2_call2_1gpu/virtual_ranks_diag.txt).
+// that only the 30 s device-side deadline breaks (every >= 3-ranks-per-GPU run and the rendezvous / copy-engine
+// transports of peer2pear on one GPU would time out).
 // Eager loading makes every kernel resident at start-up.  An explicit user setting wins.
 inline void prefer_eager_module_loading() { (void)setenv("CUDA_MODULE_LOADING", "EAGER", /*overwrite=*/0); }
 

@@ -1,6 +1,6 @@
 // NVTX ranges for timelines (nsys / ncu range filtering).  Header-only NVTX v3: no library to link;
 // when no tool is attached the calls are no-ops.  The reference has no tracing beyond
-// `set -o xtrace` in its sweep scripts (SURVEY.md §5).
+// `set -o xtrace` in its sweep scripts.
 #pragma once
 
 #include <nvtx3/nvToolsExt.h>

@@ -1,7 +1,7 @@
-// Inline-PTX vocabulary for sm_100a used by every kernel in this suite.
+// Inline-PTX vocabulary for sm_90a used by every kernel in this suite.
 //
 // This is the device-side replacement for the communication calls the
-// reference makes through GPU-aware MPICH (SURVEY.md §2.5): system-scope
+// reference makes through GPU-aware MPICH: system-scope
 // acquire/release signal words stand in for MPI_Win_fence / MPI_Waitall /
 // MPI_Barrier, vector and TMA-bulk stores to peer-mapped addresses stand in
 // for MPI_Put / MPI_Isend, `multimem.*` stands in for MPI_Allreduce.
@@ -105,33 +105,31 @@ __device__ __forceinline__ void red_add_bf16x8_sys(void* p, const uint4& v) {
                : "memory");
 }
 
-// --------------------------------------------- 256-bit ld / st (sm_100+) ----
-// One LDG.256 / STG.256 per thread: a warp covers 1 KiB contiguous per access.
+// ------------------------------------------------ 32-byte ld / st pairs ----
+// 32 bytes per thread as two adjacent 128-bit accesses (sm_90 has no 256-bit LDG/STG): a warp still covers 1 KiB
+// contiguous per loop iteration, with twice the bytes in flight per thread of the 16-byte form.
 struct alignas(32) U32x8 {
   uint32_t v[8];
 };
 __device__ __forceinline__ U32x8 ld_stream_v8(const U32x8* p) {
   U32x8 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]),
-                 "=r"(r.v[6]), "=r"(r.v[7])
-               : "l"(p));
+  const uint4 lo = ld_stream_v4(reinterpret_cast<const uint4*>(p));
+  const uint4 hi = ld_stream_v4(reinterpret_cast<const uint4*>(p) + 1);
+  r.v[0] = lo.x, r.v[1] = lo.y, r.v[2] = lo.z, r.v[3] = lo.w;
+  r.v[4] = hi.x, r.v[5] = hi.y, r.v[6] = hi.z, r.v[7] = hi.w;
   return r;
 }
 __device__ __forceinline__ U32x8 ld_weak_v8(const U32x8* p) {
   U32x8 r;
-  asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]),
-                 "=r"(r.v[6]), "=r"(r.v[7])
-               : "l"(p)
-               : "memory");
+  const uint4 lo = ld_weak_v4(reinterpret_cast<const uint4*>(p));
+  const uint4 hi = ld_weak_v4(reinterpret_cast<const uint4*>(p) + 1);
+  r.v[0] = lo.x, r.v[1] = lo.y, r.v[2] = lo.z, r.v[3] = lo.w;
+  r.v[4] = hi.x, r.v[5] = hi.y, r.v[6] = hi.z, r.v[7] = hi.w;
   return r;
 }
 __device__ __forceinline__ void st_stream_v8(U32x8* p, const U32x8& r) {
-  asm volatile("st.global.L1::no_allocate.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p),
-               "r"(r.v[0]), "r"(r.v[1]), "r"(r.v[2]), "r"(r.v[3]), "r"(r.v[4]), "r"(r.v[5]),
-               "r"(r.v[6]), "r"(r.v[7])
-               : "memory");
+  st_stream_v4(reinterpret_cast<uint4*>(p), make_uint4(r.v[0], r.v[1], r.v[2], r.v[3]));
+  st_stream_v4(reinterpret_cast<uint4*>(p) + 1, make_uint4(r.v[4], r.v[5], r.v[6], r.v[7]));
 }
 
 // ------------------------------------------------------------- mbarrier ----

@@ -12,7 +12,7 @@
 //   MPI_Barrier        p2p/peer2pear.cpp:26         -> barrier_all()
 //   blocking Send/Recv allreduce-mpi-sycl.cpp:50-58 -> per-chunk arrival words
 //
-// A hung peer must produce an error, not a hang (SURVEY.md §5 "failure
+// A hung peer must produce an error, not a hang ("failure
 // detection"): every spin has a %globaltimer deadline; on expiry the waiter
 // records a code in a status word and returns false so the kernel can drain.
 #pragma once

@@ -1,4 +1,4 @@
-// CUDA backend of the concurrency benchmark (B200).
+// CUDA backend of the concurrency benchmark (H100).
 //
 // Same question as the reference's SYCL and OpenMP-offload backends
 // (concurency/bench_sycl.cpp:19-139, bench_omp.cpp:21-137) — do independent
@@ -11,7 +11,7 @@
 //   host_threads  one host thread + stream per command              (↔ OpenMP host_threads)
 //   nowait        one thread, async launches on non-blocking streams, event
 //                 join on a master stream                           (↔ OpenMP target nowait + taskwait)
-//   fused         the whole group as ONE persistent sm_100a kernel: CTAs split
+//   fused         the whole group as ONE persistent sm_90a kernel: CTAs split
 //                 between FMA/triad math and TMA copy engines        (new — the product)
 // Memory letters: M pageable, H pinned, D device, S managed, P peer GPU (NVLink).
 #include <atomic>
@@ -159,7 +159,7 @@ class CudaBackend final : public Backend {
         c.a = static_cast<float*>(alloc_bytes(c.n * sizeof(float), AllocKind::kDevice, device_, true));
       } else if (name == "T") {
         // n = CTAs (one 128x256 accumulator tile each); b = bf16 operands A|B; a = fp32 results.
-        // HPCP_T_OUT=P puts the accumulator tiles into the PEER GPU: the tcgen05.ld epilogue stores
+        // HPCP_T_OUT=P puts the accumulator tiles into the PEER GPU: the epilogue stores
         // straight over NVLink, i.e. tensor-core tile compute -> P2P put in one kernel.
         c.tripcount = require_param(req, "tripcount_T");
         const char* t_out = std::getenv("HPCP_T_OUT");
@@ -422,11 +422,10 @@ class CudaBackend final : public Backend {
     if (req.verbose) std::cout << "#n_queues used: 1" << std::endl;
     std::vector<FusedCommand> fused;
     std::vector<const DevCommand*> side;  // launched alongside the fused kernel, one stream each
-    // PCIe traffic driven from the SMs (zero-copy TMA / ld-st on pinned memory) reaches copy-engine
-    // speed in ONE direction (51-53 vs 55 GB/s) but not in both at once (74 vs 111 GB/s measured,
-    // profiles/r1_call4_1gpu): with two or more host copies in the group they go to the copy engines.
-    // The same holds for NVLink when one GPU drives both directions at once (put + get from the same
-    // SMs: 866 vs ~1400 GB/s with the copy engines, profiles/r1_call12_2gpu).
+    // PCIe traffic driven from the SMs (zero-copy TMA / ld-st on pinned memory) can reach copy-engine
+    // speed in ONE direction but not in both at once: with two or more host copies in the group they go
+    // to the copy engines.  The same holds for NVLink when one GPU drives both directions at once (put +
+    // get from the same SMs).
     int host_copies = 0, peer_copies = 0;
     for (const auto& c : cmds) {
       if (!c.is_copy()) continue;
@@ -449,10 +448,10 @@ class CudaBackend final : public Backend {
         f.b = c.b;
         f.c = c.c;
       } else if (c.name == "T") {
-        side.push_back(&c);  // tensor-core tile loop: its own (TMEM-allocating) kernel
+        side.push_back(&c);  // tensor-core tile loop: its own (smem-hungry) kernel
         continue;
       } else if (c.src_kind == AllocKind::kPageable || c.dst_kind == AllocKind::kPageable) {
-        side.push_back(&c);  // a kernel cannot dereference pageable host memory on x86 B200
+        side.push_back(&c);  // a kernel cannot dereference pageable host memory on x86 H100
         continue;
       } else if (host_copies_on_ce && (c.src_kind == AllocKind::kPinned || c.dst_kind == AllocKind::kPinned)) {
         side.push_back(&c);
@@ -466,7 +465,7 @@ class CudaBackend final : public Backend {
         f.dst = c.dst;
         f.src = c.src;
         // A link-bound copy needs few DMA CTAs; the SMs it does not take stay with the math
-        // (PCIe ~55 GB/s: 16 CTAs; NVLink ~700 GB/s: 64 CTAs; HBM<->HBM copies share the pool).
+        // (PCIe: 16 CTAs; NVLink: 64 CTAs; HBM<->HBM copies share the pool).
         const bool host = c.src_kind == AllocKind::kPinned || c.dst_kind == AllocKind::kPinned;
         const bool peer = c.name[0] == 'P' || c.name[1] == 'P';
         if (host) f.ctas = 16;
@@ -488,10 +487,9 @@ class CudaBackend final : public Backend {
     BenchResult res;
     res.total_us = std::numeric_limits<long>::max();
     double dev_best = std::numeric_limits<double>::max();
-    // A copy that touches pageable memory blocks its calling thread while the driver stages it, and (measured,
-    // profiles/r1_call7_1gpu: `fused | C MD` ran at the serial time) it does not reliably overlap a kernel enqueued
-    // by the SAME thread just before it.  Each side copy therefore gets its own host thread — the reference's
-    // host_threads idiom (concurency/bench_omp.cpp:67-69) for the one thing a kernel cannot do itself: x86 B200s
+    // A copy that touches pageable memory blocks its calling thread while the driver stages it, and it does not
+    // reliably overlap a kernel enqueued by the SAME thread just before it.  Each side copy therefore gets its own host thread — the reference's
+    // host_threads idiom (concurency/bench_omp.cpp:67-69) for the one thing a kernel cannot do itself: x86 H100s
     // cannot dereference pageable memory from the SMs.  HPCP_FUSED_SIDE_THREADS=0 restores the single-thread order.
     const bool side_threads = [] {
       const char* e = std::getenv("HPCP_FUSED_SIDE_THREADS");

@@ -10,7 +10,7 @@
 //     backend and the CUDA backend and the mode is a runtime choice (the
 //     reference needs one build per OpenMP mode: run_omp.sh:6-7);
 //   * commands: `C` busy-wait FMA chain (identical maths to bench.hpp:23-31),
-//     `A` stream triad/axpy tile (HBM-bound compute), `T` tcgen05 tensor tile,
+//     `A` stream triad/axpy tile (HBM-bound compute), `T` wgmma tensor tile,
 //     and copies `X2Y` with X,Y in M(alloc) D(evice) H(pinned) S(managed)
 //     P(eer GPU over NVLink — new);
 //   * byte counts are 64-bit (the reference's `unsigned bytes` overflows at

@@ -100,7 +100,7 @@ std::string usage_text(const std::string& program, const Backend& backend) {
      << "Commands (a '2' inside a token is ignored, so M2D == MD):\n"
      << "  C      compute: every work-item runs 64*tripcount_C dependent FMAs\n"
      << "  A      compute: stream triad a = b + s*c over globalsize_A elements\n"
-     << "  T      compute: tcgen05 tensor-core tile loop (CUDA backend only)\n"
+     << "  T      compute: wgmma tensor-core tile loop (CUDA backend only)\n"
      << "  X2Y    copy globalsize_XY floats from memory X to memory Y, with\n"
      << "           M  pageable host memory (malloc)\n"
      << "           H  pinned host memory\n"
@@ -208,8 +208,8 @@ Params resolve_parameters(const Options& opt) {
   auto default_of = [&](const std::string& key) -> size_t {
     if (key == "globalsize_C") return 1;
     if (key == "tripcount_C") return 40000;
-    if (key == "globalsize_T") return 148;  // one tile loop (CTA) per SM
-    if (key == "tripcount_T") return 20000; // passes over the 128x256x64 tile (4 tcgen05.mma each)
+    if (key == "globalsize_T") return 132;  // one tile loop (CTA) per SM
+    if (key == "tripcount_T") return 20000; // passes over the 128x256x64 tile (4 wgmma per warpgroup each)
     if (starts_with(key, "globalsize_")) {
       const long dm = cli.at("globalsize_default_memory");
       if (dm != -1) return static_cast<size_t>(dm);

@@ -3,7 +3,7 @@
 // Reference: sycl_omp_ze_interopt/interop_omp_ze_sycl.cpp:81-116 — ze_driver / ze_context /
 // ze_device handles are pulled out of the OpenMP interop object and wrapped into SYCL
 // objects with ownership "keep", devices sharing a ze_context grouped into one SYCL context.
-// CUDA/B200 analogue: the driver-API objects underneath the runtime — CUdevice, the primary
+// CUDA/H100 analogue: the driver-API objects underneath the runtime — CUdevice, the primary
 // CUcontext, the CUstream behind a cudaStream_t, CUdeviceptr behind a void* — are taken from
 // the runtime side and used by a driver-API component (and back), via the cached table in
 // device_table.h.  No context is ever created or destroyed here: the primary context is

@@ -4,7 +4,7 @@
 // Reference: sycl_omp_ze_interopt/interop_omp_sycl.cpp:40-75 — memory allocated and
 // written by the OpenMP runtime is read by a SYCL memcpy, and memory allocated by SYCL
 // is read by an OpenMP kernel, through `omp interop ... prefer_type("sycl")`.
-// CUDA/B200 analogue: a "foreign runtime" component (stream-ordered allocator with its
+// CUDA/H100 analogue: a "foreign runtime" component (stream-ordered allocator with its
 // own memory pool + its own non-blocking stream + its own kernels, the way an OpenMP
 // or PyTorch runtime would own them) and this suite's kernels (csrc/kernels) operate on
 // each other's allocations and stream.  The PyTorch flavour of the same demo is

@@ -1,4 +1,4 @@
-// Host-callable launchers for every sm_100a kernel in the suite.
+// Host-callable launchers for every sm_90a kernel in the suite.
 //
 // Plain C++ (no torch, no MPI): raw device pointers + a cudaStream_t.  Both
 // front ends use exactly these entry points:
@@ -31,7 +31,7 @@ struct CopyTuning {
   int unroll = 0;    // LdSt: 16-byte loads in flight per thread (1,2,4,8); 0 -> 4
   int stage_kb = 0;  // Tma: smem stage size in KiB; 0 -> 16
   int stages = 0;    // Tma: number of smem stages; 0 -> 8
-  int vec_bytes = 0; // LdSt: 16 (LDG/STG.128) or 32 (sm_100 LDG/STG.256); 0 -> 16
+  int vec_bytes = 0; // LdSt: 16 (LDG/STG.128) or 32 (two LDG/STG.128 per thread); 0 -> 16
   int blocked = 0;   // LdSt: 1 = each CTA owns one contiguous region instead of a grid-stride
   int l2_hint = 0;   // triad_put, TMA engine, EXPERIMENTAL: 1 = L2 evict_first policy on the bulk loads of b, c and
                      // the local bulk store of a (streamed once); the peer store keeps the default policy
@@ -183,7 +183,7 @@ void launch_busy_wait(float* out, size_t n_items, size_t tripcount, cudaStream_t
 
 // --------------------------------------------- tensor-core compute command ----
 // `T`: per-CTA bf16 tile D[128x256] += A[128x64] . B[256x64]^T repeated `tripcount` times with
-// tcgen05.mma (TMEM accumulator), operands fetched once by TMA.  `operands` holds A then B
+// wgmma.mma_async (register accumulator), operands fetched once by TMA.  `operands` holds A then B
 // (tc_busy_operand_bytes()), `out` receives ctas * 128 * 256 floats = tripcount * (A . B^T).
 size_t tc_busy_operand_bytes();
 size_t tc_busy_out_elems_per_cta();
@@ -193,12 +193,11 @@ void launch_tc_busy(const void* operands, float* out, int ctas, uint32_t tripcou
                     cudaStream_t stream, int cluster = 1);
 
 // ------------------------------------------------- tensor-core GEMM -> put ----
-// C[M,N] fp32 = A[M,K] . B[N,K]^T (bf16, K-major) with tcgen05/TMEM/TMA; the epilogue writes the tile to
+// C[M,N] fp32 = A[M,K] . B[N,K]^T (bf16, K-major) with wgmma/TMA; the epilogue writes the tile to
 // c_local and/or straight into c_peer over NVLink, then publishes sync.signal_flag.  M % 128 == N % 256 ==
 // K % 64 == 0.  Returns the number of CTAs launched.
 // out_bf16: C is stored as bf16 (half the NVLink bytes) instead of fp32.
-// cluster: 0 = auto (CTA pairs sharing the B tile by TMA multicast when the shape allows), 1 = off, 2 = force,
-// 3 = 2-SM UMMA (tcgen05.mma.cta_group::2, one 256x256 tile per CTA pair; opt-in).
+// cluster: 0 = auto (CTA pairs sharing the B tile by TMA multicast when the shape allows), 1 = off, 2 = force.
 // tma_epilogue (opt-in): the C tile leaves through the TMA unit (swizzled smem pieces + cp.async.bulk.tensor.2d stores)
 // instead of st.global from the epilogue warps.
 int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void* c_peer, int m, int n,

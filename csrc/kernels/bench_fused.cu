@@ -166,7 +166,7 @@ void launch_busy_wait(float* out, size_t n_items, size_t tripcount, cudaStream_t
   const int threads = static_cast<int>(std::min<size_t>(std::max<size_t>(n_items, 1), 128));
   const unsigned ctas = static_cast<unsigned>((std::max<size_t>(n_items, 1) + threads - 1) / threads);
   // Keep the SM's shared-memory carveout at its maximum even though this kernel uses none: a
-  // smem-hungry kernel launched while `C` is running (TMA copies, the tcgen05 tile loop) must be
+  // smem-hungry kernel launched while `C` is running (TMA copies, the wgmma tile loop) must be
   // able to co-reside on the same SM, which is the whole point of the benchmark.
   static const cudaError_t carveout_once = cudaFuncSetAttribute(
       busy_wait_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);

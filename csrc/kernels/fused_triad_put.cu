@@ -56,7 +56,7 @@ __device__ __forceinline__ void cta_epilogue(const SyncOps& sync, const uint32_t
 }
 
 // ------------------------------------------------------------ LdSt engine ----
-// V = uint4 (4 floats, LDG/STG.128) or ptx::U32x8 (8 floats, LDG/STG.256).
+// V = uint4 (4 floats, LDG/STG.128) or ptx::U32x8 (8 floats, two LDG/STG.128).
 __device__ __forceinline__ uint4 ld_in(const uint4* p) { return ptx::ld_stream_v4(p); }
 __device__ __forceinline__ ptx::U32x8 ld_in(const ptx::U32x8* p) { return ptx::ld_stream_v8(p); }
 __device__ __forceinline__ void st_out(uint4* p, const uint4& v) { ptx::st_stream_v4(p, v); }
@@ -412,7 +412,7 @@ int launch_triad_put(const TriadPutArgs& args, CopyEngine engine, const CopyTuni
 
 void launch_fill_triad_inputs(float* b, float* c, size_t n, int rank, cudaStream_t stream) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((n + threads - 1) / threads, 148 * 8));
+  const int ctas = static_cast<int>(std::min<size_t>((n + threads - 1) / threads, 132 * 8));
   fill_triad_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(b, c, n, rank);
   HPCP_CUDA(cudaGetLastError());
 }
@@ -420,7 +420,7 @@ void launch_fill_triad_inputs(float* b, float* c, size_t n, int rank, cudaStream
 void launch_verify_triad(const float* a, size_t n, int src_rank, float s,
                          unsigned long long* mismatch_count, cudaStream_t stream) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((n + threads - 1) / threads, 148 * 8));
+  const int ctas = static_cast<int>(std::min<size_t>((n + threads - 1) / threads, 132 * 8));
   verify_triad_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(a, n, src_rank, s,
                                                                 mismatch_count);
   HPCP_CUDA(cudaGetLastError());

@@ -24,9 +24,9 @@
 //                            the transfer of block i+1 hides behind the math of block i.  Stock pattern:
 //                            ncclAllGather, then cuBLAS GEMM.
 //
-// Both kernels are policies of the suite's persistent tcgen05 tile loop (umma.cuh: gemm_persistent — TMA ring,
-// tcgen05.mma into double-buffered TMEM accumulators, tcgen05.ld epilogue, optional CTA pairs with TMA multicast
-// of the B tile).  Nothing in the reference is GEMM-shaped (SURVEY.md §2.4); its one collective is the ring
+// Both kernels are policies of the suite's persistent wgmma tile loop (wgmma.cuh: gemm_persistent — TMA ring,
+// wgmma.mma_async into register accumulators of two consumer warpgroups, epilogue straight from the registers,
+// optional CTA pairs with TMA multicast of the B tile).  Nothing in the reference is GEMM-shaped; its one collective is the ring
 // allreduce (allreduce-mpi-sycl.cpp:43-67), whose fused form here is K-ring.  These two kernels are what that
 // "compute step followed by a collective" idea looks like when the compute step runs on the tensor cores.
 //
@@ -41,7 +41,7 @@
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hpcp {
 
@@ -85,18 +85,20 @@ struct ReduceScatterPolicy {
     shard_coords(tile, g.rank, g.world, 1, g.shard_tiles_m, g.tiles_n, m_blk, n_blk);
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
     const int owner = (m0 / kBM) / g.shard_tiles_m;
-    const int row0 = m0 - owner * g.shard_tiles_m * kBM + ew * 32;  // first of this warp's rows inside the shard
+    const int row0 = m0 - owner * g.shard_tiles_m * kBM + ew * kEpiRows;  // first of this warp's rows inside the shard
     const size_t elem = g.out_bf16 ? 2 : 4;
     unsigned char* base = g.shard[owner] + (static_cast<size_t>(row0) * g.n + n0) * elem;
     const size_t ld = static_cast<size_t>(g.n) * elem;
+    float* stage_buf = epi_stage_buf(epi_smem, ew);
     if (g.out_bf16)
-      epilogue_segments(true, taddr, stage_buf, lane, [&](int row, int col, int byte, const uint4& v) {
+      epilogue_segments(true, d, stage_buf, lane, [&](int row, int col, int byte, const uint4& v) {
         ptx::red_add_bf16x8_sys(base + row * ld + col * 2 + byte, v);
       });
     else
-      epilogue_segments(false, taddr, stage_buf, lane, [&](int row, int col, int byte, const uint4& v) {
+      epilogue_segments(false, d, stage_buf, lane, [&](int row, int col, int byte, const uint4& v) {
         ptx::red_add_f32x4_sys(reinterpret_cast<float*>(base + row * ld + col * 4 + byte),
                                make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z),
                                            __uint_as_float(v.w)));
@@ -109,13 +111,13 @@ struct ReduceScatterPolicy {
   }
 };
 
-// Reduce-scatter with the TMA unit doing the additions' issue: an epilogue warp writes a [32 rows x 32 columns] fp32
-// piece of its accumulator rows into a dense, 128-byte-swizzled smem tile (lane = row; the 16-byte chunk c of row r
-// goes to chunk c ^ (r % 8): conflict-free for both the writer and the TMA), and ONE cp.reduce.async.bulk.tensor.2d
-// adds the 4 KiB tile into the owner's shard (UTMAREDG.2D.ADD) — 8 instructions per 128x256 accumulator and warp
-// instead of 2048 REDG requests through the LSU (umma.cuh: epilogue_tma_tiles).
+// Reduce-scatter with the TMA unit doing the additions' issue: a consumer warp writes a [16 rows x 32 columns] fp32
+// piece of its accumulator rows into a dense, 128-byte-swizzled smem tile (the 16-byte chunk c of row r goes to
+// chunk c ^ (r % 8), the layout the TMA reads), and ONE cp.reduce.async.bulk.tensor.2d adds the 2 KiB tile into the
+// owner's shard (UTMAREDG.2D.ADD) — 8 instructions per warp and tile instead of 1024 REDG requests through the LSU
+// (wgmma.cuh: epilogue_tma_tiles).
 struct RsMaps {
-  CUtensorMap shard[kApiMaxRanks];  // fp32 [M/P, N] of every owner, box 32 x 32, SWIZZLE_128B
+  CUtensorMap shard[kApiMaxRanks];  // fp32 [M/P, N] of every owner, box 16 x 32, SWIZZLE_128B
 };
 struct ReduceScatterTmaPolicy {
   static constexpr bool kHasAuxWarp = false;
@@ -125,11 +127,12 @@ struct ReduceScatterTmaPolicy {
     shard_coords(tile, g.rank, g.world, 1, g.shard_tiles_m, g.tiles_n, m_blk, n_blk);
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
     const int owner = (m0 / kBM) / g.shard_tiles_m;
-    const int y = m0 - owner * g.shard_tiles_m * kBM + ew * 32;  // first of this warp's rows inside the shard
+    const int y = m0 - owner * g.shard_tiles_m * kBM + ew * kEpiRows;  // first of this warp's rows inside the shard
     const CUtensorMap* map = &maps.shard[owner];
-    epilogue_tma_tiles(false, taddr, stage_buf, ew, lane,
+    epilogue_tma_tiles(false, d, epi_smem, ew, lane,
                        [&](const unsigned char* tile, int col) { tma_reduce_add_2d(map, n0 + col, y, tile); });
   }
   __device__ __forceinline__ void aux_warp(int, unsigned char*) const {}
@@ -161,10 +164,11 @@ struct AllReducePolicy {
     tile_coords(t, g.tiles_m, g.tiles_n, m_blk, n_blk);
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
-    float* base = g.c_multicast + static_cast<size_t>(m0 + ew * 32) * g.n + n0;
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
+    float* base = g.c_multicast + static_cast<size_t>(m0 + ew * kEpiRows) * g.n + n0;
     const size_t ld = static_cast<size_t>(g.n);
-    epilogue_segments(false, taddr, stage_buf, lane, [&](int row, int col, int byte, const uint4& v) {
+    epilogue_segments(false, d, epi_stage_buf(epi_smem, ew), lane, [&](int row, int col, int byte, const uint4& v) {
       ptx::multimem_red_add_f32x4(base + row * ld + col + byte / 4,
                                   make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z),
                                               __uint_as_float(v.w)));
@@ -219,12 +223,13 @@ struct AllToAllPolicy {
     shard_coords(tile, g.rank, g.world, 1, g.shard_tiles_m, g.tiles_n, m_blk, n_blk);  // the neighbour's rows first
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
     const int owner = (m0 / kBM) / g.shard_tiles_m;
     const size_t shard_rows = static_cast<size_t>(g.shard_tiles_m) * kBM;
     const size_t elem = g.out_bf16 ? 2 : 4;
     const Out out{nullptr, g.recv[owner] + static_cast<size_t>(g.rank) * shard_rows * g.n * elem, g.out_bf16, g.n};
-    epilogue_store_tile(out, taddr, stage_buf, m0 - owner * static_cast<int>(shard_rows), n0, ew, lane);
+    epilogue_store_tile(out, d, epi_stage_buf(epi_smem, ew), m0 - owner * static_cast<int>(shard_rows), n0, ew, lane);
   }
   __device__ __forceinline__ void aux_warp(int, unsigned char*) const {}
   __device__ __forceinline__ void finish() const {
@@ -238,13 +243,6 @@ __global__ void __launch_bounds__(kThreads, 1)
     gemm_all_to_all_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                            const __grid_constant__ A2aDev g) {
   gemm_persistent<kCluster, kStages>(map_a, map_b, g.tiles_m, g.tiles_n, g.k, AllToAllPolicy{g});
-}
-
-// cluster = 3: the same policy on the 2-SM UMMA tile loop (tcgen05.mma.cta_group::2, one 256x256 tile per CTA pair).
-__global__ void __launch_bounds__(kThreads, 1)
-    gemm_reduce_scatter_2sm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                                   const __grid_constant__ RsDev g) {
-  gemm_persistent_2sm(map_a, map_b, g.tiles_m, g.tiles_n, g.k, ReduceScatterPolicy{g});
 }
 
 // ------------------------------------------------------------------ all-gather -> GEMM ----
@@ -289,28 +287,31 @@ struct AllGatherPolicy {
       __syncwarp();
     }
   }
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
+    float* stage_buf = epi_stage_buf(epi_smem, ew);
     if (g.activation == 0) {
-      epilogue_store_tile(g, taddr, stage_buf, m0, n0, ew, lane);
+      epilogue_store_tile(g, d, stage_buf, m0, n0, ew, lane);
       return;
     }
     // Fused activation (the layer's nonlinearity never costs a pass over C in HBM).
     const size_t elem = g.out_bf16 ? 2 : 4;
-    unsigned char* base = static_cast<unsigned char*>(g.c_local) + (static_cast<size_t>(m0 + ew * 32) * g.n + n0) * elem;
+    unsigned char* base =
+        static_cast<unsigned char*>(g.c_local) + (static_cast<size_t>(m0 + ew * kEpiRows) * g.n + n0) * elem;
     const size_t ld = static_cast<size_t>(g.n) * elem;
     auto store = [&](int row, int col, int byte, const uint4& v) {
       *reinterpret_cast<uint4*>(base + row * ld + col * elem + byte) = v;
     };
     if (g.activation == 1)
-      epilogue_segments(g.out_bf16 != 0, taddr, stage_buf, lane, store, [](float x) { return fmaxf(x, 0.0f); });
+      epilogue_segments(g.out_bf16 != 0, d, stage_buf, lane, store, [](float x) { return fmaxf(x, 0.0f); });
     else if (g.activation == 2)
-      epilogue_segments(g.out_bf16 != 0, taddr, stage_buf, lane, store, [](float x) {
+      epilogue_segments(g.out_bf16 != 0, d, stage_buf, lane, store, [](float x) {
         float t;  // gelu, tanh form: 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))
         asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.7978845608f * (x + 0.044715f * x * x * x)));
         return 0.5f * x * (1.0f + t);
       });
     else
-      epilogue_segments(g.out_bf16 != 0, taddr, stage_buf, lane, store,
+      epilogue_segments(g.out_bf16 != 0, d, stage_buf, lane, store,
                         [](float x) { return __fdividef(x, 1.0f + __expf(-x)); });  // silu
   }
   // Gather engine: one thread per CTA streams its share of the peers' row blocks, peer (rank+1) first — the
@@ -374,12 +375,6 @@ __global__ void __launch_bounds__(kThreads, 1)
     allgather_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                           const __grid_constant__ AgDev g) {
   gemm_persistent<kCluster, kStages>(map_a, map_b, g.tiles_m, g.tiles_n, g.k, AllGatherPolicy{g});
-}
-
-__global__ void __launch_bounds__(kThreads, 1)
-    allgather_gemm_2sm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                              const __grid_constant__ AgDev g) {
-  gemm_persistent_2sm(map_a, map_b, g.tiles_m, g.tiles_n, g.k, AllGatherPolicy{g});
 }
 
 // ------------------------------------------------------------------ wait for P flags ----
@@ -457,15 +452,13 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
 int launch_gemm_reduce_scatter(const GemmRsArgs& args, int ctas, int device, cudaStream_t stream, int cluster) {
   const Shape s = check_shape("gemm_reduce_scatter", args.m, args.n, args.k, args.world);
   HPCP_REQUIRE(args.rank >= 0 && args.rank < args.world, "gemm_reduce_scatter: bad rank");
-  HPCP_REQUIRE(cluster >= 0 && cluster <= 3, "gemm_reduce_scatter: cluster must be 0 (auto), 1, 2 or 3 (2-SM UMMA)");
-  HPCP_REQUIRE(cluster < 2 || s.pairable, "gemm_reduce_scatter: cluster=2/3 needs an even number of tile rows per shard");
+  HPCP_REQUIRE(cluster >= 0 && cluster <= 2, "gemm_reduce_scatter: cluster must be 0 (auto), 1 or 2");
   HPCP_REQUIRE((reinterpret_cast<uintptr_t>(args.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(args.b) & 15) == 0,
                "gemm_reduce_scatter: operands must be 16-byte aligned");
   RsDev g{};
   const bool all_reduce = args.c_multicast != nullptr;
   HPCP_REQUIRE(!all_reduce || (reinterpret_cast<uintptr_t>(args.c_multicast) & 15) == 0,
                "gemm_reduce_scatter: the multicast mapping must be 16-byte aligned");
-  HPCP_REQUIRE(!all_reduce || cluster != 3, "gemm_reduce_scatter: the all-reduce flavour has no 2-SM variant yet");
   g.c_multicast = args.c_multicast;
   HPCP_REQUIRE(!all_reduce || !args.out_bf16, "gemm_reduce_scatter: the all-reduce flavour accumulates in fp32");
   g.out_bf16 = args.out_bf16 ? 1 : 0;
@@ -496,8 +489,7 @@ int launch_gemm_reduce_scatter(const GemmRsArgs& args, int ctas, int device, cud
   int grid = std::min(tiles, ctas > 0 ? ctas : device_sm_count(device));
   constexpr size_t smem = gemm_smem_bytes<kStages>(0);
   if (args.tma_epilogue) {  // additions issued by the TMA unit (UTMAREDG) instead of REDG requests from the LSU
-    HPCP_REQUIRE(!all_reduce && !args.out_bf16 && cluster != 3,
-                 "gemm_reduce_scatter: the TMA epilogue exists for fp32 shards and cluster 0/1/2");
+    HPCP_REQUIRE(!all_reduce && !args.out_bf16, "gemm_reduce_scatter: the TMA epilogue exists for fp32 shards");
     RsMaps maps{};
     for (int q = 0; q < args.world; ++q) maps.shard[q] = make_c_tile_map(args.shard[q], args.m / args.world, args.n, false);
     constexpr size_t smem_t = gemm_smem_bytes<kStages>(kTmaEpiSmemBytes - kEpiWarps * kEpiWarpBytes);
@@ -508,11 +500,6 @@ int launch_gemm_reduce_scatter(const GemmRsArgs& args, int ctas, int device, cud
   if (all_reduce)
     return launch_tile_loop(gemm_allreduce_kernel<1>, gemm_allreduce_kernel<2>, pairs, grid, smem, smem, stream, map_a,
                             args.b, args.n, args.k, g);
-  if (cluster == 3) {
-    HPCP_REQUIRE(grid >= 2, "gemm_reduce_scatter: cluster=3 needs at least two CTAs");
-    return launch_tile_loop(gemm_reduce_scatter_kernel<1>, gemm_reduce_scatter_2sm_kernel, true, grid, smem,
-                            gemm_2sm_smem_bytes(0), stream, map_a, args.b, args.n, args.k, g);
-  }
   return launch_tile_loop(gemm_reduce_scatter_kernel<1>, gemm_reduce_scatter_kernel<2>, pairs, grid, smem, smem, stream,
                           map_a, args.b, args.n, args.k, g);
 }
@@ -559,8 +546,8 @@ uint32_t allgather_gemm_chunks_per_block(int k, int chunk_bytes) {
 int launch_allgather_gemm(const AgGemmArgs& args, int ctas, int device, cudaStream_t stream, int cluster) {
   const Shape s = check_shape("allgather_gemm", args.m, args.n, args.k, args.world);
   HPCP_REQUIRE(args.rank >= 0 && args.rank < args.world, "allgather_gemm: bad rank");
-  HPCP_REQUIRE(cluster >= 0 && cluster <= 3, "allgather_gemm: cluster must be 0 (auto), 1, 2 or 3 (2-SM UMMA)");
-  HPCP_REQUIRE(cluster < 2 || s.pairable, "allgather_gemm: cluster=2/3 needs an even number of tile rows per shard");
+  HPCP_REQUIRE(cluster >= 0 && cluster <= 2, "allgather_gemm: cluster must be 0 (auto), 1 or 2");
+  HPCP_REQUIRE(cluster != 2 || s.pairable, "allgather_gemm: cluster=2 needs an even number of tile rows per shard");
   HPCP_REQUIRE(args.a_full != nullptr && args.b != nullptr && args.c != nullptr, "allgather_gemm: null operand");
   HPCP_REQUIRE((reinterpret_cast<uintptr_t>(args.a_full) & 127) == 0 && (reinterpret_cast<uintptr_t>(args.b) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(args.c) & 15) == 0,
@@ -609,12 +596,24 @@ int launch_allgather_gemm(const AgGemmArgs& args, int ctas, int device, cudaStre
   constexpr size_t smem = gemm_smem_bytes<kStages>(kGatherSmemBytes);
   static_assert(smem + 1024 <= 227 * 1024,  // + the static barriers, padded to the 1 KiB alignment of the ring
                 "GEMM stages + epilogue staging + gather ring must fit in 227 KiB");
-  if (cluster == 3) {
-    HPCP_REQUIRE(grid >= 2, "allgather_gemm: cluster=3 needs at least two CTAs");
-    constexpr size_t smem2 = gemm_2sm_smem_bytes(kGatherSmemBytes);
-    static_assert(smem2 + 1024 <= 227 * 1024, "2-SM stages + epilogue staging + gather ring must fit in 227 KiB");
-    return launch_tile_loop(allgather_gemm_kernel<1>, allgather_gemm_2sm_kernel, true, grid, smem, smem2, stream, map_a,
-                            args.b, args.n, args.k, g);
+  if (pairs && grid >= 2) {
+    // Not every SM can host half of a CTA pair (a GPC may have an SM left over): never more pairs than fit at once.
+    HPCP_ENABLE_SMEM(allgather_gemm_kernel<2>, smem);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid & ~1));
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    HPCP_CUDA(cudaOccupancyMaxActiveClusters(&clusters, allgather_gemm_kernel<2>, &cfg));
+    HPCP_REQUIRE(clusters >= 1, "allgather_gemm: no CTA pair fits on this device");
+    grid = std::min(grid, 2 * clusters);
   }
   return launch_tile_loop(allgather_gemm_kernel<1>, allgather_gemm_kernel<2>, pairs, grid, smem, smem, stream, map_a,
                           args.b, args.n, args.k, g);

@@ -1,24 +1,21 @@
-// K-gemm-put: bf16 GEMM on the 5th-gen tensor cores whose epilogue PUTs the result tile into a
+// K-gemm-put: bf16 GEMM on the Hopper tensor cores (wgmma) whose epilogue PUTs the result tile into a
 // peer GPU over NVLink — "compute step followed by a transfer" as ONE kernel.
 //
 //     C[M,N] (fp32) = A[M,K] (bf16, K-major) . B[N,K]^T (bf16, K-major)
 //     C is written to c_local and/or to c_peer (a peer-mapped pointer), then the arrival epoch is
 //     published on the peer (same release/acquire protocol as every other kernel of the suite).
 //
-// Nothing in the reference is GEMM-shaped (SURVEY.md §2.4); this kernel is the tensor-core member of
+// Nothing in the reference is GEMM-shaped; this kernel is the tensor-core member of
 // the suite's "fuse the transfer into the producing kernel" family, next to K-fused-triad-put
 // (stream triad -> put) and K-ring (accumulate -> forward).  Stock comparison: cuBLAS GEMM followed
 // by cudaMemcpyPeerAsync (two operations, the C tile goes to HBM and is read back before it moves).
 //
-// Structure (persistent, one CTA per SM, 256 threads, canonical Blackwell warp specialisation):
-//   warp 0      TMA producer  : cp.async.bulk.tensor.2d (SWIZZLE_128B) A[128x64] + B[256x64] per stage,
-//                               4-stage smem ring, full/empty mbarriers
-//   warp 1      MMA issuer    : one elected thread, tcgen05.mma.cta_group::1.kind::f16 (M128 N256 K16),
-//                               tcgen05.commit frees the smem stage / publishes the accumulator
-//   warp 2      TMEM allocator: 512 columns = two 128x256 fp32 accumulators (epilogue of tile i overlaps
-//                               the main loop of tile i+1)
-//   warps 4..7  epilogue      : tcgen05.ld 32x32b.x32 -> padded smem transpose -> 128-byte row segments
-//                               -> st.global to c_local and/or the peer (coalesced NVLink stores)
+// Structure (persistent, one CTA per SM, 384 threads, wgmma.cuh: gemm_persistent):
+//   warp 0          TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B) A[128x64] + B[256x64] per stage,
+//                                  4-stage smem ring, full/empty mbarriers
+//   warpgroups 1,2  consumers    : wgmma.mma_async m64n256k16 (64 rows each), fp32 accumulators in registers;
+//                                  epilogue: registers -> padded smem staging -> 128-byte row segments
+//                                  -> st.global to c_local and/or the peer (coalesced NVLink stores)
 #include "api.h"
 
 #include <cuda.h>
@@ -32,17 +29,16 @@
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hpcp {
 
 namespace {
 
-using namespace umma;  // tile geometry, descriptors, TMA / tcgen05 wrappers, rasterisation, tensor-map encoder
+using namespace umma;  // tile geometry, descriptors, TMA / wgmma wrappers, rasterisation, tensor-map encoder
 
 constexpr int kStages = 4;
-constexpr uint32_t kStageBytes = kABytes + kBBytes;     // 48 KiB
-constexpr size_t kSmemBytes = static_cast<size_t>(kStages) * kStageBytes + kEpiWarps * kEpiWarpBytes + 1024;
+constexpr size_t kSmemBytes = gemm_smem_bytes<kStages>(0);
 
 struct GemmDev {
   void* c_local;    // may be null; fp32 [M,N], or bf16 [M,N] when out_bf16
@@ -53,7 +49,7 @@ struct GemmDev {
   SyncOps sync;
 };
 
-// The kernel is the suite's persistent tile loop (umma.cuh: gemm_persistent) with this policy: grouped
+// The kernel is the suite's persistent tile loop (wgmma.cuh: gemm_persistent) with this policy: grouped
 // rasterisation over the whole C, stores (local and/or peer) in the epilogue, one arrival epoch at the end.
 struct PutPolicy {
   static constexpr bool kHasAuxWarp = false;
@@ -62,8 +58,9 @@ struct PutPolicy {
     tile_coords(tile, g.tiles_m, g.tiles_n, m_blk, n_blk);
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
-    epilogue_store_tile(g, taddr, stage_buf, m0, n0, ew, lane);
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
+    epilogue_store_tile(g, d, epi_stage_buf(epi_smem, ew), m0, n0, ew, lane);
   }
   __device__ __forceinline__ void aux_warp(int, unsigned char*) const {}
   // Put epilogue: the last CTA publishes the arrival epoch on the peer.
@@ -73,216 +70,13 @@ struct PutPolicy {
   }
 };
 
-// The default kernel is kept in the exact source form that ran on the B200 boxes (round 1, GPU calls 9-18): the tile
-// loop written out, not the policy template.  The template (umma.cuh: gemm_persistent) is the same loop with the
-// hooks factored out and every later variant uses it, but it does not compile to byte-identical SASS (register
-// allocation differs), and the contract for refactors around GPU-validated kernels is "not one instruction changes"
-// (docs/sass/VALIDATED.sha256, scripts/sass_fingerprint.py).  PutPolicy above is what the 2-SM kernel instantiates the
-// template with.
-// kCluster == 2: thread-block clusters of two CTAs working on vertically adjacent tiles (same n_blk).
-// Both need the same B tile, so each CTA fetches half of it (128 rows) and TMA-multicasts it into both
-// CTAs' shared memory: L2->SM operand traffic drops from 48 to 32 KiB per CTA per k-block.  A stage
-// may only be refilled when BOTH CTAs' MMAs have consumed it: the empty barriers count 2 arrivals and
-// every tcgen05.commit is multicast to the pair.
+// kCluster == 2: thread-block clusters of two CTAs working on vertically adjacent tiles that share the B tile
+// (wgmma.cuh: gemm_persistent).
 template <int kCluster>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_put_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                     const __grid_constant__ GemmDev g) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[kStages];
-  __shared__ __align__(8) uint64_t empty_bar[kStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_s;
-
-  unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* epi_smem = smem + static_cast<size_t>(kStages) * kStageBytes;
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = g.tiles_m * g.tiles_n;
-  const int num_kb = g.k / kBK;
-  const int crank = kCluster > 1 ? static_cast<int>(cluster_cta_rank()) : 0;
-  // Work items are tile pairs in cluster mode: pair p -> tiles 2p, 2p+1 (consecutive tiles of the
-  // grouped rasterisation share n_blk when the group height is even).
-  const int first_item = static_cast<int>(blockIdx.x) / kCluster;
-  const int item_stride = static_cast<int>(gridDim.x) / kCluster;
-  const int num_items = num_tiles / kCluster;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    for (int s = 0; s < kStages; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], kCluster);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], kEpiWarps);
-    }
-    ptx::fence_mbar_init();
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     ptx::smem_u32(&tmem_base_s)),
-                 "r"(static_cast<uint32_t>(kTmemCols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  if (kCluster > 1) cluster_sync_all();  // the peer's barriers exist before anything remote touches them
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    // The whole warp walks the loop (convergent barriers at kernel end); lane 0 issues the TMA.
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int item = first_item; item < num_items; item += item_stride) {
-      const int tile = item * kCluster + crank;
-      int m_blk, n_blk;
-      tile_coords(tile, g.tiles_m, g.tiles_n, &m_blk, &n_blk);
-      const int m0 = m_blk * kBM;
-      const int n0 = n_blk * kBN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(&empty_bar[stage], phase ^ 1);  // slot released by the MMA warp(s)
-        if (lane == 0) {
-          unsigned char* sa = smem + static_cast<size_t>(stage) * kStageBytes;
-          ptx::mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(sa, &map_a, kb * kBK, m0, &full_bar[stage]);
-          if (kCluster > 1)  // my half of the shared B tile, delivered to both CTAs of the pair
-            tma_load_2d_multicast(sa + kABytes + crank * (kBBytes / 2), &map_b, kb * kBK,
-                                  n0 + crank * (kBN / 2), &full_bar[stage], static_cast<uint16_t>(0x3));
-          else
-            tma_load_2d(sa + kABytes, &map_b, kb * kBK, n0, &full_bar[stage]);
-        }
-        __syncwarp();
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc(kBM, kBN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int local_tile = 0;
-    for (int item = first_item; item < num_items; item += item_stride, ++local_tile) {
-      const int acc = local_tile & 1;
-      const uint32_t acc_phase = static_cast<uint32_t>(local_tile >> 1) & 1;
-      ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);  // epilogue drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * kBN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase);  // TMA bytes landed
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = ptx::smem_u32(smem + static_cast<size_t>(stage) * kStageBytes);
-          const uint64_t desc_a = make_smem_desc(sa);
-          const uint64_t desc_b = make_smem_desc(sa + kABytes);
-#pragma unroll
-          for (int k = 0; k < kBK / kUmmaK; ++k) {
-            const uint64_t adv = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16(tmem_d, desc_a + adv, desc_b + adv, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          if (kCluster > 1)
-            umma_commit_multicast(&empty_bar[stage], static_cast<uint16_t>(0x3));  // frees the slot in both CTAs
-          else
-            umma_commit(&empty_bar[stage]);                            // frees the smem slot
-          if (kb == num_kb - 1) umma_commit(&tmem_full_bar[acc]);      // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int ew = warp - 4;            // 0..3 == warp % 4 -> TMEM lane group
-    float* stage_buf = reinterpret_cast<float*>(epi_smem + static_cast<size_t>(ew) * kEpiWarpBytes);
-    int local_tile = 0;
-    for (int item = first_item; item < num_items; item += item_stride, ++local_tile) {
-      const int tile = item * kCluster + crank;
-      const int acc = local_tile & 1;
-      const uint32_t acc_phase = static_cast<uint32_t>(local_tile >> 1) & 1;
-      int m_blk, n_blk;
-      tile_coords(tile, g.tiles_m, g.tiles_n, &m_blk, &n_blk);
-      const int m0 = m_blk * kBM;
-      const int n0 = n_blk * kBN;
-      ptx::mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + static_cast<uint32_t>(acc * kBN) + (static_cast<uint32_t>(ew * 32) << 16);
-      // One round moves a 128-byte row segment per accumulator row: 32 fp32 columns, or 64 bf16
-      // columns (two TMEM loads, converted before staging), so the NVLink / HBM stores below are
-      // always full 128-byte segments.
-      const int cols_per_round = g.out_bf16 ? 64 : 32;
-      const size_t elem = g.out_bf16 ? 2 : 4;
-      unsigned char* stage_row = reinterpret_cast<unsigned char*>(stage_buf) + lane * (kStageRowWords * 4);
-      for (int col = 0; col < kBN; col += cols_per_round) {
-        if (g.out_bf16) {
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t r[32];
-            tmem_ld_32x32b_x32(taddr + col + half * 32, r);
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              uint4 pk;
-              __nv_bfloat162 t;
-              t = __floats2bfloat162_rn(__uint_as_float(r[j]), __uint_as_float(r[j + 1]));
-              pk.x = *reinterpret_cast<uint32_t*>(&t);
-              t = __floats2bfloat162_rn(__uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-              pk.y = *reinterpret_cast<uint32_t*>(&t);
-              t = __floats2bfloat162_rn(__uint_as_float(r[j + 4]), __uint_as_float(r[j + 5]));
-              pk.z = *reinterpret_cast<uint32_t*>(&t);
-              t = __floats2bfloat162_rn(__uint_as_float(r[j + 6]), __uint_as_float(r[j + 7]));
-              pk.w = *reinterpret_cast<uint32_t*>(&t);
-              *reinterpret_cast<uint4*>(stage_row + half * 64 + j * 2) = pk;
-            }
-          }
-        } else {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr + col, r);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<uint4*>(stage_row + j * 4) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-        }
-        __syncwarp();
-        // 8 lanes x 16 B per row, 4 rows per instruction.
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int row = it * 4 + (lane >> 3);
-          const int c16 = lane & 7;
-          const uint4 v = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(stage_buf) +
-                                                          row * (kStageRowWords * 4) + c16 * 16);
-          const size_t off = (static_cast<size_t>(m0 + ew * 32 + row) * g.n + n0 + col) * elem + c16 * 16;
-          if (g.c_peer != nullptr)
-            ptx::st_stream_v4(reinterpret_cast<uint4*>(static_cast<unsigned char*>(g.c_peer) + off), v);
-          if (g.c_local != nullptr)
-            *reinterpret_cast<uint4*>(static_cast<unsigned char*>(g.c_local) + off) = v;
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);  // accumulator may be overwritten
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(kTmemCols))
-                 : "memory");
-  // A CTA of a pair must not retire while its partner can still multicast into it.
-  if (kCluster > 1) cluster_sync_all();
-  // Put epilogue: the last CTA publishes the arrival epoch on the peer.
-  if (g.sync.ticket != nullptr)
-    last_cta_publish(g.sync.ticket, g.sync.ticket_base + gridDim.x, g.sync.signal_flag, g.sync.signal_epoch);
+  gemm_persistent<kCluster, kStages>(map_a, map_b, g.tiles_m, g.tiles_n, g.k, PutPolicy{g});
 }
 
 // Alternative epilogue (opt-in, `tma_epilogue`): the C tile leaves through the TMA unit — swizzled [32 x 128 B]
@@ -300,10 +94,11 @@ struct PutTmaPolicy {
     tile_coords(tile, g.tiles_m, g.tiles_n, m_blk, n_blk);
   }
   __device__ __forceinline__ void a_rows_ready(int) const {}
-  __device__ __forceinline__ void epilogue(uint32_t taddr, float* stage_buf, int m0, int n0, int ew, int lane) const {
-    epilogue_tma_tiles(g.out_bf16 != 0, taddr, stage_buf, ew, lane, [&](const unsigned char* tile, int col) {
-      if (g.c_peer != nullptr) tma_store_2d(&maps.c_peer, n0 + col, m0 + ew * 32, tile);
-      if (g.c_local != nullptr) tma_store_2d(&maps.c_local, n0 + col, m0 + ew * 32, tile);
+  __device__ __forceinline__ void epilogue(const float (&d)[kAccRegs], unsigned char* epi_smem, int m0, int n0, int ew,
+                                           int lane) const {
+    epilogue_tma_tiles(g.out_bf16 != 0, d, epi_smem, ew, lane, [&](const unsigned char* tile, int col) {
+      if (g.c_peer != nullptr) tma_store_2d(&maps.c_peer, n0 + col, m0 + ew * kEpiRows, tile);
+      if (g.c_local != nullptr) tma_store_2d(&maps.c_local, n0 + col, m0 + ew * kEpiRows, tile);
     });
   }
   __device__ __forceinline__ void aux_warp(int, unsigned char*) const {}
@@ -321,19 +116,6 @@ __global__ void __launch_bounds__(kThreads, 1)
   gemm_persistent<kCluster, kStages>(map_a, map_b, g.tiles_m, g.tiles_n, g.k, PutTmaPolicy{g, maps});
 }
 
-__global__ void __launch_bounds__(kThreads, 1)
-    gemm_put_2sm_tma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                            const __grid_constant__ GemmDev g, const __grid_constant__ PutMaps maps) {
-  gemm_persistent_2sm(map_a, map_b, g.tiles_m, g.tiles_n, g.k, PutTmaPolicy{g, maps});
-}
-
-// 2-SM UMMA variant (tcgen05.mma.cta_group::2): the same policy on umma.cuh's gemm_persistent_2sm.
-__global__ void __launch_bounds__(kThreads, 1)
-    gemm_put_2sm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                        const __grid_constant__ GemmDev g) {
-  gemm_persistent_2sm(map_a, map_b, g.tiles_m, g.tiles_n, g.k, PutPolicy{g});
-}
-
 }  // namespace
 
 int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void* c_peer, int m, int n,
@@ -347,11 +129,10 @@ int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void*
                "gemm_put: pointers must be 16-byte aligned");
   HPCP_REQUIRE(sync.signal_flag == nullptr || sync.ticket != nullptr, "gemm_put: a signal needs a ticket counter");
   // Cluster mode needs an even number of tile rows per raster group (pairs share n_blk).
-  HPCP_REQUIRE(cluster >= 0 && cluster <= 3, "gemm_put: cluster must be 0 (auto), 1, 2 or 3 (2-SM UMMA)");
+  HPCP_REQUIRE(cluster >= 0 && cluster <= 2, "gemm_put: cluster must be 0 (auto), 1 or 2");
   const bool pairable = (m / kBM) % 2 == 0 && ((m / kBM) % kGroupM) % 2 == 0;
-  HPCP_REQUIRE(cluster < 2 || pairable, "gemm_put: cluster=2/3 needs an even number of 128-row tiles per raster group");
+  HPCP_REQUIRE(cluster != 2 || pairable, "gemm_put: cluster=2 needs an even number of 128-row tiles per raster group");
   const bool use_cluster = cluster != 1 && pairable;
-  const bool two_sm = cluster == 3;
   const CUtensorMap map_a = make_kmajor_map(a_bf16, m, k, kBM);
   const CUtensorMap map_b = make_kmajor_map(b_bf16, n, k, use_cluster ? kBN / 2 : kBN);
   GemmDev g{};
@@ -381,16 +162,11 @@ int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void*
       return grid;
     }
     grid &= ~1;
-    constexpr size_t smem_t2 = gemm_2sm_smem_bytes(kTmaEpiSmemBytes - kEpiWarps * kEpiWarpBytes);
-    static_assert(smem_t2 + 1024 <= 227 * 1024, "2-SM stages + two store tiles per epilogue warp must fit in 227 KiB");
-    if (two_sm)
-      HPCP_ENABLE_SMEM(gemm_put_2sm_tma_kernel, smem_t2);
-    else
-      HPCP_ENABLE_SMEM(gemm_put_tma_kernel<2>, smem_t);
+    HPCP_ENABLE_SMEM(gemm_put_tma_kernel<2>, smem_t);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(static_cast<unsigned>(grid));
     cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = two_sm ? smem_t2 : smem_t;
+    cfg.dynamicSmemBytes = smem_t;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -399,10 +175,7 @@ int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void*
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    if (two_sm)
-      HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_2sm_tma_kernel, map_a, map_b, g, maps));
-    else
-      HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_tma_kernel<2>, map_a, map_b, g, maps));
+    HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_tma_kernel<2>, map_a, map_b, g, maps));
     return grid;
   }
   if (!use_cluster || grid < 2) {
@@ -412,16 +185,12 @@ int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void*
     HPCP_CUDA(cudaGetLastError());
     return grid;
   }
-  HPCP_REQUIRE(!two_sm || grid >= 2, "gemm_put: cluster=3 needs at least two CTAs");
   grid &= ~1;  // whole pairs
-  if (two_sm)
-    HPCP_ENABLE_SMEM(gemm_put_2sm_kernel, gemm_2sm_smem_bytes(0));
-  else
-    HPCP_ENABLE_SMEM(gemm_put_kernel<2>, kSmemBytes);
+  HPCP_ENABLE_SMEM(gemm_put_kernel<2>, kSmemBytes);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(static_cast<unsigned>(grid));
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = two_sm ? gemm_2sm_smem_bytes(0) : kSmemBytes;
+  cfg.dynamicSmemBytes = kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -430,10 +199,7 @@ int launch_gemm_put(const void* a_bf16, const void* b_bf16, void* c_local, void*
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (two_sm)
-    HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_2sm_kernel, map_a, map_b, g));
-  else
-    HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_kernel<2>, map_a, map_b, g));
+  HPCP_CUDA(cudaLaunchKernelEx(&cfg, gemm_put_kernel<2>, map_a, map_b, g));
   return grid;
 }
 

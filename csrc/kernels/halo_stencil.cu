@@ -4,7 +4,7 @@
 // neighbours; wait; swap; kernel" (allreduce-mpi-sycl.cpp:167-181: Accumulate().wait(),
 // SendRecvRing(VA -> right, VB <- left), swap, Accumulate().wait()): every step's compute
 // consumes what the previous step received, and nothing overlaps.  K-halo is that dependency
-// structure as a B200 kernel.  The global field is [world * rows][row_elems] floats, periodic in
+// structure as an H100 kernel.  The global field is [world * rows][row_elems] floats, periodic in
 // the row dimension and split into slabs of `rows` rows per GPU (one row = one message of the
 // p2p benchmark, 188 743 680 B by default, p2p/peer2pear.cpp:115-116).  One step is the stream
 // triad  a = b + s * c  with  b = alpha * u[r],  c = u[r-1] + u[r+1]:
@@ -382,7 +382,7 @@ int occupancy_of(size_t smem) {
 HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device) {
   HaloGeometry g;
   g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : 16) * 1024);
-  g.stages = tune.stages > 0 ? tune.stages : 6;  // 6 x 16 KiB: two CTAs per SM (measured best, profiles/r2c1)
+  g.stages = tune.stages > 0 ? tune.stages : 6;  // 6 x 16 KiB: two CTAs per SM
   HPCP_REQUIRE(g.stages >= 6, "halo_stencil: needs >= 6 shared-memory stages");
   g.smem = static_cast<size_t>(g.stages) * g.tile_bytes + static_cast<size_t>(g.stages) * 16 + 16;
   HPCP_REQUIRE(g.smem <= 227 * 1024, "halo_stencil: stages * tile exceed 227 KiB of shared memory");
@@ -481,7 +481,7 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
 void launch_halo_init(float* u, float* halo_lo, float* halo_hi, int rows, size_t row_elems, int rank, int world,
                       cudaStream_t stream) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 148 * 8));
+  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 8));
   halo_init_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u, halo_lo, halo_hi, rows, row_elems, rank, world);
   HPCP_CUDA(cudaGetLastError());
 }
@@ -490,7 +490,7 @@ void launch_halo_verify_from_init(const float* u, int rows, size_t row_elems, in
                                   float alpha, float s, unsigned long long* mismatch_count, cudaStream_t stream) {
   HPCP_REQUIRE(rows * world <= kHaloMaxGlobalRows, "halo verify: world * rows exceeds 128 global rows");
   const int threads = 128;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 148 * 16));
+  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 16));
   halo_verify_init_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u, rows, row_elems, rank, world, steps, alpha, s,
                                                                     mismatch_count);
   HPCP_CUDA(cudaGetLastError());
@@ -500,7 +500,7 @@ void launch_halo_verify_step(const float* u_new, const float* u_old, const float
                              int rows, size_t row_elems, float alpha, float s, unsigned long long* mismatch_count,
                              cudaStream_t stream) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems / 4 + threads - 1) / threads, 148 * 8));
+  const int ctas = static_cast<int>(std::min<size_t>((row_elems / 4 + threads - 1) / threads, 132 * 8));
   halo_verify_step_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u_new, u_old, up_row, dn_row, rows, row_elems,
                                                                     alpha, s, mismatch_count);
   HPCP_CUDA(cudaGetLastError());

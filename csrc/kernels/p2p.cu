@@ -1,4 +1,4 @@
-// K-p2p: GPU<->GPU data movement over NVLink-5 peer mappings, from inside a kernel.
+// K-p2p: GPU<->GPU data movement over NVLink peer mappings, from inside a kernel.
 //
 // Replaces the transports of the reference's p2p benchmark:
 //   MPI_Isend/Irecv/Waitall  p2p/peer2pear.cpp:32-44  -> rendezvous: wait "ready" word, move, publish "done"
@@ -55,7 +55,7 @@ __device__ __forceinline__ void epilogue_signal(const SyncOps& sync) {
 }
 
 // ------------------------------------------------------------ LdSt engine ----
-// V = uint4 (LDG/STG.128) or ptx::U32x8 (LDG/STG.256, sm_100+).
+// V = uint4 (LDG/STG.128) or ptx::U32x8 (two LDG/STG.128 per thread).
 template <typename V, bool kPeerSrc>
 __device__ __forceinline__ V ld_vec(const V* p);
 template <>
@@ -331,7 +331,7 @@ int launch_copy(void* dst, const void* src, size_t bytes, bool src_is_peer, Copy
 
 void launch_fill_pattern(uint32_t* dst, size_t n_words, uint32_t seed, cudaStream_t stream) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((n_words + threads - 1) / threads, 148 * 8));
+  const int ctas = static_cast<int>(std::min<size_t>((n_words + threads - 1) / threads, 132 * 8));
   fill_pattern_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(dst, n_words, seed);
   HPCP_CUDA(cudaGetLastError());
 }
@@ -347,7 +347,7 @@ void launch_verify_pattern(const uint32_t* data, size_t n_words, uint32_t seed,
   sync.status = status;
   const int threads = 256;
   // All CTAs may spin in the prologue, so keep the grid within one resident wave.
-  const int ctas = static_cast<int>(std::min<size_t>((n_words + threads - 1) / threads, 148 * 4));
+  const int ctas = static_cast<int>(std::min<size_t>((n_words + threads - 1) / threads, 132 * 4));
   verify_pattern_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(data, n_words, seed,
                                                                   mismatch_count, word_sum, sync);
   HPCP_CUDA(cudaGetLastError());

@@ -225,8 +225,8 @@ __global__ void __launch_bounds__(512) ring_allreduce_kernel(const __grid_consta
 
 // ------------------------------------------------------------ K-ring, pull variant ----
 // Same data movement (every rank receives P-1 full blocks and accumulates P), but the bytes cross NVLink as LOADS
-// issued by the receiver instead of stores issued by the sender: SM-issued peer loads reach the copy-engine rate
-// (720-778 GB/s measured for `get`) where SM-issued peer stores stay 4-8 % below it.  Per (hop, chunk):
+// issued by the receiver instead of stores issued by the sender (which initiative moves more bytes per second over
+// the link is a measurement, not an expectation).  Per (hop, chunk):
 //   wait (acquire) arrival word c  -> the left neighbour holds hop t-1 of chunk c (its VA for t = 1, else a slot)
 //   load the chunk from the LEFT neighbour's memory, add it into VC, keep a local copy for the right neighbour
 //   publish (release) arrival word c on the RIGHT neighbour: "hop t of chunk c can be read from me".
@@ -411,9 +411,7 @@ __global__ void __launch_bounds__(kMaxThreads) nvls_kernel(const __grid_constant
     }
     return r;
   };
-  // Grid-stride with U (default 4) independent in-switch reductions in flight per thread.  (A CTA-contiguous
-  // 64 KiB-block variant with 8 in flight and 2 CTAs/SM was measured slower on 8xB200:
-  // 0.345-0.371 ms vs 0.326 ms at 2^25 floats, no gain at 2^28 - see BASELINE.md 4.4.)
+  // Grid-stride with U (default 4) independent in-switch reductions in flight per thread.
   size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   for (; i + (U - 1) * stride < a.slice_vec; i += U * stride) {
     float4 r[U];
@@ -447,7 +445,7 @@ int grid_for(size_t items, int threads, int cap) {
 
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
                   ElemType type, cudaStream_t stream) {
-  const int ctas = grid_for(n, 256, 148 * 8);
+  const int ctas = grid_for(n, 256, 132 * 8);
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     init3_kernel<T><<<ctas, 256, 0, stream>>>(static_cast<T*>(va), static_cast<T*>(vb), static_cast<T*>(vc), n,
@@ -459,7 +457,7 @@ void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, do
 void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaStream_t stream) {
   const size_t lanes = 16 / elem_size(type);
   const size_t nvec = n / lanes, tail = n % lanes;
-  const int ctas = grid_for(std::max<size_t>(nvec, 1), 512, 148 * 4);
+  const int ctas = grid_for(std::max<size_t>(nvec, 1), 512, 132 * 4);
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     accumulate_kernel<T><<<ctas, 512, 0, stream>>>(static_cast<const uint4*>(va), static_cast<uint4*>(vc), nvec,
@@ -471,7 +469,7 @@ void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaSt
 
 void launch_count_mismatch(const void* v, size_t n, double expected, ElemType type,
                            unsigned long long* count, cudaStream_t stream) {
-  const int ctas = grid_for(n, 256, 148 * 8);
+  const int ctas = grid_for(n, 256, 132 * 8);
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     count_mismatch_kernel<T><<<ctas, 256, 0, stream>>>(static_cast<const T*>(v), n, expected, count);
@@ -661,8 +659,7 @@ int launch_allreduce_nvls(const NvlsArgs& args, ElemType type, int ctas, int dev
   constexpr int threads = 512;
   const int sms = device_sm_count(device);
   // Default grid: 32 CTAs.  The in-switch reduction saturates at modest request parallelism and more requesters only
-  // queue in the switch: 8xB200, 2^25 floats 0.297 ms @32 CTAs vs 0.325 @148 vs 0.349 @296; 2^28 floats 2.23 ms @32 vs
-  // 3.41 @148 (NCCL: 0.431 / 2.907 ms) — profiles/r2_call4_8gpu/nvls_tune.txt.  HPCP_NVLS_CTAS_PER_SM / --ctas override.
+  // queue in the switch.  HPCP_NVLS_CTAS_PER_SM / --ctas override.
   const int grid = grid_for(std::max<size_t>(d.slice_vec, 1), threads, ctas > 0 ? ctas : per_sm > 0 ? sms * per_sm : 32);
   d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
 #define HPCP_NVLS(U)                                                  \

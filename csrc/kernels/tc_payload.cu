@@ -1,22 +1,18 @@
 // K-tc-busy: the tensor-core compute command `T` of the concurrency benchmark.
 //
 // The reference's compute command is a dependent-FMA chain on the general-purpose
-// ALUs (concurency/bench.hpp:23-31).  On B200 the machine's compute capacity is the
-// 5th-generation tensor cores, so the suite also offers a compute command that keeps
-// the *tensor pipe* busy while copies run next to it: a per-CTA bf16 GEMM tile
-//        D[128 x 256] (fp32, TMEM) += A[128 x 64] . B[256 x 64]^T        x tripcount
+// ALUs (concurency/bench.hpp:23-31).  On H100 most of the machine's compute capacity is the
+// tensor cores, so the suite also offers a compute command that keeps the *tensor pipe*
+// busy while copies run next to it: a per-CTA bf16 GEMM tile
+//        D[128 x 256] (fp32, registers) += A[128 x 64] . B[256 x 64]^T        x tripcount
 // * A and B tiles are fetched ONCE by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B)
 //   into shared memory, completion on an mbarrier;
-// * one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (4 x K=16 per pass over
-//   the 64-deep tile, `tripcount` passes), accumulating in tensor memory;
-// * tcgen05.commit signals an mbarrier; four epilogue warps read the accumulator back
-//   with tcgen05.ld (32x32b.x32) and store it, so the result is checkable:
+// * two warpgroups issue wgmma.mma_async m64n256k16 (64 rows each, 4 x K=16 per pass over
+//   the 64-deep tile, `tripcount` passes), accumulating in registers;
+// * each thread stores its accumulator fragment, so the result is checkable:
 //   D = tripcount * (A . B^T), exact in fp32 for the small-integer operands used.
 // The loop touches no global memory, so its duration is proportional to tripcount —
 // the same property the FMA chain has — but the busy unit is the tensor core.
-//
-// Warp roles (6 warps): 0 = TMA producer, 1 = MMA issuer, 2 = TMEM allocator +
-// epilogue, 3..5 = epilogue (warp w reads TMEM lanes 32*(w%4) .. +31).
 #include "api.h"
 
 #include <cuda.h>
@@ -28,7 +24,7 @@
 
 #include "../common/cuda_check.h"
 #include "../common/ptx.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hpcp {
 
@@ -37,115 +33,81 @@ namespace {
 constexpr int kTileM = 128;
 constexpr int kTileN = 256;
 constexpr int kTileK = 64;   // one 128-byte swizzle atom of bf16
-constexpr int kUmmaK = 16;   // K per tcgen05.mma for 16-bit operands
-constexpr int kTmemCols = 256;
-constexpr int kThreads = 192;
+constexpr int kThreads = 256;
 constexpr uint32_t kABytes = kTileM * kTileK * 2;  // 16 KiB
 constexpr uint32_t kBBytes = kTileN * kTileK * 2;  // 32 KiB
 
-// Descriptors, TMA tensor loads and tcgen05 wrappers: umma.cuh (shared with the GEMM kernels).
+// Descriptors, TMA tensor loads and wgmma wrappers: wgmma.cuh (shared with the GEMM kernels).
 using umma::cluster_cta_rank;
 using umma::cluster_sync_all;
-using umma::make_idesc;
-using umma::make_smem_desc;
+using umma::kAccRegs;
 using umma::tma_load_2d;
 using umma::tma_load_2d_multicast;
-using umma::tmem_ld_32x32b_x32;
-using umma::umma_bf16;
-using umma::umma_commit;
 
-// Dynamic smem (1024-aligned): A tile | B tile ; static smem: barriers + TMEM base.
+// Dynamic smem (1024-aligned): A tile | B tile ; static smem: the operand barrier.
 // kCluster == 2: launched as thread-block clusters of two CTAs that share the B tile — each CTA
 // fetches half of B (128 of its 256 rows) and TMA-multicasts it into both CTAs' shared memory.
 template <int kCluster>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 1)
     tc_busy_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                    float* __restrict__ out, uint32_t tripcount) {
   extern __shared__ __align__(1024) unsigned char smem[];
   __shared__ __align__(8) uint64_t full_bar;
-  __shared__ __align__(8) uint64_t mma_done_bar;
-  __shared__ uint32_t tmem_base_s;
 
   // SWIZZLE_128B operand tiles must start on a 1024-byte boundary of the shared window.
   unsigned char* smem_a = smem + ((1024u - (ptx::smem_u32(smem) & 1023u)) & 1023u);
   unsigned char* smem_b = smem_a + kABytes;
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;              // warpgroup: accumulator rows [64 wg, 64 wg + 64)
+  const int warp = (threadIdx.x >> 5) & 3;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     ptx::mbar_init(&full_bar, 1);
-    ptx::mbar_init(&mma_done_bar, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 2) {  // one warp allocates (and later frees) the accumulator columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     ptx::smem_u32(&tmem_base_s)),
-                 "r"(static_cast<uint32_t>(kTmemCols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_s;
   // The peer CTA's mbarrier must be initialised before anything is multicast into it.
   if (kCluster > 1) cluster_sync_all();
 
-  if (warp == 0) {
-    if (lane == 0) {  // TMA producer: both operand tiles, once
-      ptx::mbar_arrive_expect_tx(&full_bar, kABytes + kBBytes);
-      tma_load_2d(smem_a, &map_a, 0, 0, &full_bar);
-      if (kCluster > 1) {
-        const uint32_t r = cluster_cta_rank();  // my half of B, delivered to both CTAs
-        tma_load_2d_multicast(smem_b + r * (kBBytes / 2), &map_b, 0, static_cast<int>(r) * (kTileN / 2),
-                              &full_bar, static_cast<uint16_t>(0x3));
-      } else {
-        tma_load_2d(smem_b, &map_b, 0, 0, &full_bar);
-      }
-    }
-  } else if (warp == 1) {
-    ptx::mbar_wait(&full_bar, 0);  // operands landed in smem
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (lane == 0) {  // single-thread MMA issue
-      const uint32_t idesc = make_idesc(kTileM, kTileN);
-      const uint64_t desc_a0 = make_smem_desc(ptx::smem_u32(smem_a));
-      const uint64_t desc_b0 = make_smem_desc(ptx::smem_u32(smem_b));
-      for (uint32_t it = 0; it < tripcount; ++it) {
-#pragma unroll
-        for (int k = 0; k < kTileK / kUmmaK; ++k) {
-          // advance the start address by k * 32 bytes inside the 128-byte swizzle atom
-          const uint64_t adv = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          umma_bf16(tmem_d, desc_a0 + adv, desc_b0 + adv, idesc, (it | static_cast<uint32_t>(k)) != 0u);
-        }
-      }
-      umma_commit(&mma_done_bar);  // arrives when every MMA above has completed
-    }
-    __syncwarp();
-  }
-  if (warp >= 2) {  // epilogue: TMEM -> registers -> global
-    ptx::mbar_wait(&mma_done_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int lane_group = warp & 3;               // TMEM lanes this warp may touch
-    const int row = lane_group * 32 + lane;        // accumulator row == TMEM lane
-    float* out_row = out + (static_cast<size_t>(blockIdx.x) * kTileM + row) * kTileN;
-    for (int col = 0; col < kTileN; col += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(tmem_d + (static_cast<uint32_t>(lane_group * 32) << 16) + col, r);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(out_row + col + j) =
-            make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                        __uint_as_float(r[j + 3]));
+  if (threadIdx.x == 0) {  // TMA producer: both operand tiles, once
+    ptx::mbar_arrive_expect_tx(&full_bar, kABytes + kBBytes);
+    tma_load_2d(smem_a, &map_a, 0, 0, &full_bar);
+    if (kCluster > 1) {
+      const uint32_t r = cluster_cta_rank();  // my half of B, delivered to both CTAs
+      tma_load_2d_multicast(smem_b + r * (kBBytes / 2), &map_b, 0, static_cast<int>(r) * (kTileN / 2), &full_bar,
+                            static_cast<uint16_t>(0x3));
+    } else {
+      tma_load_2d(smem_b, &map_b, 0, 0, &full_bar);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d),
-                 "r"(static_cast<uint32_t>(kTmemCols))
-                 : "memory");
+  ptx::mbar_wait(&full_bar, 0);  // operands landed in smem
+
+  float d[kAccRegs] = {};  // tripcount 0 stores zeros
+  const uint32_t sa = ptx::smem_u32(smem_a) + static_cast<uint32_t>(wg) * (kABytes / 2);
+  const uint32_t sb = ptx::smem_u32(smem_b);
+  for (uint32_t it = 0; it < tripcount; ++it) {
+    umma::wgmma_fence_operand(d);
+    umma::wgmma_fence();
+    umma::wgmma_kblock(d, sa, sb, it != 0);
+    umma::wgmma_commit();
+    umma::wgmma_wait<1>();  // one pass in flight behind the one being issued
+    umma::wgmma_fence_operand(d);
+  }
+  umma::wgmma_wait<0>();
+  umma::wgmma_fence_operand(d);
+
+  // Fragment -> row-major out[cta][128][256] (wgmma.cuh: fragment layout of wgmma_m64n256k16_bf16).
+  const int row = wg * 64 + warp * 16 + (lane >> 2);
+  float* out_tile = out + static_cast<size_t>(blockIdx.x) * kTileM * kTileN;
+#pragma unroll
+  for (int j = 0; j < kTileN / 8; ++j) {
+    const int col = 8 * j + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(out_tile + static_cast<size_t>(row) * kTileN + col) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(out_tile + static_cast<size_t>(row + 8) * kTileN + col) =
+        make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
   // Neither CTA of a pair may retire while the other could still be receiving its multicast.
   if (kCluster > 1) cluster_sync_all();
 }

@@ -1,5 +1,5 @@
 // Tile and gather-piece orderings of the tensor-core kernels as plain integer functions, shared by the device
-// code (umma.cuh, gemm_collective.cu) and the host (bindings -> tests/test_tile_order.py checks that every order
+// code (wgmma.cuh, gemm_collective.cu) and the host (bindings -> tests/test_tile_order.py checks that every order
 // is a bijection, that CTA pairs get vertically adjacent tiles and that the gather covers every remote byte
 // exactly once — on a machine without a GPU).
 #pragma once
@@ -16,9 +16,9 @@
 namespace hpcp {
 namespace umma {
 
-// Tile rasterisation: groups of kGroupM tile-rows, m fastest inside a group, so the ~148 tiles that
-// are in flight at any time cover a near-square block of C (8 x ~18 tiles): fewer distinct A/B
-// panels per k-step than row-major order -> less HBM traffic once A and B exceed the 126 MB L2.
+// Tile rasterisation: groups of kGroupM tile-rows, m fastest inside a group, so the ~132 tiles that
+// are in flight at any time cover a near-square block of C (8 x ~17 tiles): fewer distinct A/B
+// panels per k-step than row-major order -> less HBM traffic once A and B exceed the 50 MB L2.
 constexpr int kGroupM = 8;
 HPCP_HD void tile_coords(int tile, int tiles_m, int tiles_n, int* m_blk, int* n_blk) {
   const int group_size = kGroupM * tiles_n;

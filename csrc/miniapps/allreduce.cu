@@ -94,7 +94,7 @@ void print_help() {
                " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
                " --ctas N --chunk N    kernel tuning (CTAs per rank, elements per ring chunk)\n"
                " --pull                fused ring, receiver-driven: every block is LOADED from the left neighbour's\n"
-               "                       memory (peer loads reach the copy-engine rate, peer stores stay 4-8 % below)\n"
+               "                       memory (loads issued by the receiver instead of the sender's stores)\n"
                " --slots 2             fused ring with two receive slots + per-chunk acks (the reference's VA/VB\n"
                "                       double buffer) instead of P-1 slots without flow control\n"
                " --json FILE           append one JSON row\n"
@@ -538,8 +538,8 @@ int main(int argc, char** argv) {
     if (cfg.use_collective) {
       bool want_nvls = cfg.coll == "nvls";
       if (cfg.coll == "auto") {
-        // int: two-shot (128-bit peer loads for every type) — multimem.ld_reduce has no vector form for .s32 and ran
-        // 2.5x slower than float (profiles/r1_call3_8gpu); float: in-switch reduction where multicast exists.
+        // int: two-shot (128-bit peer loads for every type) — multimem.ld_reduce has no vector form for .s32;
+        // float: in-switch reduction where multicast exists.
         want_nvls = ranks_per_dev == 1 && cfg.kind == AllocKind::kDevice && cfg.type == ElemType::kFloat;
         for (int d : devices) want_nvls = want_nvls && NodeMemory::multicast_supported(d);
       }
@@ -591,7 +591,8 @@ int main(int argc, char** argv) {
     std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << sh.best_ms << " ms | "
               << algo_name << " " << elem_type_name(cfg.type) << " " << alloc_kind_name(cfg.kind)
               << " P=" << P << " N=2^" << cfg.log2_elems << " | " << gbps
-              << " GB/s sent per rank (" << gbps / 900.0 * 100.0 << "% of 900 GB/s)" << std::endl;
+              << " GB/s sent per rank (" << gbps / 450.0 * 100.0 << "% of the 450 GB/s NVLink 4 nominal per direction)"
+              << std::endl;
     if (!cfg.json_path.empty()) {
       FILE* f = std::fopen(cfg.json_path.c_str(), "a");
       if (f) {

@@ -3,8 +3,8 @@
 // Capability parity with aurora.mpich.miniapps/src/include/devices.hpp:22-59:
 // if there are fewer devices than ranks every rank gets ONE device chosen
 // round-robin (oversubscription); otherwise the devices are dealt in contiguous
-// blocks of ndev/size per rank.  PVC "fission" into tiles has no B200
-// equivalent (one B200 is one CUDA device; MIG is out of scope), so the
+// blocks of ndev/size per rank.  PVC "fission" into tiles has no H100
+// equivalent (one H100 is one CUDA device; MIG is out of scope), so the
 // `fission` switch is accepted and ignored.
 #pragma once
 

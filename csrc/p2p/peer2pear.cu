@@ -1,4 +1,4 @@
-// peer2pear — GPU<->GPU bandwidth between rank pairs over NVLink-5 / NVSwitch.
+// peer2pear — GPU<->GPU bandwidth between rank pairs over NVLink / NVSwitch.
 //
 // Capability parity with p2p/peer2pear.cpp of the reference:
 //   * ranks are paired (2k, 2k+1); phase 1 is unidirectional (even -> odd), phase 2
@@ -11,8 +11,8 @@
 //   * the two upstream builds (two-sided Isend/Irecv, one-sided Put+fence under
 //     -DUSE_WIN) are the run-time transports `sendrecv` and `put`; `get` is new;
 //     `memcpy` (cudaMemcpyPeerAsync, copy engines) is the stock-library baseline.
-// B200 design: one process, one host thread per rank (rank_runtime.h), every GPU
-// peer-mapped; data is moved by hand-written sm_100a kernels (kernels/p2p.cu) and
+// H100 design: one process, one host thread per rank (rank_runtime.h), every GPU
+// peer-mapped; data is moved by hand-written sm_90a kernels (kernels/p2p.cu) and
 // synchronised with release/acquire epoch words in peer memory — no MPI, no NCCL.
 // Time is measured on the device (CUDA events around the rank's kernels, started
 // behind an in-kernel cross-GPU barrier) and reduced with max over ranks.
@@ -48,7 +48,7 @@ struct Config {
   std::string label = "Tile2Tile";
   int ranks = 0;  // 0 -> all GPUs (rounded down to even)
   std::string transport = "put";
-  std::string engine = "tma";   // measured best for both put (683 vs 675 GB/s) and get (731 vs 726), BASELINE.md 5.2
+  std::string engine = "tma";   // one DMA thread per CTA: frees the LSU and registers of the other threads
   std::string mapping = "compact";
   std::vector<size_t> sizes;
   bool sweep = false;
@@ -419,7 +419,7 @@ int run_on_host(const Config& cfg) {
         << "\",\"engine\":\"host\",\"fused_triad\":false,\"mapping\":\"" << cfg.mapping << "\",\"ranks\":" << P
         << ",\"bytes\":" << bytes << ",\"uni_us\":" << uni_ns * 1e-3 << ",\"bi_us\":" << bi_ns * 1e-3
         << ",\"uni_GBps\":" << uni_bw << ",\"bi_GBps\":" << 2.0 * static_cast<double>(bytes) * pairs / bi_ns
-        << ",\"uni_GBps_per_pair\":" << uni_bw / pairs << ",\"frac_of_900GBps_per_dir\":" << (uni_bw / pairs) / 900.0
+        << ",\"uni_GBps_per_pair\":" << uni_bw / pairs << ",\"frac_of_450GBps_per_dir\":" << (uni_bw / pairs) / 450.0
         << ",\"mismatches\":" << mismatches << "}\n";
     }
   }
@@ -506,7 +506,7 @@ int main(int argc, char** argv) {
           << ",\"uni_us\":" << sh.uni_ns[si] * 1e-3 << ",\"bi_us\":" << sh.bi_ns[si] * 1e-3
           << ",\"uni_GBps\":" << uni_bw << ",\"bi_GBps\":" << bi_bw
           << ",\"uni_GBps_per_pair\":" << uni_bw / pairs
-          << ",\"frac_of_900GBps_per_dir\":" << (uni_bw / pairs) / 900.0
+          << ",\"frac_of_450GBps_per_dir\":" << (uni_bw / pairs) / 450.0
           << ",\"mismatches\":" << sh.mismatches[si] << "}\n";
       }
     }

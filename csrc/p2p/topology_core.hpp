@@ -5,7 +5,7 @@
 // set and greedily merges overlapping sets into "planes" (topology.cpp:50-89),
 // then prints the planes or the k-th device id (:92-106) for tile_mapping.sh.
 //
-// B200 redesign: links come from NVML (NVLink state / remote device type / remote
+// H100 redesign: links come from NVML (NVLink state / remote device type / remote
 // PCI id per link) with cudaDeviceGetP2PAttribute as a second source; an NVSwitch
 // is modelled as one extra fabric node so that every GPU hanging off the switch
 // complex lands in the same plane.  The clustering itself is a union-find over

@@ -1,7 +1,7 @@
 // Host-only self-test of the native runtime pieces that need no GPU: the thread-per-rank runtime,
 // the device-subset policy, the dtype trait table, plane clustering and rank->device policies, and
 // the concurrency driver's pure functions.  Built as bin/native_selftest; run by tests/test_native_selftest.py
-// (the reference has no unit tests at all — SURVEY.md §4).
+// (the reference has no unit tests at all).
 #include <atomic>
 #include <cmath>
 #include <cstdio>

@@ -1,12 +1,12 @@
-"""hpc-patterns-b200: a Blackwell-native GPU-communication-pattern suite.
+"""hpc-patterns-b200: a Hopper-native GPU-communication-pattern suite.
 
 Same capabilities and entry points as argonne-lcf/HPC-Patterns (concurrency
 bench, peer2pear, topology / tile mapping, allreduce miniapps, runtime interop),
-rebuilt for 8xB200: hand-written sm_100a kernels that move data over NVLink-5 /
+rebuilt for 8xH100: hand-written sm_90a kernels that move data over NVLink 4 /
 NVSwitch peer mappings and fuse each transfer with its adjacent compute.
 
 Layout
-  ops/       Python wrappers of the sm_100a kernels (p2p copy, fused triad+put,
+  ops/       Python wrappers of the sm_90a kernels (p2p copy, fused triad+put,
              ring / two-shot / NVLS allreduce, concurrency payloads)
   parallel/  process-group plumbing: symmetric peer memory (CUDA IPC / torch
              symmetric memory), signal pads, topology, rank->device mapping
@@ -33,7 +33,7 @@ def native():
     """Return the native extension module, building nothing implicitly.
 
     Fails loudly when the extension is missing: on a GPU box a silent Python
-    fallback would hide that the sm_100a kernels are not the ones running.
+    fallback would hide that the sm_90a kernels are not the ones running.
     """
     global _ext
     if _ext is not None:

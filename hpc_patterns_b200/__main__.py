@@ -27,7 +27,7 @@ def _no_gpu_message(prog: str):
 
     if prog in _GPU_PROGRAMS and not torch.cuda.is_available():
         hint = f"; bin/{prog} --cpu is the host-only plumbing run" if prog in ("peer2pear", "allreduce") else ""
-        return f"Error: {prog}: no CUDA device (this program runs sm_100a kernels{hint})"
+        return f"Error: {prog}: no CUDA device (this program runs sm_90a kernels{hint})"
     return None
 
 

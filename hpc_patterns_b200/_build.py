@@ -1,7 +1,7 @@
 """In-tree build of the native extension ``hpc_patterns_b200/_C*.so``.
 
 ``python -m hpc_patterns_b200._build`` (or ``make ext``) compiles every CUDA
-source for sm_100a (``-gencode arch=compute_100a,code=sm_100a -lineinfo``) into
+source for sm_90a (``-gencode arch=compute_90a,code=sm_90a -lineinfo``) into
 ``build/libhpcp.a`` through the Makefile, compiles the pybind11 bindings and links
 the extension next to this file, so the ``.so`` travels with a repo snapshot.
 The reference has no Python build at all (its builds are the shell one-liners
@@ -17,7 +17,7 @@ import sysconfig
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo"]
 
 
 def host_cxx() -> str:

@@ -63,7 +63,7 @@ class AllreduceResult:
         gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
         return {"pattern": "allreduce", "algo": self.algo, "type": self.dtype, "ranks": self.world,
                 "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
-                "frac_of_900GBps": gbps / 900.0, "mismatches": self.mismatches}
+                "frac_of_450GBps": gbps / 450.0, "mismatches": self.mismatches}
 
 
 class AllreduceMiniapp:
@@ -273,8 +273,7 @@ def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int):
 
     Decided BEFORE anything is allocated and agreed across ranks (min over ranks of the local probe), so ranks can
     neither diverge on the algorithm nor leak a half-built instance:
-      * int:   two-shot — ``multimem.ld_reduce`` has no vector form for .s32 (one 4-byte request per thread, measured
-               2.5x slower than float, profiles/r1_call3_8gpu), peer loads are 128-bit for every type;
+      * int:   two-shot — ``multimem.ld_reduce`` has no vector form for .s32 (one 4-byte request per thread), peer loads are 128-bit for every type;
       * float: NVLS (in-switch reduction) when every rank reports multicast support, else two-shot."""
     C = native()
     if dtype != "float":

@@ -4,7 +4,7 @@ The reference's one communication loop is the miniapp's ring: compute, wait, exc
 full block with BOTH ring neighbours (``MPI_Send`` to the right, ``MPI_Recv`` from the
 left), wait, swap, compute on what arrived (allreduce-mpi-sycl.cpp:167-181) — a 1-D
 periodic neighbour exchange with a true step-to-step dependency and no overlap at all.
-``HaloStencil`` is that loop as a time-stepping stencil on B200s:
+``HaloStencil`` is that loop as a time-stepping stencil on H100s:
 
 * the global field ``[world * rows][row_elems]`` is periodic in the row dimension and
   split into slabs of ``rows`` rows per GPU; one row is one message (188 743 680 B by
@@ -36,17 +36,14 @@ DEFAULT_ROWS = 8
 MODES = ("pull", "push", "none")
 
 
-def balanced_rows(hbm_gbs: float = 6567.4, nvlink_gbs: float = 706.1) -> int:
+def balanced_rows(hbm_gbs: float, nvlink_gbs: float) -> int:
     """Rows per slab for which the step's HBM time equals its NVLink time.
 
     The reference's concurrency benchmark tunes its commands to equal duration before it
     overlaps them (concurency/main.cpp:219-258); the same rule here: a step streams
     (2*rows + 2) rows through HBM in pull mode (rows reads + rows writes + the two boundary
     rows the neighbours read) and moves 2 rows over NVLink in EACH direction at once.
-    Denominators are stock measurements, not this kernel's: the driver's copy peak
-    (MEASURED_PEAKS.json hbm_gbs) and the copy engines' rate with both directions of a pair
-    busy — 1412.2 GB/s per pair = 706.1 per direction (profiles/r2_call3_2gpu/p2p_tune.jsonl;
-    one direction alone reaches 717-770).  -> 8 rows.
+    Denominators are the caller's: a copy bandwidth of HBM and a per-direction NVLink rate.
     """
     rows = (2.0 * hbm_gbs / nvlink_gbs - 2.0) / 2.0
     return max(1, int(rows))
@@ -424,7 +421,7 @@ def main(argv: Optional[List[str]] = None) -> int:
     from ..utils.timing import BlockTimer
 
     ap = argparse.ArgumentParser(prog="halo")
-    ap.add_argument("--rows", type=int, default=balanced_rows())
+    ap.add_argument("--rows", type=int, default=DEFAULT_ROWS)
     ap.add_argument("--bytes", type=int, default=REFERENCE_MESSAGE_BYTES)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--iters", type=int, default=5)

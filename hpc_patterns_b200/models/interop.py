@@ -3,7 +3,7 @@
 The reference shows how two GPU runtimes (OpenMP offload and SYCL) share a device, a
 context and memory, directly (``sycl_omp_ze_interopt/interop_omp_sycl.cpp:40-75``) or through
 native Level-Zero handles (``interop_omp_ze_sycl.cpp:81-116``), with a cached per-device
-table (``xomp_get_infos_devices`` / ``xomp_get_device_info``).  On B200 the two runtimes are
+table (``xomp_get_infos_devices`` / ``xomp_get_device_info``).  On H100 the two runtimes are
 PyTorch (its caching allocator, its streams) and the raw CUDA code in ``csrc/``:
 
 direct   * a torch tensor's ``data_ptr()`` is consumed by a native kernel, launched on

@@ -266,7 +266,7 @@ class P2PResult:
                 "uni_us": self.uni_ns * 1e-3, "bi_us": self.bi_ns * 1e-3,
                 "uni_GBps": self.uni_gbps, "bi_GBps": self.bi_gbps,
                 "uni_GBps_per_pair": self.uni_gbps / max(self.pairs, 1),
-                "frac_of_900GBps_per_dir": self.uni_gbps / max(self.pairs, 1) / 900.0,
+                "frac_of_450GBps_per_dir": self.uni_gbps / max(self.pairs, 1) / 450.0,
                 "mismatches": self.mismatches, **self.extra}
 
 
@@ -280,7 +280,7 @@ class P2PBench:
                  iters: int = 10, label: str = "Tile2Tile", timeout_s: float = 30.0, put_fraction: float = 0.5):
         """``hybrid``: every message is driven from BOTH ends at once — the sender puts the first ``put_fraction`` of it
         (peer stores) while the receiver gets the rest (peer loads), two kernels on two GPUs working on one direction of
-        the link.  SM-issued stores and SM-issued loads saturate at different rates below the link's (BASELINE.md §4.1);
+        the link.  SM-issued stores and SM-issued loads can saturate at different rates below the link's;
         together they can fill what either leaves."""
         if transport not in self.TRANSPORTS:
             raise ValueError(f"transport must be one of {self.TRANSPORTS}")

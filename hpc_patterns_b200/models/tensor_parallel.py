@@ -1,10 +1,10 @@
 """Tensor-parallel linear layers whose collective is fused into the GEMM kernel.
 
-Beyond the reference (which has no GEMM, SURVEY.md §2.4): the suite's "compute step followed by a
+Beyond the reference (which has no GEMM): the suite's "compute step followed by a
 collective as ONE kernel" family applied to the tensor cores.
 
 ``RowParallelLinear``     every rank holds a K-slice of the weight; ``y = reduce_scatter(x_r @ W_r.T)``.
-                          One kernel: tcgen05 GEMM whose epilogue adds each tile into the owning rank's
+                          One kernel: wgmma GEMM whose epilogue adds each tile into the owning rank's
                           fp32 shard over NVLink (K-gemm-rs), then a wait for the P arrival epochs.
 ``ColumnParallelLinear``  activations are row-sharded, the weight column-sharded:
                           ``y = all_gather(x_r) @ W_r.T``.  One kernel: gather threads pull the peers'
@@ -298,7 +298,7 @@ def main(argv: Optional[List[str]] = None) -> int:
                                                        "(tokens = M, hidden = K, ffn = N)")
     args = ap.parse_args(argv)
     if not torch.cuda.is_available():
-        print("Error: tp: no CUDA device (this program runs sm_100a kernels)", flush=True)
+        print("Error: tp: no CUDA device (this program runs sm_90a kernels)", flush=True)
         return 1
 
     comm = Comm()

@@ -1,4 +1,4 @@
-"""Python entry points of the sm_100a kernels (csrc/kernels).  All ops fail loudly
+"""Python entry points of the sm_90a kernels (csrc/kernels).  All ops fail loudly
 if the native extension is missing — there is no eager/PyTorch fallback."""
 from .p2p import copy, fill_pattern, verify_pattern  # noqa: F401
 from .fused import triad_put, triad_reference  # noqa: F401

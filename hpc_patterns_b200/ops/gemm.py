@@ -1,8 +1,8 @@
-"""K-gemm-put: tcgen05 bf16 GEMM whose epilogue stores the result tile into a peer GPU.
+"""K-gemm-put: wgmma bf16 GEMM whose epilogue stores the result tile into a peer GPU.
 
 ``gemm_put(a, b, c_local=..., c_peer=...)`` computes ``C = A @ B.T`` (A ``[M,K]``, B ``[N,K]``, both
-bf16 row-major, fp32 result) with the hand-written sm_100a kernel in ``csrc/kernels/gemm_put.cu``
-(TMA-fed smem ring, ``tcgen05.mma`` accumulating in TMEM, ``tcgen05.ld`` epilogue) and writes every
+bf16 row-major, fp32 result) with the hand-written sm_90a kernel in ``csrc/kernels/gemm_put.cu``
+(TMA-fed smem ring, ``wgmma.mma_async`` accumulating in registers, epilogue straight from the registers) and writes every
 128x256 tile to ``c_local`` and/or straight into the peer-mapped ``c_peer`` over NVLink.
 The reference has no GEMM; this op is the tensor-core member of the suite's fused
 "produce a tile -> put it to the neighbour" family.  Stock comparison: ``torch.matmul`` (cuBLAS)
@@ -22,10 +22,9 @@ def gemm_put(a: torch.Tensor, b: torch.Tensor, c_local: Optional[torch.Tensor] =
              sync: Optional[dict] = None, ctas: int = 0, stream: Optional[int] = None,
              out_dtype: torch.dtype = torch.float32, cluster: int = 0, epilogue: str = "st") -> int:
     """Launch the fused GEMM(+put).  ``out_dtype`` fp32 or bf16 (c_local / c_peer hold that type).
-    ``cluster``: 0 auto, 1 = single CTAs, 2 = CTA pairs sharing the B tile through TMA multicast,
-    3 = 2-SM UMMA (``tcgen05.mma.cta_group::2``: one 256x256 tile per CTA pair; opt-in).
-    ``epilogue``: ``"st"`` = 128-bit stores from the epilogue warps (the measured kernel), ``"tma"`` (opt-in, not yet
-    run on a GPU) = swizzled smem pieces + ``cp.async.bulk.tensor.2d`` stores issued by the TMA unit.
+    ``cluster``: 0 auto, 1 = single CTAs, 2 = CTA pairs sharing the B tile through TMA multicast.
+    ``epilogue``: ``"st"`` = 128-bit stores from the consumer warps, ``"tma"`` (opt-in) = swizzled smem pieces +
+    ``cp.async.bulk.tensor.2d`` stores issued by the TMA unit.
     Returns the number of CTAs launched (for ticket bookkeeping)."""
     if epilogue not in ("st", "tma"):
         raise ValueError("epilogue must be 'st' or 'tma'")

@@ -1,7 +1,7 @@
 """Compute payloads of the concurrency benchmark as stand-alone ops.
 
 ``busy_wait``   the dependent-FMA chain `C` (concurency/bench.hpp:23-31 maths)
-``tc_busy``     the tcgen05/TMEM/TMA tensor-core tile loop `T` (csrc/kernels/tc_payload.cu)
+``tc_busy``     the wgmma/TMA tensor-core tile loop `T` (csrc/kernels/tc_payload.cu)
 ``fused_group`` a whole command group as ONE persistent kernel (csrc/kernels/bench_fused.cu)
 """
 from __future__ import annotations

@@ -5,7 +5,7 @@ Capability parity with ``p2p/tile_mapping.sh:1-37`` of the reference, which comp
 the last one asking ``./topology <rank>``) and exports it through ``ZE_AFFINITY_MASK`` (ZAM)
 or ``ONEAPI_DEVICE_SELECTOR`` (ODS) before exec'ing the program.
 
-B200 mapping of the two mechanisms:
+H100 mapping of the two mechanisms:
   CVD  ``CUDA_VISIBLE_DEVICES=<gpu>``  — the process sees only its GPU (↔ ZAM)
   SET  ``HPCP_DEVICE=<gpu>``           — all GPUs stay visible, the program selects the
                                           ordinal with cudaSetDevice / torch.cuda.set_device (↔ ODS)

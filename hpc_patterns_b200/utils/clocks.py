@@ -9,8 +9,7 @@ is the fallback.
 ``start()`` does all the slow work (``nvmlInit``, handle lookup, thread start) and must be called
 well before any timed region — never between a cross-rank barrier and the start event: NVML
 calls take tens of milliseconds when eight processes keep the GPUs busy, and the other ranks'
-kernels would wait for this rank inside their timed region (that was the 7.3 ms/step of the
-round-1 8-GPU record).  ``pause()`` / ``resume()`` only flip a flag the polling thread reads.
+kernels would wait for this rank inside their timed region.  ``pause()`` / ``resume()`` only flip a flag the polling thread reads.
 """
 from __future__ import annotations
 

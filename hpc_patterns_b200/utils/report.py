@@ -1,38 +1,18 @@
 """Turn the JSON rows the programs emit (``--json``) into a roofline report.
 
 Every pattern writes rows with device-timed, max-over-ranks numbers; this module adds the
-fraction of the relevant roofline — NVLink 900 GB/s nominal and 770 GB/s measured per
-direction per GPU for communication paths, measured HBM copy bandwidth for local paths
-(``MEASURED_PEAKS.json``) — and renders markdown tables.
+fraction of the relevant roofline — the H100 SXM data-sheet rates: NVLink 450 GB/s per direction per GPU for
+communication paths, 989 TFLOP/s dense bf16 for the GEMMs — and renders markdown tables.
 ``python -m hpc_patterns_b200.utils.report rows.jsonl [...] > REPORT.md``
 """
 from __future__ import annotations
 
 import json
-import os
 import sys
 from typing import Dict, Iterable, List
 
-NVLINK_NOMINAL_GBPS = 900.0
-NVLINK_MEASURED_GBPS = 770.0      # peer copy per direction, profiling recipe
-HBM_FALLBACK_GBPS = 6650.0
-BF16_FALLBACK_TFLOPS = 1600.0   # cuBLAS bf16, profiling recipe fallback
-
-
-def measured_hbm_gbps(root: str = ".") -> float:
-    try:
-        with open(os.path.join(root, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"])
-    except (OSError, KeyError, ValueError):
-        return HBM_FALLBACK_GBPS
-
-
-def measured_bf16_tflops(root: str = ".") -> float:
-    try:
-        with open(os.path.join(root, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["bf16_tflops"])
-    except (OSError, KeyError, ValueError):
-        return BF16_FALLBACK_TFLOPS
+NVLINK_NOMINAL_GBPS = 450.0     # H100 SXM, NVLink 4, per direction (900 GB/s bidirectional), data sheet
+BF16_DENSE_TFLOPS = 989.0       # H100 SXM dense bf16 at up to 700 W, data sheet
 
 
 def load_rows(paths: Iterable[str]) -> List[Dict]:
@@ -50,27 +30,27 @@ def load_rows(paths: Iterable[str]) -> List[Dict]:
 
 
 def p2p_table(rows: List[Dict]) -> str:
-    out = ["| label | transport | engine | ranks | bytes | uni GB/s | bi GB/s | uni per pair / 770 | / 900 |",
-           "|---|---|---|---|---|---|---|---|---|"]
+    out = ["| label | transport | engine | ranks | bytes | uni GB/s | bi GB/s | uni per pair / 450 |",
+           "|---|---|---|---|---|---|---|---|"]
     for r in rows:
         if r.get("pattern") != "peer2pear":
             continue
         per_pair = r["uni_GBps"] / max(r["ranks"] // 2, 1)
         out.append(f"| {r.get('label','')} | {r.get('transport','')} | {r.get('engine','')} | {r['ranks']} | "
                    f"{r['bytes']} | {r['uni_GBps']:.1f} | {r['bi_GBps']:.1f} | "
-                   f"{per_pair / NVLINK_MEASURED_GBPS:.2f} | {per_pair / NVLINK_NOMINAL_GBPS:.2f} |")
+                   f"{per_pair / NVLINK_NOMINAL_GBPS:.2f} |")
     return "\n".join(out)
 
 
 def allreduce_table(rows: List[Dict]) -> str:
-    out = ["| algo | type | ranks | elements | ms | GB/s sent per rank | / 770 | / 900 |",
-           "|---|---|---|---|---|---|---|---|"]
+    out = ["| algo | type | ranks | elements | ms | GB/s sent per rank | / 450 |",
+           "|---|---|---|---|---|---|---|"]
     for r in rows:
         if r.get("pattern") != "allreduce":
             continue
         g = r["GBps_sent_per_rank"]
         out.append(f"| {r['algo']} | {r['type']} | {r['ranks']} | {r['elements']} | {r['ms']:.4f} | {g:.1f} | "
-                   f"{g / NVLINK_MEASURED_GBPS:.2f} | {g / NVLINK_NOMINAL_GBPS:.2f} |")
+                   f"{g / NVLINK_NOMINAL_GBPS:.2f} |")
     return "\n".join(out)
 
 
@@ -86,11 +66,11 @@ def concurency_table(rows: List[Dict]) -> str:
     return "\n".join(out)
 
 
-def tensor_parallel_table(rows: List[Dict], root: str = ".") -> str:
+def tensor_parallel_table(rows: List[Dict]) -> str:
     """Rows of ``python -m hpc_patterns_b200 tp`` (one JSON object per run: ranks, m, n, k and one sub-object per
-    layer).  The roofline of a fused layer is the slower of its GEMM at the measured cuBLAS rate and its bytes over
-    NVLink at the measured 770 GB/s per direction."""
-    peak = measured_bf16_tflops(root)
+    layer).  The roofline of a fused layer is the slower of its GEMM at the data-sheet bf16 rate and its bytes over
+    NVLink at the nominal 450 GB/s per direction."""
+    peak = BF16_DENSE_TFLOPS
     out = ["| layer | ranks | M | N | K | fused ms | stock ms (cuBLAS + NCCL) | speed-up | TFLOP/s per GPU | "
            "roofline ms (tensor / NVLink) | fraction |", "|---|---|---|---|---|---|---|---|---|---|---|"]
     for r in rows:
@@ -105,7 +85,7 @@ def tensor_parallel_table(rows: List[Dict], root: str = ".") -> str:
             if not isinstance(d, dict) or "fused_ms" not in d:
                 continue
             t_tensor = flops / (peak * 1e9)
-            t_link = link_bytes / (NVLINK_MEASURED_GBPS * 1e6)
+            t_link = link_bytes / (NVLINK_NOMINAL_GBPS * 1e6)
             roof = max(t_tensor, t_link)
             label = name + (f" (chunk {r['chunk']})" if "chunk" in r else "")
             out.append(f"| {label} | {P} | {m} | {n} | {k} | {d['fused_ms']:.4f} | {d['stock_ms']:.4f} | "
@@ -114,19 +94,16 @@ def tensor_parallel_table(rows: List[Dict], root: str = ".") -> str:
     return "\n".join(out)
 
 
-def gemm_table(rows: List[Dict], root: str = ".") -> str:
+def gemm_table(rows: List[Dict]) -> str:
     """Rows of scripts/gemm_put_bench.py."""
-    peak = measured_bf16_tflops(root)
-    out = ["| M | N | K | ranks | ours TFLOP/s | 2-SM UMMA | cuBLAS | ours / measured peak | fused GEMM->put ms | "
-           "stock ms |", "|---|---|---|---|---|---|---|---|---|---|"]
+    out = ["| M | N | K | ranks | ours TFLOP/s | cuBLAS | ours / data-sheet peak | fused GEMM->put ms | "
+           "stock ms |", "|---|---|---|---|---|---|---|---|---|"]
     for r in rows:
         if "gemm_tflops" not in r:
             continue
-        two = r.get("gemm_tflops_2sm")
-        best = max(r["gemm_tflops"], two or 0)
         nan = float("nan")
         out.append(f"| {r['m']} | {r['n']} | {r['k']} | {r.get('ranks', 1)} | {r['gemm_tflops']:.0f} | "
-                   f"{'%.0f' % two if two else '-'} | {r['cublas_tflops']:.0f} | {best / peak:.2f} | "
+                   f"{r['cublas_tflops']:.0f} | {r['gemm_tflops'] / BF16_DENSE_TFLOPS:.2f} | "
                    f"{r.get('fused_gemm_put_ms', nan):.3f} | {r.get('stock_cublas_then_memcpy_ms', nan):.3f} |")
     return "\n".join(out)
 
@@ -142,7 +119,7 @@ def render(rows: List[Dict]) -> str:
     if any("row_parallel" in r or "column_parallel" in r for r in rows):
         parts += ["## tensor-parallel layers (GEMM fused with its collective)\n", tensor_parallel_table(rows), ""]
     if any("gemm_tflops" in r for r in rows):
-        parts += ["## tcgen05 GEMM (-> put)\n", gemm_table(rows), ""]
+        parts += ["## tensor-core GEMM (-> put)\n", gemm_table(rows), ""]
     return "\n".join(parts)
 
 

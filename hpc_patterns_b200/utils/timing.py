@@ -31,7 +31,7 @@ def time_region_ms(fn: Callable[[], None], device: int, stream: torch.cuda.Strea
 
 
 def flush_l2(device: int, nbytes: int = 256 << 20) -> None:
-    """Evict L2 (126 MB on B200) by writing a larger scratch buffer."""
+    """Evict L2 (50 MB on H100) by writing a larger scratch buffer."""
     buf = getattr(flush_l2, "_buf", None)
     if buf is None or buf.numel() < nbytes or buf.device.index != device:
         buf = torch.empty(nbytes, dtype=torch.uint8, device=torch.device("cuda", device))

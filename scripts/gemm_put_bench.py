@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """K-gemm-put vs the stock pattern (cuBLAS matmul, then a copy-engine peer copy).
 
-1 GPU : GEMM-only throughput of the hand-written tcgen05 kernel next to torch.matmul (cuBLAS).
+1 GPU : GEMM-only throughput of the hand-written wgmma kernel next to torch.matmul (cuBLAS).
 N GPUs: (torchrun) every rank computes C = A.B^T and puts it into its ring neighbour —
         fused in the kernel's epilogue vs matmul + cudaMemcpyAsync to the peer mapping.
 """
@@ -62,12 +62,6 @@ def main():
             t_tma = timed(lambda: gemm_put(a, b, c, 0, out_dtype=torch.bfloat16, epilogue="tma"), comm, dev)
             row["gemm_tflops_tma_epilogue"] = flops / t_tma / 1e9
             row["max_abs_diff_tma_epilogue_vs_cublas"] = float((c.float() - c_ref.float()).abs().max())
-        if True:  # 2-SM UMMA variant (cta_group::2)
-            t_2sm = timed(lambda: gemm_put(a, b, c, 0, out_dtype=torch.bfloat16, cluster=3), comm, dev)
-            row["gemm_tflops_2sm"] = flops / t_2sm / 1e9
-            t_2sm_tma = timed(lambda: gemm_put(a, b, c, 0, out_dtype=torch.bfloat16, cluster=3, epilogue="tma"), comm, dev)
-            row["gemm_tflops_2sm_tma_epilogue"] = flops / t_2sm_tma / 1e9
-            row["max_abs_diff_2sm_vs_cublas"] = float((c.float() - c_ref.float()).abs().max())
         epoch = [0]
 
         def fused():

@@ -30,13 +30,14 @@ def main() -> int:
     dev = comm.device
     torch.cuda.set_device(dev)
     points = [("memcpy", "ldst", {})]
-    tma = [(c, kb, st) for c, kb, st in itertools.product((148, 296, 592), (8, 16, 32, 64), (2, 4, 8))
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    tma = [(c, kb, st) for c, kb, st in itertools.product((sms, 2 * sms, 4 * sms), (8, 16, 32, 64), (2, 4, 8))
            if kb * st <= 224 and (not args.quick or (kb, st) in ((16, 8), (32, 4), (64, 2), (8, 8)))]
     for transport in ("put", "get"):
         for c, kb, st in tma:
             points.append((transport, "tma", {"ctas": c, "stage_kb": kb, "stages": st}))
-        for c, u, vec, thr in itertools.product((296, 592), (4, 8), (16, 32), (512, 1024)):
-            if args.quick and not (c == 296 and thr == 512):
+        for c, u, vec, thr in itertools.product((2 * sms, 4 * sms), (4, 8), (16, 32), (512, 1024)):
+            if args.quick and not (c == 2 * sms and thr == 512):
                 continue
             points.append((transport, "ldst", {"ctas": c, "unroll": u, "vec_bytes": vec, "threads": thr}))
     if args.hybrid:

@@ -10,7 +10,7 @@ work=$(mktemp -d tmp-cuda-XXXX); cd "$work" || exit 1
 rm -f cuda.log
 
 LCOMMANDS=("C C" "C M2D" "C D2M" "M2D D2M" "H2D D2H")
-EXTRA=("C D2P" "D2P P2D" "A H2D")          # new on B200: peer-GPU copies, stream-triad compute
+EXTRA=("C D2P" "D2P P2D" "A H2D")          # beyond the reference: peer-GPU copies, stream-triad compute
 MODES=(${HPCP_CUDA_MODES:-out_of_order in_order host_threads nowait fused})
 # HPCP_CUDA_ELEMS shrinks the copies (default: the reference's 1 GB); without a GPU the binary falls back to
 # its CPU backend, which only has host_threads / nowait (HPCP_CUDA_MODES="host_threads nowait").

@@ -33,7 +33,7 @@ if [ "${SANITIZE_CLI:-0}" = 1 ]; then
   for san in thread "address,-fsanitize=undefined"; do
     tag=${san%%,*}
     for prog in miniapps/allreduce miniapps/halo p2p/peer2pear; do
-      nvcc -ccbin $CXX -gencode arch=compute_100a,code=sm_100a -O1 -g -std=c++17 -Xcompiler -fopenmp,-fsanitize=$san \
+      nvcc -ccbin $CXX -gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17 -Xcompiler -fopenmp,-fsanitize=$san \
            -Icsrc csrc/$prog.cu build/libhpcp.a -o "$out/$(basename $prog)_$tag" -lgomp
     done
     ASAN_OPTIONS=protect_shadow_gap=0 "$out/allreduce_$tag" --cpu -n 6 -p 14 >> "$out/cli.log" 2>&1

@@ -21,7 +21,7 @@ except ImportError:  # hypothesis is optional for the GPU box
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs at least one CUDA GPU (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs at least one CUDA GPU (run with -m gpu on an H100)")
 
 
 def _gpu_count() -> int:
@@ -43,7 +43,7 @@ def native():
     import hpc_patterns_b200
 
     if not hpc_patterns_b200.native_available():
-        # Build in-tree once (CPU box: nvcc cross-compiles sm_100a without a GPU).
+        # Build in-tree once (CPU box: nvcc cross-compiles sm_90a without a GPU).
         from hpc_patterns_b200 import _build
 
         _build.build(cli=True)

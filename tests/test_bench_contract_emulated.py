@@ -25,14 +25,15 @@ def _load_bench():
 
 
 @pytest.mark.parametrize("extras", [False, True])
-def test_bench_line_has_the_contract_keys(emu, monkeypatch, capsys, extras):  # noqa: F811
+def test_bench_line_has_the_contract_keys(emu, monkeypatch, capsys, tmp_path, extras):  # noqa: F811
     monkeypatch.setattr(torch.cuda, "is_available", lambda: True)
     monkeypatch.setattr(torch.cuda, "Event", TickingEvent)
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "HPCP_DEVICE"):
         monkeypatch.delenv(k, raising=False)
     msg, steps = 8192, 4
     argv = ["bench.py", "--gpus", "1", "--steps", str(steps), "--warmup", "3", "--bytes", str(msg), "--tile-kb", "1",
-            "--preheat-ms", "1", "--blocks", "3", "--e2e-steps", "2"] + ([] if extras else ["--no-extras"])
+            "--preheat-ms", "1", "--blocks", "3", "--e2e-steps", "2", "--dump-outputs", str(tmp_path / "out")] + \
+        ([] if extras else ["--no-extras"])
     monkeypatch.setattr(sys, "argv", argv)
     bench = _load_bench()
     monkeypatch.setattr(bench, "cpu_concurency", lambda impl: {"impl": impl, "stub": True})
@@ -69,6 +70,16 @@ def test_bench_line_has_the_contract_keys(emu, monkeypatch, capsys, extras):  # 
         assert "legacy_triad_ring_put" in d or "legacy_error" in d
     else:
         assert "stock" not in d and "cpu_concurency" not in d
+    # --dump-outputs: the field after one block of `steps` steps from the initial field, at the sampled positions
+    import numpy as np
+
+    from hpc_patterns_b200.models.halo import initial_field, reference_steps
+
+    got = np.load(tmp_path / "out" / "field_rank0.npy")
+    idx = np.load(tmp_path / "out" / "field_index.npy")
+    assert got.dtype == np.float32 and idx.dtype == np.float64 and got.shape == idx.shape
+    want = reference_steps(initial_field(1, cfg["rows"], msg // 4), steps).reshape(-1).numpy()
+    assert np.array_equal(got, want[idx.astype(np.int64)])
     assert not emu.live, "bench.py returned every allocation"
 
 

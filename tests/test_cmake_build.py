@@ -1,5 +1,5 @@
 """The CMake front end (↔ aurora.mpich.miniapps/src/CMakeLists.txt): configure, build every target for
-sm_100a, and run the ctest cases that need no GPU (native unit tests, --cpu plumbing paths, host bench)."""
+sm_90a, and run the ctest cases that need no GPU (native unit tests, --cpu plumbing paths, host bench)."""
 import os
 import shutil
 import subprocess

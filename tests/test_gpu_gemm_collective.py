@@ -1,10 +1,8 @@
 """GPU tests of the two GEMM kernels that carry their collective (csrc/kernels/gemm_collective.cu).
 
-First run on a B200 in round 2 (profiles/r2_call2_1gpu/pytest_gemm_collective.txt: 60 passed), part of the regular
-GPU suite since.  One-GPU tests emulate P ranks with P launches on the
+One-GPU tests emulate P ranks with P launches on the
 same device ("virtual ranks": every rank's shard / row block is a separate buffer, peer pointers are plain local
 pointers), which exercises the whole tile order, ownership, gather and signalling logic without NVLink.
-``cluster=3`` cases run the same policies on the 2-SM UMMA tile loop (``tcgen05.mma.cta_group::2``).
 """
 import os
 import subprocess
@@ -38,8 +36,8 @@ def _dyadic(shape, dev, seed):
 
 @pytest.mark.parametrize("world,m,n,k,cluster", [(1, 256, 256, 64, 1), (2, 512, 512, 256, 1), (2, 1024, 512, 128, 2),
                                                  (4, 2048, 1024, 256, 0), (8, 2048, 768, 512, 0),
-                                                 (4, 8192, 2048, 256, 0), (2, 1024, 512, 128, 3),
-                                                 (4, 4096, 1024, 512, 3)])
+                                                 (4, 8192, 2048, 256, 0), (2, 2048, 512, 128, 2),
+                                                 (4, 4096, 1024, 512, 2)])
 @pytest.mark.parametrize("epilogue", ["red", "tma"])
 def test_gemm_reduce_scatter_virtual_ranks(native, dev, world, m, n, k, cluster, epilogue):
     """Every virtual rank adds its partial product into the owners' shards; the shards must hold the exact sum
@@ -58,8 +56,7 @@ def test_gemm_reduce_scatter_virtual_ranks(native, dev, world, m, n, k, cluster,
             done = [pads[q].data_ptr() + 4 * (native.PAD_DONE + r) for q in range(world)]
             ctas = gemm_reduce_scatter(a[r], b[r], shards, r, done_flags=done, done_epoch=epoch,
                                        ticket=pads[r].data_ptr() + 4 * native.PAD_LOCAL, ticket_base=issued[r],
-                                       cluster=cluster, ctas=0 if epoch == 1 else 6,
-                                       epilogue=epilogue if cluster != 3 else "red")
+                                       cluster=cluster, ctas=0 if epoch == 1 else 6, epilogue=epilogue)
             issued[r] += ctas
         for q in range(world):
             native.wait_flags(pads[q].data_ptr() + 4 * native.PAD_DONE, world, epoch, int(5e9), 0,
@@ -73,7 +70,7 @@ def test_gemm_reduce_scatter_virtual_ranks(native, dev, world, m, n, k, cluster,
 
 
 @pytest.mark.parametrize("m,n,k,cluster", [(128, 256, 64, 1), (512, 768, 256, 1), (2048, 1024, 512, 0), (1024, 512, 128, 2),
-                                           (1024, 1024, 256, 3)])
+                                           (1024, 1024, 256, 2)])
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
 def test_gemm_put_tma_store_epilogue(native, dev, m, n, k, cluster, out_dtype):
     """gemm_put with the C tile leaving through the TMA unit (swizzled smem pieces + UTMASTG) instead of st.global:
@@ -138,7 +135,7 @@ def test_gemm_all_to_all_virtual_ranks(native, dev, world, m, n, k, cluster, out
 @pytest.mark.parametrize("world,m,n,k,cluster,chunk", [(1, 256, 256, 64, 1, 0), (2, 512, 256, 128, 1, 0),
                                                        (2, 1024, 512, 256, 2, 2048), (4, 2048, 512, 512, 0, 0),
                                                        (8, 2048, 256, 1024, 0, 1024), (4, 4096, 1024, 2048, 0, 4096),
-                                                       (2, 1024, 512, 256, 3, 0), (4, 4096, 512, 1024, 3, 2048)])
+                                                       (2, 2048, 512, 256, 2, 0), (4, 4096, 512, 1024, 2, 2048)])
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
 def test_allgather_gemm_virtual_ranks(native, dev, world, m, n, k, cluster, chunk, out_dtype):
     """Every virtual rank gathers the other ranks' row blocks while it multiplies; its C must equal the product

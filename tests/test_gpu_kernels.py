@@ -1,4 +1,4 @@
-"""Single-GPU numerics tests: every sm_100a kernel against a plain PyTorch reference."""
+"""Single-GPU numerics tests: every sm_90a kernel against a plain PyTorch reference."""
 
 import pytest
 import torch
@@ -319,7 +319,7 @@ def test_smoke_entry():
 @pytest.mark.parametrize("cluster", [1, 2])
 @pytest.mark.parametrize("tripcount,ctas", [(1, 2), (3, 6), (100, 148)])
 def test_tcgen05_tile_loop_matches_reference(native, dev, tripcount, ctas, cluster):
-    """T command: out[cta] = tripcount * (A . B^T) with bf16 operands, fp32 TMEM accumulation."""
+    """T command: out[cta] = tripcount * (A . B^T) with bf16 operands, fp32 register accumulation (wgmma)."""
     ops = torch.zeros(native.tc_busy_operand_bytes() // 2, dtype=torch.bfloat16, device=dev)
     per = native.tc_busy_out_elems_per_cta()
     out = torch.full((ctas * per,), float("nan"), device=dev)
@@ -338,23 +338,24 @@ def test_tcgen05_tile_loop_matches_reference(native, dev, tripcount, ctas, clust
 
 def test_tcgen05_duration_scales_with_tripcount(native, dev):
     ops = torch.zeros(native.tc_busy_operand_bytes() // 2, dtype=torch.bfloat16, device=dev)
-    out = torch.zeros(148 * native.tc_busy_out_elems_per_cta(), device=dev)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    out = torch.zeros(sms * native.tc_busy_out_elems_per_cta(), device=dev)
     native.tc_fill_operands(ops.data_ptr(), _stream())
 
     def run(tc):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        native.tc_busy(ops.data_ptr(), out.data_ptr(), 148, tc, _stream())
+        native.tc_busy(ops.data_ptr(), out.data_ptr(), sms, tc, _stream())
         torch.cuda.synchronize()
         e0.record()
-        native.tc_busy(ops.data_ptr(), out.data_ptr(), 148, tc, _stream())
+        native.tc_busy(ops.data_ptr(), out.data_ptr(), sms, tc, _stream())
         e1.record()
         torch.cuda.synchronize()
         return e0.elapsed_time(e1)
 
     t1, t2 = run(20000), run(40000)
     assert 1.6 < t2 / t1 < 2.4, (t1, t2)
-    flops = 148 * 40000 * 2.0 * 128 * 256 * 64
-    print(f"tcgen05 tile loop: {flops / (t2 * 1e-3) / 1e12:.0f} TFLOP/s bf16 over 148 CTAs")
+    flops = sms * 40000 * 2.0 * 128 * 256 * 64
+    print(f"wgmma tile loop: {flops / (t2 * 1e-3) / 1e12:.0f} TFLOP/s bf16 over {sms} CTAs")
 
 
 def test_concurency_tensor_command(native):
@@ -368,7 +369,7 @@ def test_concurency_tensor_command(native):
 @pytest.mark.parametrize("m,n,k", [(128, 256, 64), (256, 512, 256), (1024, 1024, 512), (384, 768, 4096),
                                    (2048, 2048, 1024), (1280, 512, 192)])
 def test_gemm_put_matches_fp32_reference(native, dev, m, n, k, cluster):
-    """tcgen05 GEMM (TMA ring, TMEM accumulators) vs a plain PyTorch fp32 matmul; loop-back 'peer'."""
+    """wgmma GEMM (TMA ring, register accumulators) vs a plain PyTorch fp32 matmul; loop-back 'peer'."""
     from hpc_patterns_b200.ops.gemm import gemm_put, gemm_reference
 
     torch.manual_seed(m + n + k)
@@ -419,10 +420,9 @@ def test_gemm_put_signal_and_few_ctas(native, dev):
 
 @pytest.mark.parametrize("m,n,k", [(256, 256, 64), (256, 512, 256), (1024, 1024, 512), (2048, 2048, 1024),
                                    (512, 768, 4096), (8192, 8192, 512)])
-def test_gemm_put_2sm_umma(native, dev, m, n, k):
-    """tcgen05.mma.cta_group::2, one 256x256 tile per CTA pair (`cluster=3`): exact against the fp32 reference (inputs
-    are multiples of 1/4, sums are exact).  Written without GPU access in round 1, first run in round 2 (6/6 exact, then
-    2x faster after the barrier fix: profiles/r2_call6_1gpu -> r2_call7_1gpu)."""
+def test_gemm_put_cta_pairs_exact(native, dev, m, n, k):
+    """CTA pairs sharing the B tile through TMA multicast (`cluster=2`): exact against the fp32 reference (inputs are
+    multiples of 1/4, sums are exact), local and 'peer' copy, fp32 and bf16 output."""
     from hpc_patterns_b200.ops.gemm import gemm_put, gemm_reference
 
     torch.manual_seed(m + n + k)
@@ -430,14 +430,14 @@ def test_gemm_put_2sm_umma(native, dev, m, n, k):
     b = (torch.randint(-4, 5, (n, k), device=dev).float() / 4).to(torch.bfloat16)
     c_local = torch.full((m, n), float("nan"), device=dev)
     c_peer = torch.full((m, n), float("nan"), device=dev)
-    ctas = gemm_put(a, b, c_local, c_peer, cluster=3)
+    ctas = gemm_put(a, b, c_local, c_peer, cluster=2)
     torch.cuda.synchronize()
     ref = gemm_reference(a, b)
     assert ctas >= 2 and ctas % 2 == 0
     assert torch.equal(c_local, ref), float((c_local - ref).abs().max())
     assert torch.equal(c_peer, c_local)
     c_bf = torch.zeros(m, n, device=dev, dtype=torch.bfloat16)
-    gemm_put(a, b, c_bf, 0, out_dtype=torch.bfloat16, cluster=3, ctas=6)   # several tiles per pair
+    gemm_put(a, b, c_bf, 0, out_dtype=torch.bfloat16, cluster=2, ctas=6)   # several tiles per pair
     torch.cuda.synchronize()
     assert torch.equal(c_bf, ref.to(torch.bfloat16))
 

@@ -1,4 +1,4 @@
-"""Multi-GPU tests (>= 2 B200): native CLIs (thread-per-rank) and torchrun workers (process-per-rank)."""
+"""Multi-GPU tests (>= 2 H100): native CLIs (thread-per-rank) and torchrun workers (process-per-rank)."""
 import json
 import os
 import subprocess
@@ -212,8 +212,8 @@ def test_cli_allreduce_ring_variants_every_type_class(bin_dir, variant, type_):
                                      (6, "uchar")])
 def test_cli_two_shot_remaining_type_classes(bin_dir, n, type_):
     """Two-shot for the (world bucket, add class) pairs the other tests do not reach, as thread-ranks on one GPU.
-    (More than 8 ranks on ONE GPU time out in the device barrier — 12 and 16 tried, profiles/r2_call14_2gpu: the
-    spinning kernels of ranks that share a hardware queue serialise — so the 16-wide instantiation stays unvalidated.)"""
+    (More than 8 ranks on ONE GPU time out in the device barrier: the spinning kernels of ranks that share a hardware
+    queue serialise — so the 16-wide instantiation stays unvalidated.)"""
     rc, out, err = _run([os.path.join(bin_dir, "allreduce"), "-n", str(n), "-p", "16", "--iters", "2", "-a", "--coll",
                          "twoshot", "--type", type_], env={"CUDA_VISIBLE_DEVICES": "0"}, timeout=180)
     assert rc == 0, out + err

@@ -174,7 +174,7 @@ def test_bench_line_at_two_ranks(extras, port):
     assert d["value"] == pytest.approx(2 * 2 * 65536 / (d["ms_per_step"] * 1e-3) / 1e9, abs=0.006)
     roof = d["roofline"]
     assert roof["nvlink_ms"] > 0 and roof["bound_ms"] == max(roof["hbm_ms"], roof["nvlink_ms"])
-    assert d["frac_of_nvlink_900_nominal"] is not None and d["per_gpu_per_direction_GBps"] > 0
+    assert d["frac_of_nvlink_450_nominal"] is not None and d["per_gpu_per_direction_GBps"] > 0
     if extras:
         assert d["stock"]["wrong_words"] == 0
         assert d["stock"]["nccl_sendrecv_ms"] is not None or "nccl_error" in d

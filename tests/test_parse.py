@@ -68,10 +68,9 @@ def test_report_tables(tmp_path):
     p = tmp_path / "rows.jsonl"
     p.write_text("\n".join(json.dumps(r) for r in rows) + "\nnot json\n")
     text = report.render(report.load_rows([str(p)]))
-    assert "| 0.50 | 0.43 |" in text          # 385 / 770 and 385 / 900
-    assert "| 1.00 | 0.86 |" in text          # 770 / 770 and 770 / 900
+    assert "| 700.0 | 0.86 |" in text         # 385 / 450 per direction
+    assert "| 770.0 | 1.71 |" in text         # 770 / 450
     assert "95%" in text and "SUCCESS" in text
-    assert report.measured_hbm_gbps(str(tmp_path)) == report.HBM_FALLBACK_GBPS
 
 
 def test_clock_sampler_without_a_driver_reports_no_samples():
@@ -113,17 +112,17 @@ def test_report_renders_tensor_parallel_and_gemm_rows(tmp_path):
              "row_parallel": {"fused_ms": 0.4, "stock_ms": 0.8, "speedup": 2.0},
              "row_parallel_allreduce": {"unavailable": "no multicast"},
              "column_parallel": {"fused_ms": 0.35, "stock_ms": 0.5, "speedup": 1.43}},
-            {"m": 8192, "n": 8192, "k": 4096, "ranks": 2, "gemm_tflops": 1486.0, "gemm_tflops_2sm": 1600.0,
+            {"m": 8192, "n": 8192, "k": 4096, "ranks": 2, "gemm_tflops": 1486.0,
              "cublas_tflops": 1662.0, "fused_gemm_put_ms": 0.401, "stock_cublas_then_memcpy_ms": 0.514}]
     p = tmp_path / "rows.jsonl"
     p.write_text("\n".join(json.dumps(r) for r in rows))
     text = report.render(report.load_rows([str(p)]))
-    assert "## tensor-parallel layers" in text and "## tcgen05 GEMM" in text
+    assert "## tensor-parallel layers" in text and "## tensor-core GEMM" in text
     line = [ln for ln in text.splitlines() if ln.startswith("| row_parallel (chunk 2048)")][0]
     cells = [c.strip() for c in line.split("|")]
     assert cells[2:6] == ["8", "8192", "8192", "28672"] and cells[8] == "2.00"
     assert "row_parallel_allreduce" not in text                      # unavailable rows are skipped
-    assert "| 8192 | 8192 | 4096 | 2 | 1486 | 1600 | 1662 |" in text
+    assert "| 8192 | 8192 | 4096 | 2 | 1486 | 1662 | 1.50 |" in text     # 1486 / 989
 
 
 def test_clock_sampler_nvml_thread_with_a_fake_driver(monkeypatch):

@@ -1,46 +1,86 @@
-"""Drop-in parity against the REAL reference program, where it can be built here.
+"""Drop-in parity against the REAL reference program.
 
 The reference's OpenMP backend (concurency/bench_omp.cpp + main.cpp) compiles with plain ``g++ -fopenmp``
 (target regions fall back to the host) once the Intel-only ``omp_target_alloc_host`` is mapped to
-``omp_target_alloc`` on the command line — the sources are used unmodified, straight from the read-only
-mount.  That gives a ground truth for the stdout contract (SURVEY.md §2.2-A):
+``omp_target_alloc`` on the command line.  That gives a ground truth for the stdout contract:
 
 * our binary and the reference binary print the same sequence of line shapes for the same arguments;
-* the reference's own ``parse.py`` turns OUR log into the same table our parser renders, and vice versa.
+* the reference's own ``parse.py`` turns logs into the same tables our parser renders.
 
-Skipped when the reference tree is not mounted (e.g. on the GPU box).
+What the reference printed for every command line and log used here is stored in tests/golden/reference_parity.json.gz,
+so the comparison runs anywhere.  ``HPCP_REFERENCE_RECORD=<reference tree> pytest tests/test_reference_parity.py``
+runs the reference itself instead and rewrites that file.
 """
+import gzip
+import hashlib
+import json
 import os
 import re
-import shutil
 import subprocess
 import sys
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("HPCP_REFERENCE", "/root/reference")
-REF_CON = os.path.join(REF, "concurency")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_parity.json.gz")
+RECORD = os.environ.get("HPCP_REFERENCE_RECORD")
 
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF_CON, "bench_omp.cpp")),
-                                reason="reference tree not mounted")
+
+class Reference:
+    """The reference's answers: looked up in the golden file, or (record mode) computed by the real programs."""
+
+    def __init__(self, tmp):
+        self.data = {"run": {}, "parse": {}, "log": {}}
+        if RECORD:
+            from oracle import build_ref
+
+            self.parse_py = os.path.join(RECORD, "concurency", "parse.py")
+            self.bins = build_ref.build(RECORD, str(tmp))
+            assert set(self.bins) == set(build_ref.MODES), "the reference's OpenMP bench does not build"
+        else:
+            with gzip.open(GOLDEN, "rt") as f:
+                self.data = json.load(f)
+
+    def _get(self, table, key, compute):
+        if RECORD:
+            self.data[table][key] = compute()
+        assert key in self.data[table], f"no stored reference answer for {key!r}: rerun with HPCP_REFERENCE_RECORD"
+        return self.data[table][key]
+
+    def run(self, binary, argv):
+        """Exit status and stdout of the reference program built as `binary` (host_threads or nowait)."""
+        def compute():
+            p = subprocess.run([self.bins[binary]] + argv, capture_output=True, text=True, timeout=300)
+            return {"returncode": p.returncode, "stdout": p.stdout}
+        return self._get("run", json.dumps([binary] + argv), compute)
+
+    def parse(self, text, *args):
+        """stdout of the reference's parse.py on a log with this text."""
+        def compute():
+            path = os.path.join(os.path.dirname(self.bins["nowait"]), f"log{len(self.data['parse'])}.log")
+            with open(path, "w") as f:
+                f.write(text)
+            p = subprocess.run([sys.executable, self.parse_py, path, *args], capture_output=True, text=True, timeout=60)
+            assert p.returncode == 0, p.stderr
+            return p.stdout
+        return self._get("parse", hashlib.sha256(json.dumps([text, *args]).encode()).hexdigest(), compute)
+
+    def log(self, name, compute):
+        """A log recorded together with the reference's answers (its numbers are timings)."""
+        return self._get("log", name, compute)
+
+    def save(self):
+        os.makedirs(os.path.dirname(GOLDEN), exist_ok=True)
+        with open(GOLDEN, "wb") as raw, gzip.GzipFile(fileobj=raw, mode="wb", mtime=0) as f:
+            f.write((json.dumps(self.data, indent=0, sort_keys=True) + "\n").encode())
 
 
 @pytest.fixture(scope="module")
-def ref_bins(tmp_path_factory):
-    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-    out = tmp_path_factory.mktemp("refomp")
-    bins = {}
-    for mode, flag in (("host_threads", "HOST_THREADS"), ("nowait", "NOWAIT")):
-        exe = out / f"omp_{mode}"
-        p = subprocess.run([cxx, "-O2", "-std=c++17", "-fopenmp", f"-D{flag}",
-                            "-Domp_target_alloc_host=omp_target_alloc",      # Intel extension -> standard call
-                            os.path.join(REF_CON, "main.cpp"), os.path.join(REF_CON, "bench_omp.cpp"), "-o", str(exe)],
-                           capture_output=True, text=True, timeout=600)
-        if p.returncode != 0:
-            pytest.skip("the reference's OpenMP bench does not build with this g++: " + p.stderr[-300:])
-        bins[mode] = str(exe)
-    return bins
+def ref(tmp_path_factory):
+    r = Reference(tmp_path_factory.mktemp("refomp"))
+    yield r
+    if RECORD:
+        r.save()
 
 
 def _shape(text: str):
@@ -64,50 +104,55 @@ ARGS = ["--tripcount_C", "3000", "--commands", "C", "C"]
 @pytest.mark.parametrize("extra", [[], ["--verbose", "--repetitions", "3"], ["--min_bandwidth", "100000"],
                                    ["--queues", "1", "--verbose", "--repetitions", "2"]])
 @pytest.mark.parametrize("mode", ["host_threads", "nowait"])
-def test_same_stdout_shape_as_the_reference_binary(ref_bins, bin_dir, mode, extra):
-    ref = subprocess.run([ref_bins[mode], mode] + extra + ARGS, capture_output=True, text=True, timeout=300)
+def test_same_stdout_shape_as_the_reference_binary(ref, bin_dir, mode, extra):
+    theirs = ref.run(mode, [mode] + extra + ARGS)
     ours = subprocess.run([os.path.join(bin_dir, "omp_con"), mode] + extra + ARGS, capture_output=True, text=True,
                           timeout=300)
-    assert "## " + mode + " | C C | " in ref.stdout, ref.stdout + ref.stderr
-    assert _shape(ours.stdout) == _shape(ref.stdout)
-    assert ref.returncode in (0, 1) and ours.returncode in (0, 1)      # 1 = some group FAILED (same rule)
+    assert "## " + mode + " | C C | " in theirs["stdout"], theirs["stdout"]
+    assert _shape(ours.stdout) == _shape(theirs["stdout"])
+    assert theirs["returncode"] in (0, 1) and ours.returncode in (0, 1)      # 1 = some group FAILED (same rule)
 
 
-def test_usage_and_exit_status_match(ref_bins, bin_dir):
-    ref = subprocess.run([ref_bins["nowait"]], capture_output=True, text=True)
+def test_usage_and_exit_status_match(ref, bin_dir):
+    theirs = ref.run("nowait", [])
     ours = subprocess.run([os.path.join(bin_dir, "omp_con")], capture_output=True, text=True)
-    assert ref.returncode == ours.returncode == 1
+    assert theirs["returncode"] == ours.returncode == 1
     for flag in ("--commands", "--repetitions", "--min_bandwidth", "--queues", "--enable_profiling"):
-        assert flag in ref.stdout and flag in ours.stdout
+        assert flag in theirs["stdout"] and flag in ours.stdout
     for bad in (["bogus_mode", "--commands", "C", "C"], ["nowait", "--bogus"], ["nowait", "--commands", "C", "X"]):
-        r = subprocess.run([ref_bins["nowait"]] + bad, capture_output=True, text=True)
+        r = ref.run("nowait", bad)
         o = subprocess.run([os.path.join(bin_dir, "omp_con")] + bad, capture_output=True, text=True)
-        assert r.returncode == o.returncode == 1
-        assert r.stdout.splitlines()[0] == o.stdout.splitlines()[0]          # same ERROR line, then the usage text
-        assert r.stdout.splitlines()[0].startswith("ERROR: ")
-    bad_ref = subprocess.run([ref_bins["nowait"], "nowait", "--commands", "C", "H2M"], capture_output=True, text=True)
+        assert r["returncode"] == o.returncode == 1
+        assert r["stdout"].splitlines()[0] == o.stdout.splitlines()[0]          # same ERROR line, then the usage text
+        assert r["stdout"].splitlines()[0].startswith("ERROR: ")
+    bad_ref = ref.run("nowait", ["nowait", "--commands", "C", "H2M"])
     bad_ours = subprocess.run([os.path.join(bin_dir, "omp_con"), "nowait", "--commands", "C", "H2M"],
                               capture_output=True, text=True)
-    assert bad_ref.returncode == bad_ours.returncode == 1              # HM / MH are rejected by both
+    assert bad_ref["returncode"] == bad_ours.returncode == 1              # HM / MH are rejected by both
 
 
-def test_parsers_are_interchangeable(ref_bins, bin_dir, tmp_path):
-    logs = {}
-    for who, exe in (("ref", None), ("ours", os.path.join(bin_dir, "omp_con"))):
+def test_parsers_are_interchangeable(ref, bin_dir, tmp_path):
+    """A log of the reference binary and a log of ours (both recorded with the reference's answers: their numbers are
+    timings) render the same through the reference's parse.py and ours."""
+    def record(who):
         text = "+ export OMP_PROC_BIND=false\n"
         for mode in ("nowait", "host_threads"):
-            p = subprocess.run([exe or ref_bins[mode], mode] + ARGS, capture_output=True, text=True, timeout=300)
-            text += p.stdout
-        path = tmp_path / f"{who}.log"
-        path.write_text(text)
-        logs[who] = str(path)
+            if who == "ref":
+                text += ref.run(mode, [mode] + ARGS)["stdout"]
+            else:
+                text += subprocess.run([os.path.join(bin_dir, "omp_con"), mode] + ARGS, capture_output=True, text=True,
+                                       timeout=300).stdout
+        return text
     env = dict(os.environ, PYTHONPATH=ROOT)
-    for log in logs.values():
-        theirs = subprocess.run([sys.executable, os.path.join(REF_CON, "parse.py"), log], capture_output=True, text=True)
-        mine = subprocess.run([sys.executable, "-m", "hpc_patterns_b200.utils.parse", log], capture_output=True,
+    for who in ("ref", "ours"):
+        text = ref.log(who, lambda: record(who))
+        log = tmp_path / f"{who}.log"
+        log.write_text(text)
+        theirs = ref.parse(text)
+        mine = subprocess.run([sys.executable, "-m", "hpc_patterns_b200.utils.parse", str(log)], capture_output=True,
                               text=True, env=env)
-        assert theirs.returncode == 0 and mine.returncode == 0, theirs.stderr + mine.stderr
-        assert mine.stdout == theirs.stdout and "OMP_PROC_BIND=false" in mine.stdout
+        assert mine.returncode == 0, mine.stderr
+        assert mine.stdout == theirs and "OMP_PROC_BIND=false" in mine.stdout
 
 
 # ------------------------------------------------------------------------------------------------ differential fuzz ----
@@ -126,7 +171,7 @@ _flags = st.lists(st.sampled_from([["--verbose"], ["--enable_profiling"], ["--qu
 
 @given(groups=_groups, flags=_flags, mode=st.sampled_from(["nowait", "host_threads", "serial", "in_order", ""]))
 @settings(max_examples=60, deadline=None, derandomize=True, suppress_health_check=[HealthCheck.function_scoped_fixture])
-def test_random_command_lines_behave_like_the_reference(ref_bins, bin_dir, groups, flags, mode):
+def test_random_command_lines_behave_like_the_reference(ref, bin_dir, groups, flags, mode):
     """Random argv (valid and invalid) through the reference binary and ours: same exit status, same usage-or-run
     decision, same sequence of line shapes.  Sizes are tiny, the verdict text itself is normalised away.
     (derandomize: the suite runs the same 60 command lines every time; drop the flag locally to explore other seeds; 8 x 60 more were run when this was written.)"""
@@ -138,19 +183,20 @@ def test_random_command_lines_behave_like_the_reference(ref_bins, bin_dir, group
         argv += ["--globalsize_" + cmd, "2000"]
     for g in groups:
         argv += ["--commands"] + list(g)
-    ref = subprocess.run([ref_bins.get(mode, ref_bins["nowait"])] + argv, capture_output=True, text=True, timeout=120)
+    r = ref.run(mode if mode in ("nowait", "host_threads") else "nowait", argv)
     ours = subprocess.run([os.path.join(bin_dir, "omp_con")] + argv, capture_output=True, text=True, timeout=120)
-    ref_usage = "--commands" in ref.stdout and "## " not in ref.stdout and ref.returncode == 1
+    ref_rc, ref_out = r["returncode"], r["stdout"]
+    ref_usage = "--commands" in ref_out and "## " not in ref_out and ref_rc == 1
     ours_usage = "--commands" in ours.stdout and "## " not in ours.stdout and ours.returncode == 1
     assert ours.returncode in (0, 1), (argv, ours.returncode, ours.stderr[-300:])                 # we never crash
-    if ref.returncode < 0:
+    if ref_rc < 0:
         # the reference's offload allocator aborts ("Wrong Allocation") for device buffers when g++ has no offload
         # device to fall back to — an artefact of building it for the host; nothing to compare with
         return
-    assert ref_usage == ours_usage, (argv, ref.stdout[-300:], ours.stdout[-300:])
+    assert ref_usage == ours_usage, (argv, ref_out[-300:], ours.stdout[-300:])
     if not ref_usage:
-        assert (ref.returncode in (0, 1)) and (ours.returncode in (0, 1)), (argv, ref.returncode, ours.returncode)
-        assert _shape(ours.stdout) == _shape(ref.stdout), (argv, ref.stdout, ours.stdout)
+        assert (ref_rc in (0, 1)) and (ours.returncode in (0, 1)), (argv, ref_rc, ours.returncode)
+        assert _shape(ours.stdout) == _shape(ref_out), (argv, ref_out, ours.stdout)
 
 
 _modes = st.sampled_from(["nowait", "host_threads", "in_order", "out_of_order", "fused", "serial"])
@@ -170,13 +216,12 @@ _noise = st.sampled_from(["# nowait | C MD | Starting Benchmarking...", "Minimum
 @given(lines=st.lists(st.one_of(_verdict, _verdict, _export, _noise), min_size=0, max_size=25),
        fmt=st.sampled_from(["simple", "github", "plain"]))
 @settings(max_examples=40, deadline=None, derandomize=True, suppress_health_check=[HealthCheck.function_scoped_fixture])
-def test_random_logs_render_like_the_reference_parser(tmp_path, lines, fmt):
+def test_random_logs_render_like_the_reference_parser(ref, tmp_path, lines, fmt):
     """The reference's parse.py and ours print the same tables for any log a sweep script can produce."""
     log = tmp_path / "fuzz.log"
     log.write_text("\n".join(lines) + "\n")
-    theirs = subprocess.run([sys.executable, os.path.join(REF_CON, "parse.py"), str(log), fmt], capture_output=True,
-                            text=True, timeout=60)
+    theirs = ref.parse("\n".join(lines) + "\n", fmt)
     mine = subprocess.run([sys.executable, "-m", "hpc_patterns_b200.utils.parse", str(log), fmt], capture_output=True,
                           text=True, env=dict(os.environ, PYTHONPATH=ROOT), timeout=60)
-    assert theirs.returncode == 0 and mine.returncode == 0, theirs.stderr + mine.stderr
-    assert mine.stdout == theirs.stdout, (lines, theirs.stdout, mine.stdout)
+    assert mine.returncode == 0, mine.stderr
+    assert mine.stdout == theirs, (lines, theirs, mine.stdout)

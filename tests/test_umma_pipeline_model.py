@@ -1,13 +1,16 @@
-"""Executable model of the mbarrier pipelines of the tensor-core tile loops (csrc/kernels/umma.cuh), on the CPU.
+"""Executable model of the mbarrier pipeline of the tensor-core tile loop (csrc/kernels/wgmma.cuh: gemm_persistent),
+on the CPU.
 
-The 2-SM UMMA loop (``gemm_persistent_2sm``) was written without access to a GPU; a protocol error there is a hang.
-This model re-states its barrier protocol — who initialises which barrier with which count, who arrives / expects
-bytes / waits on which parity — with mbarrier semantics (pending arrivals, transaction bytes, phase bit), runs the
-warps of a CTA pair as coroutines under a random scheduler in which every asynchronous completion (TMA bytes landing,
-tcgen05.commit arrivals) is delayed arbitrarily, and checks: no deadlock, no arrival on a barrier whose phase is
-already full, no smem stage refilled before the MMAs that read it were committed, no accumulator overwritten before
-both epilogues drained it.  The CTA-pair multicast loop (``gemm_persistent<2>``, validated on B200) runs through
-the same checker as a control, and mutated protocols (a wrong arrival count, a missing remote arrive) must be caught.
+A protocol error in the tile loop is a hang or silently wrong data.  This model re-states its barrier protocol — who
+initialises which barrier with which count, who arrives / expects bytes / waits on which parity — with mbarrier
+semantics (pending arrivals, transaction bytes, phase bit), runs the producer warp and the two consumer warpgroups of
+each CTA (one CTA, or a pair sharing the B tile by TMA multicast) as coroutines under a random scheduler in which every
+asynchronous completion (TMA bytes landing, wgmma groups retiring) is delayed arbitrarily, and checks: no deadlock,
+no MMA on a stage whose bytes have not all landed, no stage refilled (in either CTA of a pair) while a consumer still
+holds it.  The consumers release a stage after ``wgmma.wait_group 1`` has retired the k-block that read it, with a
+remote ``mbarrier.arrive`` into every CTA of the pair; the empty barriers count 2 x kConsumers arrivals in a pair.
+Mutated protocols (a wrong arrival count, a missing remote arrive, a release before the MMA retired, a short
+transaction count) must be caught.
 """
 import random
 
@@ -70,184 +73,108 @@ def run(agents, pending_events, rng, max_steps=200000):
 
 
 A_BYTES, B_BYTES = 16384, 32768
+CONSUMERS = 2
 
 
-def simulate_2sm(num_items, num_kb, stages, seed, full_count=2, peer_arrives=True, tmem_empty_count=8):
+def simulate_wgmma(num_items, num_kb, stages, seed, cluster=2, empty_count=None, remote_release=True,
+                   release_before_retire=False, expect_bytes=A_BYTES + B_BYTES):
     rng = random.Random(seed)
-    full = [MBar(f"full[{s}]", full_count) for s in range(stages)]                       # leader-owned
-    empty = [[MBar(f"empty[{c}][{s}]", 1) for s in range(stages)] for c in range(2)]     # one set per CTA
-    tmem_full = [[MBar(f"tmem_full[{c}][{a}]", 1) for a in range(2)] for c in range(2)]
-    tmem_empty = [MBar(f"tmem_empty[{a}]", tmem_empty_count) for a in range(2)]           # leader-owned
-    stage_state = [["free"] * stages for _ in range(2)]   # free -> loading -> (full barrier) -> reading -> free
-    acc_state = ["free", "free"]                          # free -> accumulating -> full -> (drained by 8 warps) free
-    acc_readers = [0, 0]
-    tma_q = [[], []]          # per CTA: TMA completions in issue order
-    tc_q = []                 # tensor-core commit arrivals, in issue order (tcgen05.commit tracks all prior MMAs)
-    stage_bytes = A_BYTES + B_BYTES // 2
+    empty_count = CONSUMERS * cluster if empty_count is None else empty_count
+    full = [[MBar(f"full[{c}][{s}]", 1) for s in range(stages)] for c in range(cluster)]
+    empty = [[MBar(f"empty[{c}][{s}]", empty_count) for s in range(stages)] for c in range(cluster)]
+    landed = {}                                        # (cta, stage, fill) -> bytes landed for that fill
+    holders = [[0] * stages for _ in range(cluster)]   # consumers that acquired stage s of cta c and not released it
+    reading = [[0] * stages for _ in range(cluster)]   # issued wgmma groups on stage s of cta c not yet retired
+    tma_q = [[] for _ in range(cluster)]
+    mma_q = [[[] for _ in range(CONSUMERS)] for _ in range(cluster)]   # wgmma groups retire in order, per warpgroup
+    outstanding = [[0] * CONSUMERS for _ in range(cluster)]
 
     def producer(cta):
-        stage, phase = 0, 0
+        stage, phase, t = 0, 0, 0
         for _ in range(num_items):
             for _ in range(num_kb):
                 yield lambda s=stage, p=phase: empty[cta][s].done(p ^ 1)
-                if stage_state[cta][stage] != "free":
-                    raise ProtocolError(f"cta {cta}: stage {stage} refilled while {stage_state[cta][stage]}")
-                stage_state[cta][stage] = "loading"
-                if cta == 0:
-                    full[stage].arrive(expect_tx=2 * stage_bytes)
+                for d in range(cluster):                   # my half of B lands in every CTA of the pair
+                    if holders[d][stage] or reading[d][stage]:
+                        raise ProtocolError(f"cta {cta} refills stage {stage} while cta {d} still uses it")
+                full[cta][stage].arrive(expect_tx=expect_bytes)
+                own_bytes = A_BYTES + (B_BYTES if cluster == 1 else 0)
 
-                def landed(s=stage, c=cta):
-                    stage_state[c][s] = "landed"
-                    full[s].complete_tx(stage_bytes)
+                def own(s=stage, c=cta, n=t // stages, b=own_bytes):
+                    landed[c, s, n] = landed.get((c, s, n), 0) + b
+                    full[c][s].complete_tx(b)
 
-                tma_q[cta].append(landed)
-                if cta == 1 and peer_arrives:
-                    full[stage].arrive()
+                def half_b(s=stage, n=t // stages):
+                    for d in range(cluster):
+                        landed[d, s, n] = landed.get((d, s, n), 0) + B_BYTES // 2
+                        full[d][s].complete_tx(B_BYTES // 2)
+
+                tma_q[cta] += [own] + ([half_b] if cluster > 1 else [])
+                t += 1
                 stage += 1
                 if stage == stages:
                     stage, phase = 0, phase ^ 1
 
-    def mma():
-        stage, phase = 0, 0
-        for item in range(num_items):
-            acc, acc_phase = item & 1, (item >> 1) & 1
-            yield lambda a=acc, p=acc_phase: tmem_empty[a].done(p ^ 1)
-            if acc_state[acc] != "free":
-                raise ProtocolError(f"accumulator {acc} overwritten while {acc_state[acc]}")
-            acc_state[acc] = "accumulating"
-            for kb in range(num_kb):
-                yield lambda s=stage, p=phase: full[s].done(p)
-                for c in range(2):
-                    if stage_state[c][stage] != "landed":
-                        raise ProtocolError(f"MMA reads stage {stage} of cta {c} while {stage_state[c][stage]}")
-                    stage_state[c][stage] = "reading"
+    def release(cta, s):
+        holders[cta][s] -= 1
+        for d in (range(cluster) if remote_release else [cta]):
+            empty[d][s].arrive()
 
-                def stage_free(s=stage):
-                    for c in range(2):
-                        stage_state[c][s] = "free"
-                        empty[c][s].arrive()
-
-                tc_q.append(stage_free)
-                if kb == num_kb - 1:
-                    def acc_full(a=acc):
-                        acc_state[a] = "full"
-                        acc_readers[a] = 8
-                        for c in range(2):
-                            tmem_full[c][a].arrive()
-
-                    tc_q.append(acc_full)
-                stage += 1
-                if stage == stages:
-                    stage, phase = 0, phase ^ 1
-
-    def epilogue(cta, warp):
-        for item in range(num_items):
-            acc, acc_phase = item & 1, (item >> 1) & 1
-            yield lambda a=acc, p=acc_phase: tmem_full[cta][a].done(p)
-            if acc_state[acc] != "full":
-                raise ProtocolError(f"epilogue reads accumulator {acc} while {acc_state[acc]}")
-            yield None  # tcgen05.ld + stores take a while
-            acc_readers[acc] -= 1
-            if acc_readers[acc] == 0:
-                acc_state[acc] = "free"
-            tmem_empty[acc].arrive()
-
-    agents = [producer(0), producer(1), mma()] + [epilogue(c, w) for c in range(2) for w in range(4)]
-    run(agents, tma_q + [tc_q], rng)
-    return True
-
-
-def simulate_pair_multicast(num_items, num_kb, stages, seed):
-    """gemm_persistent<2>: every CTA runs its own MMAs on its own accumulator; B halves are multicast, so a stage of
-    EITHER CTA may only be refilled when BOTH MMAs consumed it (empty count 2, commits multicast to the pair)."""
-    rng = random.Random(seed)
-    full = [[MBar(f"full[{c}][{s}]", 1) for s in range(stages)] for c in range(2)]
-    empty = [[MBar(f"empty[{c}][{s}]", 2) for s in range(stages)] for c in range(2)]
-    tmem_full = [[MBar(f"tmem_full[{c}][{a}]", 1) for a in range(2)] for c in range(2)]
-    tmem_empty = [[MBar(f"tmem_empty[{c}][{a}]", 4) for a in range(2)] for c in range(2)]
-    readers = [[0] * stages for _ in range(2)]      # MMAs that still have to consume stage s of cta c
-    landed = [[0] * stages for _ in range(2)]
-    tma_q, tc_q = [[], []], [[], []]
-
-    def producer(cta):
-        stage, phase = 0, 0
+    def consumer(cta, g):
+        stage, phase, t = 0, 0, 0
         for _ in range(num_items):
+            prev = None
             for _ in range(num_kb):
-                yield lambda s=stage, p=phase: empty[cta][s].done(p ^ 1)
-                full[cta][stage].arrive(expect_tx=A_BYTES + B_BYTES)
-
-                def own(s=stage, c=cta):
-                    landed[c][s] += A_BYTES
-                    full[c][s].complete_tx(A_BYTES)
-
-                def half_b(s=stage):
-                    for c in range(2):  # multicast: my half of B lands in both CTAs
-                        if readers[c][s]:
-                            raise ProtocolError(f"multicast into stage {s} of cta {c} while its MMA still reads it")
-                        landed[c][s] += B_BYTES // 2
-                        full[c][s].complete_tx(B_BYTES // 2)
-
-                tma_q[cta] += [own, half_b]
-                stage += 1
-                if stage == stages:
-                    stage, phase = 0, phase ^ 1
-
-    def mma(cta):
-        stage, phase = 0, 0
-        for item in range(num_items):
-            acc, acc_phase = item & 1, (item >> 1) & 1
-            yield lambda a=acc, p=acc_phase: tmem_empty[cta][a].done(p ^ 1)
-            for kb in range(num_kb):
                 yield lambda s=stage, p=phase: full[cta][s].done(p)
-                if landed[cta][stage] != A_BYTES + B_BYTES:
-                    raise ProtocolError(f"cta {cta}: MMA on a stage with {landed[cta][stage]} bytes")
-                readers[cta][stage] = 1
+                got = landed.get((cta, stage, t // stages), 0)
+                if got != A_BYTES + B_BYTES:
+                    raise ProtocolError(f"cta {cta}: MMA on stage {stage} with {got} bytes landed")
+                holders[cta][stage] += 1
+                reading[cta][stage] += 1
+                outstanding[cta][g] += 1
 
-                def consumed(s=stage, c=cta):
-                    readers[c][s] = 0
-                    landed[c][s] = 0
-                    for d in range(2):
-                        empty[d][s].arrive()
+                def retired(c=cta, w=g, s=stage):
+                    outstanding[c][w] -= 1
+                    reading[c][s] -= 1
 
-                tc_q[cta].append(consumed)
-                if kb == num_kb - 1:
-                    tc_q[cta].append(lambda a=acc, c=cta: tmem_full[c][a].arrive())
+                mma_q[cta][g].append(retired)
+                if release_before_retire:
+                    release(cta, stage)
+                    prev = None
+                else:
+                    yield lambda c=cta, w=g: outstanding[c][w] <= 1       # wgmma.wait_group 1
+                    if prev is not None:
+                        release(cta, prev)
+                    prev = stage
+                t += 1
                 stage += 1
                 if stage == stages:
                     stage, phase = 0, phase ^ 1
+            yield lambda c=cta, w=g: outstanding[c][w] == 0               # wgmma.wait_group 0
+            if prev is not None:
+                release(cta, prev)
+            yield None                                                     # the epilogue stores the tile
 
-    def epilogue(cta, warp):
-        for item in range(num_items):
-            acc, acc_phase = item & 1, (item >> 1) & 1
-            yield lambda a=acc, p=acc_phase: tmem_full[cta][a].done(p)
-            yield None
-            tmem_empty[cta][acc].arrive()
-
-    agents = [producer(0), producer(1), mma(0), mma(1)] + [epilogue(c, w) for c in range(2) for w in range(4)]
-    run(agents, tma_q + tc_q, rng)
+    agents = [producer(c) for c in range(cluster)] + [consumer(c, g) for c in range(cluster) for g in range(CONSUMERS)]
+    run(agents, tma_q + [q for per_cta in mma_q for q in per_cta], rng)
     return True
 
 
+@pytest.mark.parametrize("cluster", [1, 2])
 @pytest.mark.parametrize("num_items,num_kb", [(1, 1), (1, 7), (2, 3), (3, 6), (5, 13), (4, 1)])
-def test_two_sm_pipeline_has_no_deadlock_and_no_hazard(num_items, num_kb):
+def test_wgmma_pipeline_has_no_deadlock_and_no_hazard(num_items, num_kb, cluster):
     for seed in range(25):
-        assert simulate_2sm(num_items, num_kb, stages=6, seed=seed)
+        assert simulate_wgmma(num_items, num_kb, stages=4, seed=seed, cluster=cluster)
 
 
-@pytest.mark.parametrize("num_items,num_kb", [(1, 1), (2, 5), (5, 9)])
-def test_validated_pair_multicast_pipeline_passes_the_same_checker(num_items, num_kb):
-    for seed in range(25):
-        assert simulate_pair_multicast(num_items, num_kb, stages=4, seed=seed)
-
-
-@pytest.mark.parametrize("mutation", [dict(full_count=1), dict(full_count=3), dict(peer_arrives=False),
-                                      dict(tmem_empty_count=4), dict(tmem_empty_count=9)])
+@pytest.mark.parametrize("mutation", [dict(empty_count=2), dict(empty_count=3), dict(remote_release=False),
+                                      dict(release_before_retire=True), dict(expect_bytes=A_BYTES + B_BYTES // 2)])
 def test_checker_catches_broken_protocols(mutation):
     """Not vacuous: each of these one-line protocol errors is reported (as a deadlock or as a hazard)."""
     caught = 0
     for seed in range(40):
         try:
-            simulate_2sm(4, 5, stages=6, seed=seed, **mutation)
+            simulate_wgmma(4, 5, stages=4, seed=seed, **mutation)
         except ProtocolError:
             caught += 1
     assert caught > 0, mutation
