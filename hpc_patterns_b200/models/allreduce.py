@@ -29,6 +29,7 @@ from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
 ALGOS = ("ring", "ring-unfused", "twoshot", "nvls", "nccl", "ring-nccl")
+VIRTUAL_ALGOS = ("ring", "ring-unfused", "twoshot")   # the ones whose peers are plain pointers (no NCCL, no multicast)
 # element types of the reference's datatype trait (mpi_datatype.hpp:28-51) -> the torch dtype whose add is bit-identical
 # (unsigned integers share the two's-complement add of the signed type of the same width; NCCL rows only)
 _TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32, "double": torch.float64,
@@ -66,26 +67,47 @@ class AllreduceResult:
                 "frac_of_450GBps": gbps / 450.0, "mismatches": self.mismatches}
 
 
+def element_count(elem_bytes: int, world: int, log2_elems: int = 25, n_elems: int = 0) -> int:
+    """Elements per rank: ``n_elems`` when given (it must split into 16-byte vectors, one slice per rank), else
+    2^log2_elems rounded up to such a multiple."""
+    unit = 16 // elem_bytes * world
+    if n_elems:
+        if n_elems < 0 or n_elems % unit:
+            raise ValueError(f"n_elems must be a positive multiple of {unit} (16-byte vectors x {world} ranks)")
+        return int(n_elems)
+    n = 1 << log2_elems
+    return -(-n // unit) * unit
+
+
+def ring_layout(nbytes: int, n_chunks: int, world: int, slots_policy: int):
+    """(words after the fixed signal pad, bytes of receive slots) of the fused ring: one arrival word per chunk, then
+    with two slots one ack word per chunk; two blocks of slots with acks, else world-1 blocks."""
+    two = slots_policy == 2
+    return n_chunks * (2 if two else 1), nbytes * (2 if two else max(world - 1, 1))
+
+
 class AllreduceMiniapp:
     def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float",
                  algo: str = "ring", chunk_elems: int = 0, ctas: int = 0, timeout_s: float = 30.0,
-                 slots: int = 0, pull: bool = False):
+                 slots: int = 0, pull: bool = False, n_elems: int = 0, _shared: Optional[dict] = None):
         """``slots=2`` (fused ring only): two receive slots + per-chunk acks — the reference's VA/VB double
         buffer — instead of ``world-1`` slots without flow control.  ``pull=True`` (fused ring only): receiver-driven,
-        every block is loaded from the left neighbour's memory instead of being stored into the right neighbour's."""
+        every block is loaded from the left neighbour's memory instead of being stored into the right neighbour's.
+        ``n_elems``: exact element count per rank instead of 2^log2_elems.  ``_shared``: buffers made by an
+        in-process group (``VirtualAllreduce``): ``pads``, ``va``, ``vc`` and, where the algorithm uses them, ``vb`` and
+        ``slots``."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
         if dtype not in _TORCH_DTYPE:
             raise ValueError(f"dtype must be one of {sorted(_TORCH_DTYPE)}")
+        if _shared is not None and algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
         self.C = native()
         self.comm, self.device = comm, device
         self.rank, self.world = comm.rank, comm.world
         self.algo, self.dtype, self.ctas, self.chunk_elems = algo, dtype, ctas, chunk_elems
         self.esz = self.C.elem_size(dtype)
-        lanes = 16 // self.esz
-        n = 1 << log2_elems
-        if n % (lanes * self.world):
-            n = (n // (lanes * self.world) + 1) * lanes * self.world
+        n = element_count(self.esz, self.world, log2_elems, n_elems)
         self.n, self.nbytes = n, n * self.esz
         self.right, self.left = (self.rank + 1) % self.world, (self.rank - 1) % self.world
         torch.cuda.set_device(device)
@@ -94,26 +116,28 @@ class AllreduceMiniapp:
         self.slots_policy = slots if algo == "ring" else 0
         self.pull = bool(pull) and algo == "ring"
         self.n_chunks = self.C.ring_num_chunks(n, chunk_elems, self.esz)
-        # arrival words, then (two-slot ring) ack words
-        self.pads = SignalPads(comm, device, extra_words=self.n_chunks * (2 if self.slots_policy == 2 else 1),
-                               timeout_s=timeout_s)
         self.ring_epoch = 0
         self.step_epoch = 0
         self.launches = 0
         self.va = self.vb = self.vc = self.slots = None
         self._symm = None
-        if algo == "nvls":
+        pad_words, slot_bytes = ring_layout(self.nbytes, self.n_chunks, self.world, self.slots_policy)
+        if _shared is not None:         # virtual ranks of one process (VirtualAllreduce): buffers made by the group
+            self.pads, self.va, self.vb, self.vc, self.slots = (_shared.get(k) for k in ("pads", "va", "vb", "vc",
+                                                                                          "slots"))
+        elif algo == "nvls":
+            self.pads = SignalPads(comm, device, extra_words=pad_words, timeout_s=timeout_s)
             try:
                 self._init_nvls()
             except Exception:
                 self.pads.close()   # collectively allocated just above: do not leak it on the failure path
                 raise
         else:
+            self.pads = SignalPads(comm, device, extra_words=pad_words, timeout_s=timeout_s)
             self.va = SymmetricBuffer(comm, self.nbytes, device)
             self.vc = SymmetricBuffer(comm, self.nbytes, device)
             if algo == "ring":
-                n_slots = 2 if self.slots_policy == 2 else max(self.world - 1, 1)
-                self.slots = SymmetricBuffer(comm, self.nbytes * n_slots, device, zero=False)
+                self.slots = SymmetricBuffer(comm, slot_bytes, device, zero=False)
             if algo in ("ring-unfused", "ring-nccl"):
                 self.vb = SymmetricBuffer(comm, self.nbytes, device)
 
@@ -266,6 +290,79 @@ class AllreduceMiniapp:
             if b is not None:
                 b.close()
         self.pads.close()
+
+
+class VirtualAllreduce:
+    """``world`` AllreduceMiniapp ranks driven by ONE process on one GPU: virtual ranks whose peer pointers are plain
+    pointers, so the ring's arrival and ack words, the two-shot barrier and the unfused ring's rendezvous run on a
+    1-GPU box with the same ``run_once`` plumbing as one process per GPU.  ``run_once()`` enqueues one allreduce per
+    rank, each on its own stream.  The fused ring's CTAs spin per chunk on their neighbours, so every rank's grid is
+    kept co-resident: at most ``sms // world`` CTAs each.  At most 8 ranks: more streams than the device's hardware
+    queues would serialise the spinning kernels.  The unfused ring launches a kernel for the first time next to spinning
+    ones, which needs the eager module loading this package asks for when it is imported before CUDA starts."""
+
+    MAX_WORLD = 8
+
+    def __init__(self, world: int, n: int, dtype: str = "float", algo: str = "ring", slots: int = 0,
+                 pull: bool = False, ctas: int = 0, chunk_elems: int = 0, device: int = 0, timeout_s: float = 10.0):
+        from ..parallel.local import LocalGroup
+
+        if not 1 <= world <= self.MAX_WORLD:
+            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
+        if algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        C = native()
+        esz = C.elem_size(dtype)
+        n = element_count(esz, world, n_elems=n)
+        cap = max(1, C.sm_count(device) // world)
+        self.ctas = min(ctas, cap) if ctas > 0 else cap
+        self.dtype, self.device, self.n = dtype, device, n
+        self.group = LocalGroup(world, [device] * world)
+        policy = slots if algo == "ring" else 0
+        pad_words, slot_bytes = ring_layout(n * esz, C.ring_num_chunks(n, chunk_elems, esz), world, policy)
+        none = [None] * world
+        pads = self.group.pads(extra_words=pad_words, timeout_s=timeout_s)
+        va = self.group.symmetric(n * esz)
+        vc = self.group.symmetric(n * esz)
+        vb = self.group.symmetric(n * esz) if algo == "ring-unfused" else none
+        sl = self.group.symmetric(slot_bytes, zero=False) if algo == "ring" else none
+        self.ranks: List[AllreduceMiniapp] = [
+            AllreduceMiniapp(self.group.comms[r], device, dtype=dtype, algo=algo, chunk_elems=chunk_elems,
+                             ctas=self.ctas, timeout_s=timeout_s, slots=slots, pull=pull, n_elems=n,
+                             _shared={"pads": pads[r], "va": va[r], "vb": vb[r], "vc": vc[r], "slots": sl[r]})
+            for r in range(world)]
+        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
+
+    def load(self, vas: List[torch.Tensor]) -> None:
+        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the rings accumulate into it)."""
+        td = _TORCH_DTYPE[self.dtype]
+        torch.cuda.synchronize(self.device)
+        for app, v in zip(self.ranks, vas):
+            app.va.tensor(td).copy_(v)
+            app.vc.tensor(td).zero_()
+        torch.cuda.synchronize(self.device)
+
+    def run_once(self) -> None:
+        """One allreduce: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one (it
+        stands in for the cross-rank barrier that separates consecutive launches)."""
+        for app, st in zip(self.ranks, self.streams):
+            with torch.cuda.device(app.device), torch.cuda.stream(st):
+                app.run_once()
+
+    def synchronize(self) -> None:
+        for st in self.streams:
+            st.synchronize()
+        for app in self.ranks:
+            app.pads.check()
+
+    def results(self) -> List[torch.Tensor]:
+        """VC of every rank, on the host."""
+        self.synchronize()
+        return [app.vc.tensor(_TORCH_DTYPE[self.dtype]).cpu() for app in self.ranks]
+
+    def close(self) -> None:
+        for app in self.ranks:
+            app.close()
 
 
 def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int):
