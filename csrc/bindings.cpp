@@ -595,6 +595,22 @@ PYBIND11_MODULE(_C, m) {
   m.def("ring_pull_src_slot", &ring_pull_src_slot);
   m.def("ring_pull_waits_for_ack", &ring_pull_waits_for_ack);
   m.def("ring_pull_publishes_ack", &ring_pull_publishes_ack);
+  // Hop rules of the reduce-scatter + all-gather ring (phase: RSAG_ALLREDUCE, RSAG_REDUCE_SCATTER, RSAG_ALL_GATHER).
+  m.attr("RSAG_ALLREDUCE") = static_cast<int>(kRsAgAllreduce);
+  m.attr("RSAG_REDUCE_SCATTER") = static_cast<int>(kRsAgReduceScatter);
+  m.attr("RSAG_ALL_GATHER") = static_cast<int>(kRsAgAllGather);
+  m.def("rsag_first_hop", &rsag_first_hop);
+  m.def("rsag_last_hop", &rsag_last_hop);
+  m.def("rsag_segment", &rsag_segment);
+  m.def("rsag_reads_vc", &rsag_reads_vc);
+  m.def("rsag_src_slot", &rsag_src_slot);
+  m.def("rsag_writes_own_vc", &rsag_writes_own_vc);
+  m.def("rsag_forwards", &rsag_forwards);
+  m.def("rsag_fwd_slot", &rsag_fwd_slot);
+  m.def("rsag_waits", &rsag_waits);
+  m.def("rsag_publishes", &rsag_publishes);
+  m.def("rsag_arrival", &rsag_arrival);
+  m.def("rsag_epoch_advance", &rsag_epoch_advance);
   m.def("ring_num_chunks", &ring_num_chunks, py::arg("n"), py::arg("chunk_elems") = 0, py::arg("elem_bytes") = 4);
   m.def("elem_size", [](const std::string& dtype) { return elem_size(elem_from(dtype)); });
   m.def(
@@ -631,6 +647,44 @@ PYBIND11_MODULE(_C, m) {
       py::arg("status") = 0, py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0,
       py::arg("stream") = 0, py::arg("n_slots") = 0, py::arg("ack_local") = 0, py::arg("ack_left") = 0,
       py::arg("pull") = false, py::arg("va_left") = 0, py::arg("slots_left") = 0);
+  m.def(
+      "ring_rsag",
+      [](uintptr_t va, uintptr_t vc, uintptr_t slots_local, uintptr_t slots_right, uintptr_t vc_right,
+         uintptr_t arrived_local, uintptr_t arrived_right, int rank, int world, size_t n, size_t chunk_elems,
+         uint32_t epoch_base, uint64_t timeout_ns, uintptr_t status, const std::string& dtype, int ctas, int device,
+         uintptr_t stream, const std::string& phases) {
+        RingRsAgArgs a;
+        a.va = as_ptr<const void>(va);
+        a.vc = as_ptr<void>(vc);
+        a.slots_local = as_ptr<void>(slots_local);
+        a.slots_right = as_ptr<void>(slots_right);
+        a.vc_right = as_ptr<void>(vc_right);
+        a.arrived_local = as_ptr<uint32_t>(arrived_local);
+        a.arrived_right = as_ptr<uint32_t>(arrived_right);
+        a.rank = rank;
+        a.world = world;
+        a.n = n;
+        a.chunk_elems = chunk_elems;
+        a.epoch_base = epoch_base;
+        a.timeout_ns = timeout_ns;
+        a.status = as_ptr<uint32_t>(status);
+        if (phases == "allreduce")
+          a.phases = kRsAgAllreduce;
+        else if (phases == "reduce_scatter")
+          a.phases = kRsAgReduceScatter;
+        else if (phases == "all_gather")
+          a.phases = kRsAgAllGather;
+        else
+          HPCP_FAIL("ring_rsag: phases must be allreduce, reduce_scatter or all_gather, not " + phases);
+        launch_ring_rsag(a, elem_from(dtype), ctas, device, as_stream(stream));
+      },
+      py::arg("va"), py::arg("vc"), py::arg("slots_local"), py::arg("slots_right"), py::arg("vc_right"),
+      py::arg("arrived_local"), py::arg("arrived_right"), py::arg("rank"), py::arg("world"), py::arg("n"),
+      py::arg("chunk_elems") = 0, py::arg("epoch_base") = 0, py::arg("timeout_ns") = 0, py::arg("status") = 0,
+      py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0,
+      py::arg("phases") = "allreduce",
+      "Reduce-scatter + all-gather ring in one launch per rank (kernels/ring_order.h: rsag_*); "
+      "phases = allreduce | reduce_scatter | all_gather.");
   m.def(
       "allreduce_two_shot",
       [](const std::vector<uintptr_t>& va, const std::vector<uintptr_t>& vc,

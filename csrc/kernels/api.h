@@ -341,6 +341,31 @@ size_t ring_num_chunks(size_t n, size_t chunk_elems, size_t elem_bytes = 4);
 void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int device,
                            cudaStream_t stream);
 
+// Bandwidth-optimal ring in ONE launch per rank: a ring reduce-scatter (segment s of the block is summed by rank s)
+// followed by a ring all-gather, each rank talking only to its right neighbour.  It sends 2(P-1)/P of the block per
+// rank and needs (P-1)/P of it in receive slots.  Hop rules: kernels/ring_order.h (rsag_*).  `phases` selects the
+// hops: kRsAgAllreduce (all), kRsAgReduceScatter (only own VC[r] is written), kRsAgAllGather (VC[s] <- rank s's VA[s]).
+// A launch advances the arrival epochs by rsag_epoch_advance(phases, world); as with the ring, launches that reuse
+// the slots must be separated by a cross-rank barrier.
+struct RingRsAgArgs {
+  const void* va = nullptr;           // local input block, never written
+  void* vc = nullptr;                 // local output block; must not overlap VA
+  void* slots_local = nullptr;        // (world-1) segments of n/world elements, written by the left neighbour
+  void* slots_right = nullptr;        // peer-mapped: the right neighbour's slots
+  void* vc_right = nullptr;           // peer-mapped: the right neighbour's VC (all-gather pushes)
+  uint32_t* arrived_local = nullptr;  // one word per chunk of a segment, written by the left neighbour
+  uint32_t* arrived_right = nullptr;  // peer-mapped: the right neighbour's arrival words
+  int rank = 0;
+  int world = 0;
+  size_t n = 0;                       // elements per rank; a multiple of world 16-byte vectors
+  size_t chunk_elems = 0;             // 0 -> 128 KiB worth of elements; chunk bytes a multiple of 16
+  uint32_t epoch_base = 0;
+  uint64_t timeout_ns = 0;
+  uint32_t* status = nullptr;
+  int phases = 0;                     // RsAgPhase (ring_order.h)
+};
+void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int device, cudaStream_t stream);
+
 // One-kernel "collective" allreduce (the miniapp's -a path, ↔ MPI_Allreduce :61-67).
 // two-shot over peer mappings: rank r reduces slice r by loading it from every
 // rank's VA and stores the sum into every rank's VC, then a cross-GPU barrier.

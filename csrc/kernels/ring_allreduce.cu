@@ -300,6 +300,85 @@ __global__ void __launch_bounds__(512) ring_pull_kernel(const __grid_constant__ 
   }
 }
 
+// ------------------------------------------------- K-ring, reduce-scatter + all-gather ----
+// Bandwidth-optimal ring: segment s (nvec / P vectors) of the block is reduced hop by hop on its way to rank s, then
+// the finished segments travel once more round the ring.  Per (hop, chunk) a CTA waits on arrival word c, reads the
+// chunk once (slot + own VA while reducing, own VC while gathering), stores it into the right neighbour's slot or VC
+// and, at hop P-1, into its own VC, then publishes arrival word c on the right neighbour.  Rules: ring_order.h.
+struct RingRsAgDev {
+  const uint4* va;
+  uint4* vc;
+  const uint4* slots_local;
+  uint4* slots_right;
+  uint4* vc_right;
+  uint32_t* arrived_local;
+  uint32_t* arrived_right;
+  int rank;
+  int world;
+  int phases;
+  size_t seg_vec;     // vectors per segment
+  size_t chunk_vec;   // vectors per chunk
+  size_t n_chunks;    // chunks per segment
+  uint32_t epoch_base;
+  uint64_t timeout_ns;
+  uint32_t* status;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(512) ring_rsag_kernel(const __grid_constant__ RingRsAgDev a) {
+  __shared__ int ok_s;
+  const int last = rsag_last_hop(a.phases, a.world);
+  for (int h = rsag_first_hop(a.phases, a.world); h <= last; ++h) {
+    const size_t seg = static_cast<size_t>(rsag_segment(h, a.rank, a.world)) * a.seg_vec;
+    const uint4* src = (rsag_reads_vc(h, a.world) ? a.vc : a.va) + seg;
+    const int rs = rsag_src_slot(h, a.phases, a.world);
+    const uint4* slot = rs >= 0 ? a.slots_local + static_cast<size_t>(rs) * a.seg_vec : nullptr;
+    uint4* own = rsag_writes_own_vc(h, a.world) ? a.vc + seg : nullptr;
+    const int fs = rsag_fwd_slot(h, a.world);
+    uint4* fwd = !rsag_forwards(h, a.phases, a.world) ? nullptr
+                 : fs >= 0                             ? a.slots_right + static_cast<size_t>(fs) * a.seg_vec
+                                                       : a.vc_right + seg;
+    const bool waits = rsag_waits(h, a.phases, a.world);
+    const uint32_t want = a.epoch_base + rsag_arrival(h, a.phases, a.world);
+    for (size_t c = blockIdx.x; c < a.n_chunks; c += gridDim.x) {
+      if (waits) {
+        if (threadIdx.x == 0) ok_s = wait_epoch(a.arrived_local + c, want, a.timeout_ns, a.status) ? 1 : 0;
+        __syncthreads();
+        if (!ok_s) return;  // peer hung: status word set, drain
+      }
+      const size_t begin = c * a.chunk_vec;
+      const size_t end = begin + a.chunk_vec < a.seg_vec ? begin + a.chunk_vec : a.seg_vec;
+      size_t i = (own || fwd) ? begin + threadIdx.x : end;  // the last hop of a gather only waits
+      for (; i + 3 * blockDim.x < end; i += 4 * blockDim.x) {
+        uint4 x[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) x[k] = ptx::ld_weak_v4(src + i + k * blockDim.x);
+        if (slot) {
+          uint4 s[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) s[k] = ptx::ld_weak_v4(slot + i + k * blockDim.x);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) x[k] = Vec4<T>::add(s[k], x[k]);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (own) own[i + k * blockDim.x] = x[k];
+          if (fwd) ptx::st_stream_v4(fwd + i + k * blockDim.x, x[k]);
+        }
+      }
+      for (; i < end; i += blockDim.x) {
+        uint4 x = ptx::ld_weak_v4(src + i);
+        if (slot) x = Vec4<T>::add(ptx::ld_weak_v4(slot + i), x);
+        if (own) own[i] = x;
+        if (fwd) ptx::st_stream_v4(fwd + i, x);
+      }
+      __syncthreads();  // whole chunk stored by this CTA (and ok_s consumed by everyone)
+      if (fwd && threadIdx.x == 0)
+        publish_epoch_light(a.arrived_right + c, a.epoch_base + rsag_arrival(h + 1, a.phases, a.world));
+    }
+  }
+}
+
 // ---------------------------------------------------------------- two-shot ----
 struct TwoShotDev {
   const uint4* va[kApiMaxRanks];
@@ -441,6 +520,38 @@ int grid_for(size_t items, int threads, int cap) {
   return static_cast<int>(std::max<size_t>(1, std::min<size_t>(want, static_cast<size_t>(cap))));
 }
 
+// Grid of a ring kernel whose CTAs own chunks round-robin.  All CTAs may spin on arrival (and ack) words, so the whole
+// grid must be co-resident: clamp it with the real occupancy of the instantiation that is about to run (512 threads x
+// its register count), never with a guess.  Ranks that share a GPU divide the clamp among themselves on the caller's
+// side (`ctas`).
+int ring_grid(const void* kernel, size_t n_chunks, int ctas, int device) {
+  int per_sm = 0;
+  HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 512, 0));
+  HPCP_REQUIRE(per_sm >= 1, "ring: the kernel does not fit on an SM");
+  const int sms = device_sm_count(device);
+  int grid = ctas > 0 ? ctas : sms * std::min(per_sm, 2);
+  grid = std::min(grid, sms * per_sm);
+  grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(grid), std::max<size_t>(n_chunks, 1)));
+  if (ctas <= 0 && n_chunks > static_cast<size_t>(grid)) {
+    // Chunks are dealt round-robin: pick the grid in [3/4 cap, cap] that wastes the least
+    // (every CTA should own the same number of chunks, or the slowest CTA paces the ring).
+    int best = grid;
+    size_t best_waste = ~size_t{0};
+    for (int g = grid; g >= grid * 3 / 4 && g >= 1; --g) {
+      const size_t rounds = (n_chunks + g - 1) / g;
+      const size_t waste = rounds * g - n_chunks;
+      // compare wasted chunk-slots relative to useful parallelism
+      if (waste * best < best_waste * g || best_waste == ~size_t{0}) {
+        best_waste = waste;
+        best = g;
+      }
+      if (waste == 0) break;
+    }
+    grid = best;
+  }
+  return grid;
+}
+
 }  // namespace
 
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
@@ -517,9 +628,6 @@ void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int de
   HPCP_REQUIRE(!args.pull || args.n_slots != 2 || args.world <= 4 ||
                    (args.ack_local != nullptr && args.ack_left != nullptr),
                "ring: pull with n_slots=2 needs the ack words");
-  // All CTAs may spin on arrival (and ack) words, so the whole grid must be co-resident: clamp it with the real
-  // occupancy of the instantiation that is about to run (512 threads x its register count), never with a guess.
-  // Ranks that share a GPU divide the clamp among themselves on the caller's side (`ctas`).
   const bool two_slots_k = args.n_slots == 2;
   const void* kernel = nullptr;
   dispatch_add_class(type, [&](auto tag) {
@@ -531,30 +639,7 @@ void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int de
       kernel = two_slots_k ? reinterpret_cast<const void*>(ring_allreduce_kernel<C, true>)
                            : reinterpret_cast<const void*>(ring_allreduce_kernel<C, false>);
   });
-  int per_sm = 0;
-  HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 512, 0));
-  HPCP_REQUIRE(per_sm >= 1, "ring: the kernel does not fit on an SM");
-  const int sms = device_sm_count(device);
-  int grid = ctas > 0 ? ctas : sms * std::min(per_sm, 2);
-  grid = std::min(grid, sms * per_sm);
-  grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(grid), std::max<size_t>(d.n_chunks, 1)));
-  if (ctas <= 0 && d.n_chunks > static_cast<size_t>(grid)) {
-    // Chunks are dealt round-robin: pick the grid in [3/4 cap, cap] that wastes the least
-    // (every CTA should own the same number of chunks, or the slowest CTA paces the ring).
-    int best = grid;
-    size_t best_waste = ~size_t{0};
-    for (int g = grid; g >= grid * 3 / 4 && g >= 1; --g) {
-      const size_t rounds = (d.n_chunks + g - 1) / g;
-      const size_t waste = rounds * g - d.n_chunks;
-      // compare wasted chunk-slots relative to useful parallelism
-      if (waste * best < best_waste * g || best_waste == ~size_t{0}) {
-        best_waste = waste;
-        best = g;
-      }
-      if (waste == 0) break;
-    }
-    grid = best;
-  }
+  const int grid = ring_grid(kernel, d.n_chunks, ctas, device);
   const bool two_slots = args.n_slots == 2;  // slot index t % 2 even when no ack is ever needed (P <= 3)
   if (args.pull) {
     RingPullDev p{};
@@ -590,6 +675,44 @@ void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int de
       ring_allreduce_kernel<C, true><<<grid, 512, 0, stream>>>(d);
     else
       ring_allreduce_kernel<C, false><<<grid, 512, 0, stream>>>(d);
+  });
+  HPCP_CUDA(cudaGetLastError());
+}
+
+void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int device, cudaStream_t stream) {
+  HPCP_REQUIRE(args.world >= 1 && args.world <= kApiMaxRanks, "ring-rsag: world out of range");
+  HPCP_REQUIRE(args.rank >= 0 && args.rank < args.world, "ring-rsag: rank out of range");
+  HPCP_REQUIRE(args.phases == kRsAgAllreduce || args.phases == kRsAgReduceScatter || args.phases == kRsAgAllGather,
+               "ring-rsag: phases must be allreduce, reduce_scatter or all_gather");
+  const size_t esz = elem_size(type), lanes = 16 / esz;
+  HPCP_REQUIRE(args.n % (lanes * static_cast<size_t>(args.world)) == 0,
+               "ring-rsag: every rank's segment must be a multiple of 16 bytes");
+  const size_t ce = args.chunk_elems == 0 ? kRingDefaultChunkBytes / esz : args.chunk_elems;
+  HPCP_REQUIRE(ce % lanes == 0, "ring-rsag: a chunk must be a multiple of 16 bytes");
+  const auto va = reinterpret_cast<uintptr_t>(args.va), vc = reinterpret_cast<uintptr_t>(args.vc);
+  const uintptr_t bytes = args.n * esz;
+  HPCP_REQUIRE(va + bytes <= vc || vc + bytes <= va, "ring-rsag: VA and VC must not overlap (no in-place operation)");
+  RingRsAgDev d{};
+  d.va = static_cast<const uint4*>(args.va);
+  d.vc = static_cast<uint4*>(args.vc);
+  d.slots_local = static_cast<const uint4*>(args.slots_local);
+  d.slots_right = static_cast<uint4*>(args.slots_right);
+  d.vc_right = static_cast<uint4*>(args.vc_right);
+  d.arrived_local = args.arrived_local;
+  d.arrived_right = args.arrived_right;
+  d.rank = args.rank;
+  d.world = args.world;
+  d.phases = args.phases;
+  d.seg_vec = args.n / lanes / args.world;
+  d.chunk_vec = ce / lanes;
+  d.n_chunks = ring_num_chunks(args.n / args.world, ce, esz);
+  d.epoch_base = args.epoch_base;
+  d.timeout_ns = args.timeout_ns;
+  d.status = args.status;
+  dispatch_add_class(type, [&](auto tag) {
+    using C = decltype(tag);
+    const int grid = ring_grid(reinterpret_cast<const void*>(ring_rsag_kernel<C>), d.n_chunks, ctas, device);
+    ring_rsag_kernel<C><<<grid, 512, 0, stream>>>(d);
   });
   HPCP_CUDA(cudaGetLastError());
 }

@@ -17,6 +17,8 @@
 //   ring          fused K-ring: all P-1 exchanges + P accumulations in one launch/rank
 //   ring-unfused  same data movement as the reference with separate kernels:
 //                 rendezvous put kernel, then Accumulate kernel, per step (VA/VB swap)
+//   ring-rsag     bandwidth-optimal ring: reduce-scatter + all-gather in one launch/rank,
+//                 2(P-1)/P of the block sent per rank (n padded to whole 16-byte vectors x P)
 //   (with -a)     nvls when NVSwitch multicast is available, else two-shot P2P;
 //                 force with --coll nvls|twoshot
 #include <cuda_profiler_api.h>
@@ -39,6 +41,7 @@
 #include "../common/rank_runtime.h"
 #include "../common/signal_layout.h"
 #include "../kernels/api.h"
+#include "../kernels/ring_order.h"
 #include "devices.hpp"
 
 namespace {
@@ -88,8 +91,9 @@ void print_help() {
                " -n N        ranks (one host thread + one GPU each; default: all GPUs;\n"
                "             more ranks than GPUs are placed round-robin)\n"
                " --type T   element type: float int uint double long ulong short ushort uchar (default float, or binary-name suffix)\n"
-               " --algo ring|ring-unfused   fused persistent ring kernel (default) or\n"
-               "                            separate put + accumulate kernels per step\n"
+               " --algo ring|ring-unfused|ring-rsag   fused persistent ring kernel (default),\n"
+               "                            separate put + accumulate kernels per step, or the\n"
+               "                            bandwidth-optimal reduce-scatter + all-gather ring\n"
                " --coll auto|nvls|twoshot   collective used with -a\n"
                " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
                " --ctas N --chunk N    kernel tuning (CTAs per rank, elements per ring chunk)\n"
@@ -107,6 +111,7 @@ struct Shared {
   size_t n = 0;
   size_t n_chunks = 0;
   size_t pad_extra = 0;  // words after the fixed pad: arrival words (+ ack words with --slots 2)
+  uint32_t epoch_advance = 0;  // arrival epochs one launch of the fused ring uses
   SymmetricBuffer va, vb, vc, slots, pads;
   MulticastBuffer mc_va, mc_vc;
   std::vector<void*> host_va, host_vc;  // -R: the host arrays whose mapped copies are va / vc
@@ -228,7 +233,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       a.world = P;
       a.n = sh.n;
       a.chunk_elems = cfg.chunk_elems;
-      a.epoch_base = replay ? ring_epoch - static_cast<uint32_t>(P) : ring_epoch;
+      a.epoch_base = replay ? ring_epoch - sh.epoch_advance : ring_epoch;
       a.timeout_ns = cfg.timeout_ns;
       a.status = status;
       a.n_slots = cfg.slots;
@@ -241,8 +246,27 @@ void rank_main(RankCtx& ctx, Shared& sh) {
         a.ack_local = my_pad + kPadWords + sh.n_chunks;
         a.ack_left = pad_of(sh, left) + kPadWords + sh.n_chunks;
       }
-      if (!replay) ring_epoch += static_cast<uint32_t>(P);
+      if (!replay) ring_epoch += sh.epoch_advance;
       launch_ring_allreduce(a, cfg.type, cfg.ctas, dev, stream);
+    } else if (cfg.algo == "ring-rsag") {
+      RingRsAgArgs a;
+      a.va = va;
+      a.vc = vc;
+      a.slots_local = sh.slots.ptr[me];
+      a.slots_right = sh.slots.ptr[right];
+      a.vc_right = sh.vc.ptr[right];
+      a.arrived_local = my_pad + kPadWords;
+      a.arrived_right = pad_of(sh, right) + kPadWords;
+      a.rank = me;
+      a.world = P;
+      a.n = sh.n;
+      a.chunk_elems = cfg.chunk_elems;
+      a.epoch_base = replay ? ring_epoch - sh.epoch_advance : ring_epoch;
+      a.timeout_ns = cfg.timeout_ns;
+      a.status = status;
+      a.phases = kRsAgAllreduce;
+      if (!replay) ring_epoch += sh.epoch_advance;
+      launch_ring_rsag(a, cfg.type, cfg.ctas, dev, stream);
     } else {  // ring-unfused: the reference's step structure with separate kernels
       HPCP_REQUIRE(!replay, "--profile-relaunch supports the one-launch algorithms only");
       void* cur = va;
@@ -358,10 +382,16 @@ void rank_main(RankCtx& ctx, Shared& sh) {
 // neighbour" is a memcpy into its VB, the collective is a direct sum over every rank's VA.  No GPU,
 // no kernels: this is the plumbing configuration used to test the program logic (options, ring
 // order, verification, output) on a machine without a device.
+// --algo ring-rsag runs the hops of ring_rsag_kernel with the same rules (ring_order.h): whole segments are memcpy'd
+// into the right neighbour's slot or VC, with a barrier between hops.
 template <typename T>
 int run_on_host_typed(const Config& cfg) {
   const int P = cfg.ranks > 0 ? cfg.ranks : 4;
-  const size_t n = size_t{1} << cfg.log2_elems;
+  const bool rsag = cfg.algo == "ring-rsag" && !cfg.use_collective;
+  size_t n = size_t{1} << cfg.log2_elems;
+  const size_t unit = 16 / sizeof(T) * static_cast<size_t>(P);
+  if (rsag && n % unit != 0) n = (n / unit + 1) * unit;  // whole 16-byte vectors per segment, as on the device
+  const size_t seg_n = n / P;
   std::vector<std::vector<T>> va(P), vb(P), vc(P);
   double elapsed_ms = 0;
   unsigned long long total_bad = 0;
@@ -375,6 +405,24 @@ int run_on_host_typed(const Config& cfg) {
     if (cfg.use_collective) {
       for (int r = 0; r < P; ++r)
         for (size_t i = 0; i < n; ++i) vc[me][i] += va[r][i];
+    } else if (rsag) {
+      vb[me].resize(seg_n * std::max(P - 1, 1));  // receive slots
+      ctx.barrier();
+      std::vector<T> x(seg_n);
+      for (int h = 0; h <= rsag_last_hop(kRsAgAllreduce, P); ++h) {
+        const size_t seg = static_cast<size_t>(rsag_segment(h, me, P)) * seg_n;
+        const T* src = (rsag_reads_vc(h, P) ? vc[me].data() : va[me].data()) + seg;
+        const int rs = rsag_src_slot(h, kRsAgAllreduce, P);
+        for (size_t i = 0; i < seg_n; ++i)
+          x[i] = rs >= 0 ? static_cast<T>(vb[me][rs * seg_n + i] + src[i]) : src[i];
+        if (rsag_writes_own_vc(h, P)) std::memcpy(vc[me].data() + seg, x.data(), seg_n * sizeof(T));
+        if (rsag_forwards(h, kRsAgAllreduce, P)) {
+          const int fs = rsag_fwd_slot(h, P);
+          T* dst = fs >= 0 ? vb[right].data() + fs * seg_n : vc[right].data() + seg;
+          std::memcpy(dst, x.data(), seg_n * sizeof(T));  // "send right"
+        }
+        ctx.barrier();  // the hop has landed everywhere
+      }
     } else {
       for (size_t i = 0; i < n; ++i) vc[me][i] += va[me][i];
       for (int s = 1; s < P; ++s) {
@@ -402,17 +450,19 @@ int run_on_host_typed(const Config& cfg) {
     }
   });
   std::cout << "Elapsed (max over ranks): " << elapsed_ms << " ms | "
-            << (cfg.use_collective ? "collective" : "ring") << " " << elem_type_name(cfg.type)
+            << (cfg.use_collective ? "collective" : rsag ? "host-ring-rsag" : "ring") << " " << elem_type_name(cfg.type)
             << " host-threads P=" << P << " N=2^" << cfg.log2_elems << " arrays=" << alloc_kind_name(cfg.kind)
             << " (host vectors in this mode)" << std::endl;
   if (!cfg.json_path.empty()) {  // same row shape as the GPU path; the algo name marks the plumbing run
     if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
-      const size_t n = size_t{1} << cfg.log2_elems;
-      const double sent = cfg.use_collective ? 0.0 : static_cast<double>(P - 1) * n * sizeof(T);
+      const double sent = cfg.use_collective ? 0.0
+                          : rsag             ? 2.0 * (P - 1) / P * n * sizeof(T)
+                                             : static_cast<double>(P - 1) * n * sizeof(T);
       std::fprintf(f,
                    "{\"pattern\":\"allreduce\",\"algo\":\"%s\",\"type\":\"%s\",\"alloc\":\"host-vectors\","
                    "\"ranks\":%d,\"elements\":%zu,\"ms\":%.6f,\"GBps_sent_per_rank\":%.3f,\"mismatches\":%llu}\n",
-                   cfg.use_collective ? "host-collective" : "host-ring", elem_type_name(cfg.type), P, n, elapsed_ms,
+                   cfg.use_collective ? "host-collective" : rsag ? "host-ring-rsag" : "host-ring",
+                   elem_type_name(cfg.type), P, n, elapsed_ms,
                    elapsed_ms > 0 ? sent / (elapsed_ms * 1e6) : 0.0, total_bad);
       std::fclose(f);
     }
@@ -499,9 +549,12 @@ int main(int argc, char** argv) {
         default: print_help(); return 1;
       }
     }
-    HPCP_REQUIRE(cfg.algo == "ring" || cfg.algo == "ring-unfused", "unknown --algo " + cfg.algo);
+    HPCP_REQUIRE(cfg.algo == "ring" || cfg.algo == "ring-unfused" || cfg.algo == "ring-rsag",
+                 "unknown --algo " + cfg.algo);
     HPCP_REQUIRE(cfg.log2_elems >= 4 && cfg.log2_elems <= 32, "-p must be in [4,32]");
     HPCP_REQUIRE(cfg.slots == 0 || cfg.slots == 2, "--slots must be 2 (or omitted)");
+    HPCP_REQUIRE(cfg.algo != "ring-rsag" || (cfg.slots == 0 && !cfg.pull),
+                 "--slots 2 and --pull are variants of --algo ring, not of ring-rsag");
 
     if (cfg.cpu) return run_on_host(cfg);
     const int ndev = visible_device_count();
@@ -526,13 +579,16 @@ int main(int argc, char** argv) {
     sh.mem = &mem;
     sh.n = size_t{1} << cfg.log2_elems;
     const size_t esz = elem_size(cfg.type), lanes = 16 / esz;
-    if (cfg.use_collective && sh.n % (lanes * static_cast<size_t>(P)) != 0)
+    const bool rsag = cfg.algo == "ring-rsag" && !cfg.use_collective;
+    if ((cfg.use_collective || rsag) && sh.n % (lanes * static_cast<size_t>(P)) != 0)
       sh.n = (sh.n / (lanes * P) + 1) * (lanes * P);  // pad so that every rank owns a 16-byte aligned slice
     else if (sh.n % lanes != 0)
       sh.n = (sh.n / lanes + 1) * lanes;
     const size_t bytes = sh.n * esz;
-    sh.n_chunks = ring_num_chunks(sh.n, cfg.chunk_elems, elem_size(cfg.type));
+    // ring-rsag: one arrival word per chunk of a segment
+    sh.n_chunks = ring_num_chunks(rsag ? sh.n / P : sh.n, cfg.chunk_elems, elem_size(cfg.type));
     sh.pad_extra = sh.n_chunks * (cfg.slots == 2 ? 2 : 1);
+    sh.epoch_advance = static_cast<uint32_t>(rsag ? rsag_epoch_advance(kRsAgAllreduce, P) : P);
     sh.pads = mem.alloc_pads(sh.pad_extra);
 
     if (cfg.use_collective) {
@@ -573,6 +629,8 @@ int main(int argc, char** argv) {
     if (!cfg.use_collective) {
       if (cfg.algo == "ring")
         sh.slots = mem.alloc(bytes * static_cast<size_t>(cfg.slots == 2 ? 2 : P - 1), array_kind, /*zero=*/false);
+      else if (rsag)
+        sh.slots = mem.alloc(bytes / P * (P - 1), array_kind, /*zero=*/false);
       else
         sh.vb = mem.alloc(bytes, array_kind);
     }
@@ -584,8 +642,10 @@ int main(int argc, char** argv) {
     // Reporting: the number the reference computes and drops.
     const std::string algo_name =
         cfg.use_collective ? (sh.nvls ? "nvls" : "twoshot") : cfg.algo;
-    // Per-rank bytes sent over NVLink: faithful ring (P-1)*N; bandwidth-optimal collectives (P-1)/P*N.
+    // Per-rank bytes sent over NVLink: faithful ring (P-1)*N; bandwidth-optimal collectives (P-1)/P*N; the
+    // reduce-scatter + all-gather ring 2(P-1)/P*N.
     const double sent = cfg.use_collective ? static_cast<double>(bytes) * (P - 1) / P
+                        : rsag             ? 2.0 * static_cast<double>(bytes) * (P - 1) / P
                                            : static_cast<double>(bytes) * (P - 1);
     const double gbps = sent / (sh.best_ms * 1e-3) * 1e-9;
     std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << sh.best_ms << " ms | "

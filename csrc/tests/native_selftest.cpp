@@ -198,6 +198,34 @@ void test_kernel_orderings() {
       CHECK(ring_src_slot(t + 1, true) == ring_fwd_slot(t, true));   // what hop t forwards is what hop t+1 reads
       CHECK(ring_src_slot(t + 1, false) == ring_fwd_slot(t, false));
     }
+  // Reduce-scatter + all-gather ring: segment r is finished on rank r, every slot is written once and read by the next
+  // hop, the all-gather never pushes into the right neighbour's own segment, and every publish is awaited.
+  for (int P = 1; P <= 9; ++P)
+    for (int phase : {int(kRsAgAllreduce), int(kRsAgReduceScatter), int(kRsAgAllGather)}) {
+      const int first = rsag_first_hop(phase, P), last = rsag_last_hop(phase, P);
+      CHECK(rsag_epoch_advance(phase, P) == (phase == kRsAgAllreduce ? 2 : 1) * (P - 1));
+      CHECK(!rsag_waits(first, phase, P) && rsag_arrival(first, phase, P) == 0);
+      std::set<int> slots_written;
+      for (int h = first; h <= last; ++h)
+        for (int r = 0; r < P; ++r) {
+          const int seg = rsag_segment(h, r, P);
+          CHECK(seg >= 0 && seg < P);
+          CHECK(!rsag_writes_own_vc(h, P) || seg == r);
+          CHECK(seg == rsag_segment(h - 1, (r - 1 + P) % P, P));  // the left neighbour's previous hop: same segment
+          if (rsag_publishes(h, phase, P)) {
+            CHECK(h < last && rsag_waits(h + 1, phase, P));
+            CHECK(rsag_arrival(h + 1, phase, P) == rsag_arrival(h, phase, P) + 1);
+            const int fs = rsag_fwd_slot(h, P);
+            if (fs >= 0) {
+              CHECK(rsag_src_slot(h + 1, phase, P) == fs);
+              if (r == 0) CHECK(slots_written.insert(fs).second);
+            } else {
+              CHECK(seg != (r + 1) % P);
+            }
+          }
+        }
+      CHECK(static_cast<int>(slots_written.size()) == (phase == kRsAgAllGather ? 0 : P - 1));
+    }
 }
 
 int main() {

@@ -6,6 +6,8 @@ OpenMP variants): every rank holds VA = rank, VC = 0; after the allreduce every
 element of VC equals P(P-1)/2.  Algorithms:
 
   ring          fused K-ring kernel: P-1 neighbour exchanges + P accumulations, one launch
+  ring-rsag     bandwidth-optimal ring, one launch: reduce-scatter + all-gather between neighbours only,
+                2(P-1)/P of the block sent per rank
   ring-unfused  the reference's step structure with separate kernels (rendezvous put, then
                 accumulate), no host sync between steps
   twoshot       one-launch collective over peer mappings            (↔ MPI_Allreduce, -a)
@@ -28,8 +30,8 @@ from .. import native
 from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
-ALGOS = ("ring", "ring-unfused", "twoshot", "nvls", "nccl", "ring-nccl")
-VIRTUAL_ALGOS = ("ring", "ring-unfused", "twoshot")   # the ones whose peers are plain pointers (no NCCL, no multicast)
+ALGOS = ("ring", "ring-unfused", "twoshot", "nvls", "nccl", "ring-nccl", "ring-rsag")
+VIRTUAL_ALGOS = ("ring", "ring-unfused", "twoshot", "ring-rsag")   # the ones whose peers are plain pointers (no NCCL, no multicast)
 # element types of the reference's datatype trait (mpi_datatype.hpp:28-51) -> the torch dtype whose add is bit-identical
 # (unsigned integers share the two's-complement add of the signed type of the same width; NCCL rows only)
 _TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32, "double": torch.float64,
@@ -42,9 +44,12 @@ def expected_value(world: int) -> float:
 
 
 def bytes_sent_per_rank(algo: str, nbytes: int, world: int) -> float:
-    """Faithful ring forwards the full block P-1 times; bandwidth-optimal collectives (P-1)/P of it."""
+    """Faithful ring forwards the full block P-1 times; bandwidth-optimal collectives (P-1)/P of it; the ring
+    reduce-scatter + all-gather (P-1)/P of it per half."""
     if algo in ("ring", "ring-unfused", "ring-nccl"):
         return float(nbytes) * (world - 1)
+    if algo == "ring-rsag":
+        return 2.0 * nbytes * (world - 1) / max(world, 1)
     return float(nbytes) * (world - 1) / max(world, 1)
 
 
@@ -86,6 +91,21 @@ def ring_layout(nbytes: int, n_chunks: int, world: int, slots_policy: int):
     return n_chunks * (2 if two else 1), nbytes * (2 if two else max(world - 1, 1))
 
 
+def rsag_layout(nbytes: int, n_chunks: int, world: int):
+    """(words after the fixed signal pad, bytes of receive slots) of the reduce-scatter + all-gather ring: one arrival
+    word per chunk of a segment, world-1 segments of slots (one segment at world 1, where none is used)."""
+    return n_chunks, nbytes // world * max(world - 1, 1)
+
+
+def _layout(algo: str, C, n: int, esz: int, world: int, chunk_elems: int, slots_policy: int):
+    """(chunks that carry an arrival word, pad words, slot bytes) of ``algo``."""
+    if algo == "ring-rsag":
+        n_chunks = C.ring_num_chunks(n // world, chunk_elems, esz)
+        return (n_chunks,) + rsag_layout(n * esz, n_chunks, world)
+    n_chunks = C.ring_num_chunks(n, chunk_elems, esz)
+    return (n_chunks,) + ring_layout(n * esz, n_chunks, world, slots_policy)
+
+
 class AllreduceMiniapp:
     def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float",
                  algo: str = "ring", chunk_elems: int = 0, ctas: int = 0, timeout_s: float = 30.0,
@@ -115,13 +135,13 @@ class AllreduceMiniapp:
             raise ValueError("slots must be 0 (world-1 slots) or 2")
         self.slots_policy = slots if algo == "ring" else 0
         self.pull = bool(pull) and algo == "ring"
-        self.n_chunks = self.C.ring_num_chunks(n, chunk_elems, self.esz)
+        self.n_chunks, pad_words, slot_bytes = _layout(algo, self.C, n, self.esz, self.world, chunk_elems,
+                                                       self.slots_policy)
         self.ring_epoch = 0
         self.step_epoch = 0
         self.launches = 0
         self.va = self.vb = self.vc = self.slots = None
         self._symm = None
-        pad_words, slot_bytes = ring_layout(self.nbytes, self.n_chunks, self.world, self.slots_policy)
         if _shared is not None:         # virtual ranks of one process (VirtualAllreduce): buffers made by the group
             self.pads, self.va, self.vb, self.vc, self.slots = (_shared.get(k) for k in ("pads", "va", "vb", "vc",
                                                                                           "slots"))
@@ -136,7 +156,7 @@ class AllreduceMiniapp:
             self.pads = SignalPads(comm, device, extra_words=pad_words, timeout_s=timeout_s)
             self.va = SymmetricBuffer(comm, self.nbytes, device)
             self.vc = SymmetricBuffer(comm, self.nbytes, device)
-            if algo == "ring":
+            if algo in ("ring", "ring-rsag"):
                 self.slots = SymmetricBuffer(comm, slot_bytes, device, zero=False)
             if algo in ("ring-unfused", "ring-nccl"):
                 self.vb = SymmetricBuffer(comm, self.nbytes, device)
@@ -189,6 +209,15 @@ class AllreduceMiniapp:
                              self.pull, self.va.ptrs[self.left] if self.pull else 0,
                              self.slots.ptrs[self.left] if self.pull else 0)
             self.ring_epoch += P
+            self.launches += 1
+        elif self.algo == "ring-rsag":
+            C.ring_rsag(va=va, vc=vc, slots_local=self.slots.local_ptr, slots_right=self.slots.ptrs[self.right],
+                        vc_right=self.vc.ptrs[self.right], arrived_local=pads.chunk_word(me),
+                        arrived_right=pads.chunk_word(self.right), rank=me, world=P, n=self.n,
+                        chunk_elems=self.chunk_elems, epoch_base=self.ring_epoch, timeout_ns=pads.timeout_ns,
+                        status=pads.status_ptr, dtype=self.dtype, ctas=self.ctas, device=self.device, stream=st,
+                        phases="allreduce")
+            self.ring_epoch += C.rsag_epoch_advance(C.RSAG_ALLREDUCE, P)
             self.launches += 1
         elif self.algo == "twoshot":
             pads.barrier_epoch += 1
@@ -319,13 +348,13 @@ class VirtualAllreduce:
         self.dtype, self.device, self.n = dtype, device, n
         self.group = LocalGroup(world, [device] * world)
         policy = slots if algo == "ring" else 0
-        pad_words, slot_bytes = ring_layout(n * esz, C.ring_num_chunks(n, chunk_elems, esz), world, policy)
+        _, pad_words, slot_bytes = _layout(algo, C, n, esz, world, chunk_elems, policy)
         none = [None] * world
         pads = self.group.pads(extra_words=pad_words, timeout_s=timeout_s)
         va = self.group.symmetric(n * esz)
         vc = self.group.symmetric(n * esz)
         vb = self.group.symmetric(n * esz) if algo == "ring-unfused" else none
-        sl = self.group.symmetric(slot_bytes, zero=False) if algo == "ring" else none
+        sl = self.group.symmetric(slot_bytes, zero=False) if algo in ("ring", "ring-rsag") else none
         self.ranks: List[AllreduceMiniapp] = [
             AllreduceMiniapp(self.group.comms[r], device, dtype=dtype, algo=algo, chunk_elems=chunk_elems,
                              ctas=self.ctas, timeout_s=timeout_s, slots=slots, pull=pull, n_elems=n,
@@ -334,7 +363,8 @@ class VirtualAllreduce:
         self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, vas: List[torch.Tensor]) -> None:
-        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the rings accumulate into it)."""
+        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the rings accumulate into it;
+        ring-rsag overwrites it)."""
         td = _TORCH_DTYPE[self.dtype]
         torch.cuda.synchronize(self.device)
         for app, v in zip(self.ranks, vas):
