@@ -25,6 +25,8 @@ def gemm_put(a: torch.Tensor, b: torch.Tensor, c_local: Optional[torch.Tensor] =
     ``cluster``: 0 auto, 1 = single CTAs, 2 = CTA pairs sharing the B tile through TMA multicast.
     ``epilogue``: ``"st"`` = 128-bit stores from the consumer warps, ``"tma"`` (opt-in) = swizzled smem pieces +
     ``cp.async.bulk.tensor.2d`` stores issued by the TMA unit.
+    fp32 results below 2^-126 (subnormal) are kept exactly by both epilogues: the tensor cores do not flush them
+    (measured on an H100, tests/test_gpu_gemm_numerics.py).  bf16 output is the fp32 accumulator rounded to nearest even.
     Returns the number of CTAs launched (for ticket bookkeeping)."""
     if epilogue not in ("st", "tma"):
         raise ValueError("epilogue must be 'st' or 'tma'")
@@ -40,6 +42,8 @@ def gemm_put(a: torch.Tensor, b: torch.Tensor, c_local: Optional[torch.Tensor] =
         raise ValueError("M, N, K must be multiples of 128, 256, 64")
     if c_local is not None and (c_local.dtype != out_dtype or tuple(c_local.shape) != (m, n)):
         raise ValueError("c_local must be [M,N] of out_dtype")
+    if isinstance(c_peer, torch.Tensor) and (c_peer.dtype != out_dtype or tuple(c_peer.shape) != (m, n)):
+        raise ValueError("c_peer must be [M,N] of out_dtype")
     dev = a.device.index
     return native().gemm_put(ptr(a), ptr(b), ptr(c_local) if c_local is not None else 0,
                              ptr(c_peer) if not isinstance(c_peer, int) else c_peer, m, n, k,
@@ -75,7 +79,11 @@ def gemm_reduce_scatter(a: torch.Tensor, b: torch.Tensor, shards: Sequence[PtrLi
     ``shards`` then only tells the world size.  ``out_dtype=torch.bfloat16``: bf16 shards, ``REDG.E.ADD.BF16x8`` —
     half the NVLink bytes, every one of the P additions rounds to bf16.  ``epilogue="tma"`` (fp32 shards): the
     additions are issued by the TMA unit, one ``cp.reduce.async.bulk.tensor.2d`` per 32x32 piece staged in swizzled
-    shared memory, instead of ``REDG`` requests from the LSU (``"red"``).  Returns the CTAs launched."""
+    shared memory, instead of ``REDG`` requests from the LSU (``"red"``).
+    Subnormal fp32 sums: the ``"red"`` epilogue's ``REDG.E.ADD.F32x4.FTZ.RN`` flushes subnormal values to +-0, so a
+    shard element whose partial sums are all below 2^-126 ends as 0 where ``gemm_reference`` keeps it; the ``"tma"``
+    epilogue's ``cp.reduce.async.bulk`` keeps them exactly (both measured on an H100, tests/test_gpu_gemm_numerics.py).
+    Returns the CTAs launched."""
     if epilogue not in ("red", "tma"):
         raise ValueError("epilogue must be 'red' or 'tma'")
     _check_operands(a, b)
@@ -147,6 +155,9 @@ def allgather_gemm(a_full: torch.Tensor, a_src: Sequence[PtrLike], b: torch.Tens
         raise ValueError("c must be fp32 or bf16 [M, N]")
     if world > 1 and isinstance(ready, torch.Tensor) and (ready.dtype != torch.int32 or ready.numel() < m // 128):
         raise ValueError("ready must be int32 with one word per 128-row block")
+    for s in a_src:
+        if isinstance(s, torch.Tensor) and (s.dtype != torch.bfloat16 or s.numel() != m // world * k):
+            raise ValueError("every a_src row block must be bf16 with M/world * K elements")
     dev = a_full.device.index
     return native().allgather_gemm(ptr(a_full), [ptr(s) for s in a_src], ptr(b), ptr(c), c.dtype == torch.bfloat16,
                                    ptr(ready), ready_base, chunk_bytes, [int(f) for f in done_flags], done_epoch,

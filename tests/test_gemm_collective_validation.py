@@ -3,7 +3,7 @@ import pytest
 import torch
 
 import hpc_patterns_b200
-from hpc_patterns_b200.ops.gemm import allgather_gemm, gemm_all_to_all, gemm_reduce_scatter
+from hpc_patterns_b200.ops.gemm import allgather_gemm, gemm_all_to_all, gemm_put, gemm_reduce_scatter
 
 
 def _bf16(*shape):
@@ -28,6 +28,19 @@ def test_python_wrappers_reject_bad_operands():
         gemm_all_to_all(_bf16(256, 64), _bf16(256, 64), [torch.zeros(2, 128, 128), torch.zeros(2, 128, 256)], 0)
     with pytest.raises(TypeError):
         gemm_all_to_all(_bf16(256, 64), _bf16(256, 64), [0, 0], 0, out_dtype=torch.float16)
+    # a tensor c_peer of the wrong type or size would be written past its end
+    with pytest.raises(ValueError, match="c_peer"):
+        gemm_put(_bf16(128, 64), _bf16(256, 64), None, _bf16(128, 256))                 # bf16, out_dtype fp32
+    with pytest.raises(ValueError, match="c_peer"):
+        gemm_put(_bf16(128, 64), _bf16(256, 64), None, torch.zeros(128, 256), out_dtype=torch.bfloat16)
+    with pytest.raises(ValueError, match="c_peer"):
+        gemm_put(_bf16(256, 64), _bf16(256, 64), torch.zeros(256, 256), torch.zeros(128, 256))
+    # a short or mistyped a_src row block would be read past its end
+    with pytest.raises(ValueError, match="a_src"):
+        allgather_gemm(_bf16(256, 64), [_bf16(128, 64), _bf16(64, 64)], _bf16(256, 64), torch.zeros(256, 256), 0)
+    with pytest.raises(ValueError, match="a_src"):
+        allgather_gemm(_bf16(256, 64), [_bf16(128, 64), torch.zeros(128, 64)], _bf16(256, 64),
+                       torch.zeros(256, 256), 0)
 
 
 def test_native_launchers_reject_bad_shapes_and_modes():
