@@ -76,7 +76,7 @@ HaloTuning halo_tuning_from(const py::dict& d) {
   if (d.contains("ctas")) t.ctas = d["ctas"].cast<int>();
   if (d.contains("tile_kb")) t.tile_kb = d["tile_kb"].cast<int>();
   if (d.contains("stages")) t.stages = d["stages"].cast<int>();
-  if (d.contains("l2_hint")) t.l2_hint = d["l2_hint"].cast<int>();
+  if (d.contains("out_stages")) t.out_stages = d["out_stages"].cast<int>();
   return t;
 }
 

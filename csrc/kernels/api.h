@@ -117,9 +117,9 @@ constexpr int kHaloFlagSets = 16;    // independent flag sets (chunked launches 
 constexpr size_t kHaloFlagBytes = static_cast<size_t>(kHaloFlagSets) * 2 * kHaloMaxCtas * kHaloFlagWords * 4;
 struct HaloTuning {
   int ctas = 0;     // 0 -> every resident CTA slot (SMs x occupancy); always clamped to it
-  int tile_kb = 0;  // bytes of a row per shared-memory stage in KiB; 0 -> 16
-  int stages = 0;   // shared-memory stages (>= 6); 0 -> 6 (two CTAs per SM with 16 KiB tiles)
-  int l2_hint = 0;  // 1: L2 evict_first policy on the streaming loads / stores of the slab's own rows
+  int tile_kb = 0;     // bytes of a row per shared-memory stage in KiB (<= 32); 0 -> 16
+  int stages = 0;      // shared-memory tile slots, input ring + output ring (>= 3); 0 -> 12
+  int out_stages = 0;  // of those, the output staging ring (>= 2); 0 -> max(2, stages / 4)
 };
 struct HaloStencilArgs {
   float* u[2] = {nullptr, nullptr};                 // local field, ping-pong: step g reads u[g&1], writes u[(g+1)&1]

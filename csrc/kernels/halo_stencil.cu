@@ -21,22 +21,41 @@
 // `none` reads local halo buffers and talks to nobody: the compute kernel of the stock arm
 // (kernel -> cudaMemcpyAsync / NCCL send+recv -> host wait), which models/halo.py times next to it.
 //
-// Work split.  A CTA owns column tiles j = blockIdx.x + k * gridDim.x of EVERY row and marches down
-// the rows of a column tile, so each input tile is fetched from HBM once and used three times from
-// shared memory (as u[r+1], u[r], u[r-1]); the result of row r overwrites the tile of row r-1 in
-// place and leaves through the TMA unit.  Because a column tile is owned by the same CTA index on
-// every rank and in every step, the only cross-CTA dependency of step g+1 is "CTA c of my two
-// neighbours finished step g".  That is one monotonic word per (neighbour, CTA):
+// Work split.  A CTA owns column tiles j = blockIdx.x + k * gridDim.x of EVERY row and marches down the rows of a column
+// tile.  Each input tile is fetched once into a shared-memory input ring and read once from there, by the math warps,
+// into a register row window; the result of row r is written to a separate output staging ring and leaves through the
+// TMA unit.  Because a column tile is owned by the same CTA index on every rank and in every step, the only cross-CTA
+// dependency of step g+1 is "CTA c of my two neighbours finished step g".  That is one monotonic word per
+// (neighbour, CTA):
 //   * RAW  my step g reads the neighbour's u_g boundary tile / my halo[g&1]: written in its step g-1;
 //   * WAR  my step g overwrites u[(g+1)&1] / the neighbour's halo[(g+1)&1]: last read in its step g-1.
 // Both are "neighbour's CTA c completed step g-1", i.e. flag >= g.  So K steps run in ONE launch
 // with no grid barrier, no host sync and no per-step launch (`steps` > 1), or one launch per step
 // (`steps` == 1) with the same words carrying the dependency across launches.
 //
-// Warp roles (TMA engine, one or two CTAs per SM):
-//   warp 0 / lane 0   DMA thread: waits for the two neighbour words, streams tiles global -> smem
-//                     (mbarrier complete_tx), stores finished tiles smem -> global (+ peers), publishes.
-//   warps 1..4        math: wait full[up|centre|down], stencil in place, fence.proxy.async, arrive.
+// Load order of a column tile: boundary rows first — own row R-1, up halo, own row 0, down halo, then rows 1 .. R-2
+// (R = 2: row 1, up, row 0, down; R = 1: row 0, up, down).  Every boundary row is read twice per step by somebody: by
+// its owner as a centre row and by a neighbour as its halo (at N = 1 the neighbour is the rank itself, so up halo = own
+// row R-1 and down halo = own row 0).  With this order the two reads of a row sit next to each other, and since ranks
+// run CTA by CTA in near lock-step the second one is served from L2: a step moves 2 * rows rows through HBM, not 2 *
+// rows + 2.  L2 policy by role: interior-row loads and the local stores stream with evict_first, boundary-row loads keep
+// the default policy so that the second read finds them.
+//
+// Warp roles (one CTA per SM):
+//   warp 0 / lane 0   producer: per step, waits until this CTA's previous-step stores are performed (`stored`, a
+//                     CTA-local mbarrier: step g+1 reads what step g wrote here, which the neighbour words do not
+//                     cover at N > 1) and for the two neighbour words, then streams tiles global -> smem into the input
+//                     ring (full / empty mbarriers).  It only ever blocks on `stored`, the words and `empty`.
+//   warp 1 / lane 0   store thread: waits for a finished output slot (`ofull`), stores it smem -> global (+ the peer
+//                     puts in push mode), keeps up to two stores reading shared memory and frees a slot once
+//                     bulk_wait_read has seen its store read (`oempty`); at the end of a step bulk_wait<0>,
+//                     fence.proxy.async, releases both step words and arrives on `stored`.
+//   warps 2..9        math: each thread owns the float4 columns v = t + k * 256 of the tile.  Per column it reads each
+//                     input tile once into registers (row R-1 and the down halo are kept aside), frees the slot, and
+//                     writes stencil1(up, ce, dn) of row r into the output ring, rows 0 .. R-1 in order.  An interior
+//                     lower row is read and consumed in the same pass, so only four rows are live per thread.
+// Ordering: every step-g load has been read by the math warps before the last step-g result exists, so before the last
+// step-g store is issued; step-g+1 loads are issued only after `stored` (own step-g stores performed) and the words.
 #include "api.h"
 
 #include <algorithm>
@@ -50,8 +69,13 @@ namespace hpcp {
 
 namespace {
 
-constexpr int kHaloMathWarps = 4;
-constexpr int kHaloThreads = 32 * (1 + kHaloMathWarps);
+constexpr int kHaloMathWarps = 8;
+constexpr int kHaloMathThreads = 32 * kHaloMathWarps;
+constexpr int kHaloThreads = 32 * (2 + kHaloMathWarps);
+constexpr int kHaloVec = 8;  // float4 per math thread and tile row: the register window covers tiles up to 32 KiB
+constexpr uint32_t kHaloMaxTileBytes = 16u * kHaloVec * kHaloMathThreads;
+constexpr int kHaloDefaultTileKb = 16;
+constexpr int kHaloDefaultStages = 12;  // 9 input + 3 output slots of 16 KiB
 
 struct HaloParams {
   unsigned char* u[2];
@@ -68,8 +92,7 @@ struct HaloParams {
   size_t row_bytes;
   size_t tile_begin, tile_end;      // column tiles [begin, end) of a row handled by this launch
   uint32_t tile_bytes;
-  int stages;
-  int l2_hint;                      // 1: L2 evict_first policy on the local streaming loads and stores (used once)
+  int in_stages, out_stages;        // input ring and output staging ring, in tiles
   float alpha, s;
   uint32_t step_base;
   int steps;
@@ -88,25 +111,29 @@ __device__ __forceinline__ float4 stencil4(const float4& up, const float4& ce, c
                      stencil1(up.z, ce.z, dn.z, alpha, s), stencil1(up.w, ce.w, dn.w, alpha, s));
 }
 
+// Row of the q-th load of a column tile (q = 0 .. R+1), boundary rows first; -1 is the up halo, R the down halo.
+__device__ __forceinline__ int halo_load_row(int q, int R) {
+  if (q == 0) return R - 1;
+  if (q == 1) return -1;
+  if (R == 1) return 1;  // q == 2: the down halo
+  if (q == 2) return 0;
+  if (q == 3) return R;
+  return q - 3;
+}
+
 // Cursor into a ring of S mbarrier-guarded slots: slot index + the phase parity of its current use.
 struct Ring {
   int slot;
   uint32_t phase;
-  __device__ __forceinline__ void advance(int n, int S) {  // n < S
-    slot += n;
-    if (slot >= S) {
-      slot -= S;
+  __device__ __forceinline__ void advance(int S) {
+    if (++slot == S) {
+      slot = 0;
       phase ^= 1u;
     }
   }
-  __device__ __forceinline__ Ring at(int n, int S) const {
-    Ring r = *this;
-    r.advance(n, S);
-    return r;
-  }
 };
 
-// mbarrier wait that gives up when the DMA thread reported a dead peer.
+// mbarrier wait that gives up when the producer reported a dead peer.
 __device__ __forceinline__ bool mbar_wait_or_abort(uint64_t* bar, uint32_t parity, const volatile int* abort_w) {
   while (!ptx::mbar_try_wait(bar, parity)) {
     if (*abort_w != 0) return false;
@@ -114,21 +141,114 @@ __device__ __forceinline__ bool mbar_wait_or_abort(uint64_t* bar, uint32_t parit
   return true;
 }
 
+// One tile row of a math thread's columns, kept in registers.
+struct RowRegs {
+  float4 v[kHaloVec];
+};
+
+// The math warps' side of both rings.
+struct MathPipe {
+  unsigned char* in_base;
+  unsigned char* out_base;
+  uint64_t* full;
+  uint64_t* empty;
+  uint64_t* ofull;
+  uint64_t* oempty;
+  const volatile int* abort_w;
+  uint32_t T;
+  int S_in, S_out;
+  int mt;
+  Ring in, out;
+
+  // Wait for the next input tile, copy this thread's part into `dst`, free the slot.
+  __device__ __forceinline__ bool read(RowRegs& dst, uint32_t nv) {
+    if (!mbar_wait_or_abort(&full[in.slot], in.phase, abort_w)) return false;
+    const float4* t = reinterpret_cast<const float4*>(in_base + static_cast<size_t>(in.slot) * T);
+#pragma unroll
+    for (int k = 0; k < kHaloVec; ++k) {
+      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
+      if (v < nv) dst.v[k] = t[v];
+    }
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&empty[in.slot]);
+    in.advance(S_in);
+    return true;
+  }
+  // Wait for a free output slot.
+  __device__ __forceinline__ bool acquire_out() {
+    return mbar_wait_or_abort(&oempty[out.slot], out.phase ^ 1u, abort_w);
+  }
+  // The math warps' writes to the output slot -> visible to the TMA store; hand the slot to the store thread.
+  __device__ __forceinline__ void publish_out() {
+    ptx::fence_proxy_async_smem();
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&ofull[out.slot]);
+    out.advance(S_out);
+  }
+  __device__ __forceinline__ float4* out_tile() const {
+    return reinterpret_cast<float4*>(out_base + static_cast<size_t>(out.slot) * T);
+  }
+  // Output row from three rows held in registers.
+  __device__ __forceinline__ bool write(const RowRegs& up, const RowRegs& ce, const RowRegs& dn, uint32_t nv,
+                                        float alpha, float s) {
+    if (!acquire_out()) return false;
+    float4* t = out_tile();
+#pragma unroll
+    for (int k = 0; k < kHaloVec; ++k) {
+      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
+      if (v < nv) t[v] = stencil4(up.v[k], ce.v[k], dn.v[k], alpha, s);
+    }
+    publish_out();
+    return true;
+  }
+  // Output row whose lower neighbour is the next input tile, read straight into the window: up <- ce <- next tile.
+  // Only four rows are live in the math warps (up, ce and the two saved boundary rows).
+  __device__ __forceinline__ bool read_write(RowRegs& up, RowRegs& ce, uint32_t nv, float alpha, float s) {
+    if (!mbar_wait_or_abort(&full[in.slot], in.phase, abort_w) || !acquire_out()) return false;
+    const float4* src = reinterpret_cast<const float4*>(in_base + static_cast<size_t>(in.slot) * T);
+    float4* t = out_tile();
+#pragma unroll
+    for (int k = 0; k < kHaloVec; ++k) {
+      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
+      if (v < nv) {
+        const float4 dn = src[v];
+        t[v] = stencil4(up.v[k], ce.v[k], dn, alpha, s);
+        up.v[k] = ce.v[k];
+        ce.v[k] = dn;
+      }
+    }
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&empty[in.slot]);
+    in.advance(S_in);
+    publish_out();
+    return true;
+  }
+};
+
 // kMode: 0 none, 1 pull, 2 push.
 template <int kMode>
-__global__ void __launch_bounds__(kHaloThreads) halo_stencil_kernel(const HaloParams p) {
+__global__ void __launch_bounds__(kHaloThreads, 1) halo_stencil_kernel(const HaloParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t T = p.tile_bytes;
-  const int S = p.stages;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(S) * T);
-  uint64_t* computed = full + S;
-  volatile int* abort_w = reinterpret_cast<volatile int*>(computed + S);
+  const int S_in = p.in_stages, S_out = p.out_stages;
+  unsigned char* out_base = smem + static_cast<size_t>(S_in) * T;
+  uint64_t* full = reinterpret_cast<uint64_t*>(out_base + static_cast<size_t>(S_out) * T);
+  uint64_t* empty = full + S_in;
+  uint64_t* ofull = empty + S_in;
+  uint64_t* oempty = ofull + S_out;
+  uint64_t* stored = oempty + S_out;
+  volatile int* abort_w = reinterpret_cast<volatile int*>(stored + 1);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < S; ++i) {
+    for (int i = 0; i < S_in; ++i) {
       ptx::mbar_init(&full[i], 1);
-      ptx::mbar_init(&computed[i], kHaloMathWarps);
+      ptx::mbar_init(&empty[i], kHaloMathWarps);
     }
+    for (int i = 0; i < S_out; ++i) {
+      ptx::mbar_init(&ofull[i], kHaloMathWarps);
+      ptx::mbar_init(&oempty[i], 1);
+    }
+    ptx::mbar_init(stored, 1);
     *abort_w = 0;
     ptx::fence_mbar_init();
   }
@@ -138,8 +258,6 @@ __global__ void __launch_bounds__(kHaloThreads) halo_stencil_kernel(const HaloPa
   const size_t n_tiles = p.tile_end - p.tile_begin;
   const size_t ncols = n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   if (ncols == 0) return;  // same geometry on every rank: nobody waits for this CTA index
-  const uint64_t loads_per_step = ncols * static_cast<uint64_t>(R + 2);
-  const uint64_t comps_per_step = ncols * static_cast<uint64_t>(R);
   auto col_off = [&](size_t jj) { return (p.tile_begin + blockIdx.x + jj * gridDim.x) * static_cast<size_t>(T); };
   auto col_len = [&](size_t off) {
     return static_cast<uint32_t>(p.row_bytes - off < T ? p.row_bytes - off : T);
@@ -148,14 +266,13 @@ __global__ void __launch_bounds__(kHaloThreads) halo_stencil_kernel(const HaloPa
   const int warp = threadIdx.x >> 5;
   if (warp == 0) {
     if (threadIdx.x != 0) return;
-    // ------------------------------------------------------------------ DMA thread ----
-    const uint64_t policy = p.l2_hint ? ptx::l2_policy_evict_first() : 0;
-    Ring ld{0, 0};    // next tile to load
-    Ring st{0, 0};    // tile the next finished row overwrote (= the next one to store)
-    Ring done{0, 0};  // next `computed` barrier to consume
+    // ------------------------------------------------------------------ producer ----
+    const uint64_t evict_first = ptx::l2_policy_evict_first();
+    Ring ld{0, 0};
     for (int si = 0; si < p.steps; ++si) {
       const uint32_t g = p.step_base + static_cast<uint32_t>(si);
-      const int in = static_cast<int>(g & 1u), out = in ^ 1;
+      const int in = static_cast<int>(g & 1u);
+      if (si > 0) ptx::mbar_wait(stored, static_cast<uint32_t>(si - 1) & 1u);  // own step g-1 stores performed
       if (kMode != 0) {
         const bool ok = wait_epoch(p.wait_lo + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status) &&
                         wait_epoch(p.wait_hi + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status);
@@ -166,104 +283,90 @@ __global__ void __launch_bounds__(kHaloThreads) halo_stencil_kernel(const HaloPa
         asm volatile("fence.proxy.async;" ::: "memory");  // acquired peer data -> visible to the bulk loads
       }
       const unsigned char* uin = p.u[in];
+      for (size_t jj = 0; jj < ncols; ++jj) {
+        const size_t off = col_off(jj);
+        const uint32_t len = col_len(off);
+        for (int q = 0; q < R + 2; ++q) {
+          const int row = halo_load_row(q, R);
+          const unsigned char* src = row < 0    ? p.up_src[in] + off
+                                     : row == R ? p.dn_src[in] + off
+                                                : uin + static_cast<size_t>(row) * p.row_bytes + off;
+          ptx::mbar_wait(&empty[ld.slot], ld.phase ^ 1u);
+          unsigned char* dst = smem + static_cast<size_t>(ld.slot) * T;
+          ptx::mbar_arrive_expect_tx(&full[ld.slot], len);
+          if (row > 0 && row < R - 1)  // interior: read once per step, never again through L2
+            ptx::bulk_g2s_hint(dst, src, len, &full[ld.slot], evict_first);
+          else  // boundary rows: read twice per step, back to back
+            ptx::bulk_g2s(dst, src, len, &full[ld.slot]);
+          ld.advance(S_in);
+        }
+      }
+    }
+  } else if (warp == 1) {
+    if (threadIdx.x != 32) return;
+    // ------------------------------------------------------------------ store thread ----
+    const uint64_t evict_first = ptx::l2_policy_evict_first();
+    // Store groups left reading shared memory after each commit; the math warps keep at least one free slot.
+    const int lag = S_out >= 3 ? 2 : 1;
+    Ring st{0, 0};
+    for (int si = 0; si < p.steps; ++si) {
+      const uint32_t g = p.step_base + static_cast<uint32_t>(si);
+      const int out = static_cast<int>(g & 1u) ^ 1;
       unsigned char* uout = p.u[out];
-      const unsigned char* up_src = p.up_src[in];
-      const unsigned char* dn_src = p.dn_src[in];
-      uint64_t issued = 0, retired = 0;  // tiles of THIS step, in load order
-      size_t jj_l = 0;                   // load cursor: column tile, row slot m = row + 1
-      int m_l = 0;
-      auto issue_next = [&]() {
-        const size_t off = col_off(jj_l);
+      uint64_t n = 0;  // stores issued in this step; slots are used in ring order
+      for (size_t jj = 0; jj < ncols; ++jj) {
+        const size_t off = col_off(jj);
         const uint32_t len = col_len(off);
-        const unsigned char* src = m_l == 0       ? up_src + off
-                                   : m_l == R + 1 ? dn_src + off
-                                                  : uin + static_cast<size_t>(m_l - 1) * p.row_bytes + off;
-        ptx::mbar_arrive_expect_tx(&full[ld.slot], len);
-        if (p.l2_hint && m_l != 0 && m_l != R + 1)  // own rows: streamed once, never re-read through L2
-          ptx::bulk_g2s_hint(smem + static_cast<size_t>(ld.slot) * T, src, len, &full[ld.slot], policy);
-        else
-          ptx::bulk_g2s(smem + static_cast<size_t>(ld.slot) * T, src, len, &full[ld.slot]);
-        ld.advance(1, S);
-        ++issued;
-        if (++m_l == R + 2) {
-          m_l = 0;
-          ++jj_l;
-        }
-      };
-      size_t jj_c = 0;  // compute cursor
-      int r = 0;
-      uint64_t i0 = 0;  // tile (in load order) that row r of column jj_c overwrites
-      for (uint64_t c = 0; c < comps_per_step; ++c) {
-        while (issued < loads_per_step && issued < retired + static_cast<uint64_t>(S)) issue_next();
-        if (!mbar_wait_or_abort(&computed[done.slot], done.phase, abort_w)) return;
-        done.advance(1, S);
-        const size_t off = col_off(jj_c);
-        const uint32_t len = col_len(off);
-        const unsigned char* sa = smem + static_cast<size_t>(st.slot) * T;
-        // interior rows are not read again before the next step has streamed the whole slab through L2; the boundary
-        // rows are what the neighbours pull, leave them to the default policy
-        if (p.l2_hint && r != 0 && r != R - 1)
-          ptx::bulk_s2g_hint(uout + static_cast<size_t>(r) * p.row_bytes + off, sa, len, policy);
-        else
-          ptx::bulk_s2g(uout + static_cast<size_t>(r) * p.row_bytes + off, sa, len);
-        if (kMode == 2) {
-          if (r == 0) ptx::bulk_s2g(p.put_first[out] + off, sa, len);
-          if (r == R - 1) ptx::bulk_s2g(p.put_last[out] + off, sa, len);
-        }
-        ptx::bulk_commit();
-        ptx::bulk_wait_read<1>();  // every store but the newest has left shared memory
-        retired = i0;              // tiles [0, i0) are free (incl. the two never-stored tiles of a finished column)
-        if (++r == R) {            // next column: skip the centre-last and down-halo tiles
-          r = 0;
-          ++jj_c;
-          i0 += 3;
-          st.advance(3, S);
-        } else {
-          i0 += 1;
-          st.advance(1, S);
+        for (int r = 0; r < R; ++r) {
+          if (!mbar_wait_or_abort(&ofull[st.slot], st.phase, abort_w)) return;
+          const unsigned char* sa = out_base + static_cast<size_t>(st.slot) * T;
+          ptx::bulk_s2g_hint(uout + static_cast<size_t>(r) * p.row_bytes + off, sa, len, evict_first);
+          if (kMode == 2) {
+            if (r == 0) ptx::bulk_s2g(p.put_first[out] + off, sa, len);
+            if (r == R - 1) ptx::bulk_s2g(p.put_last[out] + off, sa, len);
+          }
+          ptx::bulk_commit();
+          // every store group but the `lag` newest has left shared memory: free the slot of the one just before them
+          if (lag == 2)
+            ptx::bulk_wait_read<2>();
+          else
+            ptx::bulk_wait_read<1>();
+          if (n >= static_cast<uint64_t>(lag)) ptx::mbar_arrive(&oempty[(st.slot + S_out - lag) % S_out]);
+          ++n;
+          st.advance(S_out);
         }
       }
       ptx::bulk_wait<0>();  // this step's stores are performed (local field and, in push mode, the peers' halos)
+      for (int k = n < static_cast<uint64_t>(lag) ? static_cast<int>(n) : lag; k >= 1; --k)
+        ptx::mbar_arrive(&oempty[(st.slot + S_out - k) % S_out]);
       asm volatile("fence.proxy.async;" ::: "memory");
       if (kMode != 0) {
         ptx::fence_acq_rel_sys();
         ptx::st_release_sys(p.signal_hi + blockIdx.x * kHaloFlagWords, g + 1u);
         ptx::st_release_sys(p.signal_lo + blockIdx.x * kHaloFlagWords, g + 1u);
       }
+      ptx::mbar_arrive(stored);  // the producer may load what this step wrote
     }
   } else {
     // ------------------------------------------------------------------ math warps ----
-    const int mt = static_cast<int>(threadIdx.x) - 32;
     const float alpha = p.alpha, s = p.s;
-    Ring up_t{0, 0};  // tile of row r-1 (overwritten with the result of row r)
-    Ring done{0, 0};
+    MathPipe mp{smem, out_base, full, empty, ofull, oempty, abort_w, T, S_in, S_out,
+                static_cast<int>(threadIdx.x) - 64, {0, 0}, {0, 0}};
+    RowRegs last, up, ce, dnh;
     for (int si = 0; si < p.steps; ++si) {
-      size_t jj = 0;
-      int r = 0;
-      for (uint64_t c = 0; c < comps_per_step; ++c) {
-        const Ring ce_t = up_t.at(1, S), dn_t = up_t.at(2, S);
-        if (r == 0) {
-          if (!mbar_wait_or_abort(&full[up_t.slot], up_t.phase, abort_w)) return;
-          if (!mbar_wait_or_abort(&full[ce_t.slot], ce_t.phase, abort_w)) return;
-        }
-        if (!mbar_wait_or_abort(&full[dn_t.slot], dn_t.phase, abort_w)) return;
-        float4* up = reinterpret_cast<float4*>(smem + static_cast<size_t>(up_t.slot) * T);
-        const float4* ce = reinterpret_cast<const float4*>(smem + static_cast<size_t>(ce_t.slot) * T);
-        const float4* dn = reinterpret_cast<const float4*>(smem + static_cast<size_t>(dn_t.slot) * T);
+      for (size_t jj = 0; jj < ncols; ++jj) {
         const uint32_t nv = col_len(col_off(jj)) / 16;
-#pragma unroll 4
-        for (uint32_t v = mt; v < nv; v += 32 * kHaloMathWarps) up[v] = stencil4(up[v], ce[v], dn[v], alpha, s);
-        ptx::fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA store
-        __syncwarp();
-        if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&computed[done.slot]);
-        done.advance(1, S);
-        if (++r == R) {
-          r = 0;
-          ++jj;
-          up_t.advance(3, S);
-        } else {
-          up_t.advance(1, S);
+        // loads in halo_load_row order: row R-1 (row 0 when R == 1), up halo, [row 0,] down halo, rows 1 .. R-2
+        if (!mp.read(last, nv) || !mp.read(up, nv)) return;
+        if (R == 1) {
+          if (!mp.read(dnh, nv) || !mp.write(up, last, dnh, nv, alpha, s)) return;
+          continue;
         }
+        if (!mp.read(ce, nv) || !mp.read(dnh, nv)) return;
+        for (int r = 0; r + 2 < R; ++r)  // rows 0 .. R-3: the lower neighbour is the next interior row
+          if (!mp.read_write(up, ce, nv, alpha, s)) return;
+        if (!mp.write(up, ce, last, nv, alpha, s)) return;   // row R-2
+        if (!mp.write(ce, last, dnh, nv, alpha, s)) return;  // row R-1
       }
     }
   }
@@ -348,7 +451,7 @@ __global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const f
 
 struct HaloGeometry {
   uint32_t tile_bytes;
-  int stages;
+  int in_stages, out_stages;
   size_t smem;
   int ctas;
 };
@@ -381,10 +484,16 @@ int occupancy_of(size_t smem) {
 
 HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device) {
   HaloGeometry g;
-  g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : 16) * 1024);
-  g.stages = tune.stages > 0 ? tune.stages : 6;  // 6 x 16 KiB: two CTAs per SM
-  HPCP_REQUIRE(g.stages >= 6, "halo_stencil: needs >= 6 shared-memory stages");
-  g.smem = static_cast<size_t>(g.stages) * g.tile_bytes + static_cast<size_t>(g.stages) * 16 + 16;
+  g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : kHaloDefaultTileKb) * 1024);
+  HPCP_REQUIRE(g.tile_bytes <= kHaloMaxTileBytes, "halo_stencil: tiles of at most 32 KiB (the math warps' registers)");
+  // `stages` counts every tile slot in shared memory: the input ring plus the output staging ring.
+  const int stages = tune.stages > 0 ? tune.stages : kHaloDefaultStages;
+  g.out_stages = tune.out_stages > 0 ? tune.out_stages : std::max(2, stages / 4);
+  g.in_stages = stages - g.out_stages;
+  // The store thread keeps its newest slot until the next store's bulk_wait_read: one output slot would deadlock.
+  HPCP_REQUIRE(g.out_stages >= 2 && g.in_stages >= 1,
+               "halo_stencil: needs >= 2 output and >= 1 input shared-memory stages");
+  g.smem = static_cast<size_t>(stages) * g.tile_bytes + static_cast<size_t>(2 * stages + 1) * 8 + 16;
   HPCP_REQUIRE(g.smem <= 227 * 1024, "halo_stencil: stages * tile exceed 227 KiB of shared memory");
   const int sms = device_sm_count(device);
   int per_sm = 1;
@@ -449,8 +558,8 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
   p.tile_end = a.tile_end == 0 ? tiles_per_row : a.tile_end;
   HPCP_REQUIRE(p.tile_begin < p.tile_end && p.tile_end <= tiles_per_row, "halo_stencil: bad column-tile range");
   p.tile_bytes = g.tile_bytes;
-  p.stages = g.stages;
-  p.l2_hint = tune.l2_hint;
+  p.in_stages = g.in_stages;
+  p.out_stages = g.out_stages;
   p.alpha = a.alpha;
   p.s = a.s;
   p.step_base = a.step_base;

@@ -63,8 +63,7 @@ void print_help() {
                "                    their halo buffers — both from inside the stencil kernel\n"
                " --per-step    one launch per step instead of one persistent K-step launch\n"
                " --stock memcpy     the reference's shape through stock calls: kernel; wait; copies; wait\n"
-               " --ctas N --tile-kb N --stages N   kernel geometry\n"
-               " --l2-hint             evict_first L2 policy on the slab's own streaming loads / stores\n"
+               " --ctas N --tile-kb N --stages N --out-stages N   kernel geometry (stages: input + output ring)\n"
                " --json FILE   append one JSON row\n"
                " --cpu         no GPU: ranks are host threads, the exchange is a memcpy into (push) or a read out of\n"
                "               (pull) the neighbours' arrays, one barrier per step: options, ring order, verification\n"
@@ -345,7 +344,7 @@ int main(int argc, char** argv) {
         {"per-step", no_argument, nullptr, 7}, {"stock", required_argument, nullptr, 8},
         {"ctas", required_argument, nullptr, 9}, {"tile-kb", required_argument, nullptr, 10},
         {"stages", required_argument, nullptr, 11}, {"json", required_argument, nullptr, 12},
-        {"l2-hint", no_argument, nullptr, 13}, {"cpu", no_argument, nullptr, 14},
+        {"out-stages", required_argument, nullptr, 13}, {"cpu", no_argument, nullptr, 14},
         {"dump", required_argument, nullptr, 15}, {"help", no_argument, nullptr, 'h'}, {nullptr, 0, nullptr, 0}};
     int opt;
     while ((opt = getopt_long(argc, argv, "hn:", long_opts, nullptr)) != -1) {
@@ -364,7 +363,7 @@ int main(int argc, char** argv) {
         case 10: cfg.tune.tile_kb = std::atoi(optarg); break;
         case 11: cfg.tune.stages = std::atoi(optarg); break;
         case 12: cfg.json_path = optarg; break;
-        case 13: cfg.tune.l2_hint = 1; break;
+        case 13: cfg.tune.out_stages = std::atoi(optarg); break;
         case 14: cfg.cpu = true; break;
         case 15: cfg.dump_path = optarg; break;
         default: print_help(); return 1;
