@@ -43,6 +43,7 @@ cli: $(CLIS) aliases
 #   omp_host_threads / omp_nowait (one build per mode upstream, run_omp.sh:6-7; the mode is argv[1] here).
 aliases: $(CLIS)
 	@for n in allreduce.float allreduce.int allreduce.double allreduce.long allreduce.short allreduce.uint allreduce.uchar \
+	          allreduce.bfloat16 allreduce.half \
 	          allreduce-mpi-sycl.float allreduce-mpi-sycl.int \
 	          allreduce-usm-mpi-omp-offload.float allreduce-map-mpi-omp-offload.float; do ln -sf allreduce bin/$$n; done
 	@ln -sf peer2pear bin/peer2pear_i; ln -sf peer2pear bin/peer2pear_w

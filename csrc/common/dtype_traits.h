@@ -9,7 +9,15 @@
 // SUM kernels here (ring, accumulate, two-shot: csrc/kernels/ring_allreduce.cu);
 // `long double` has no device representation on NVIDIA GPUs and, like any other
 // type, falls back to "bytes" (copy-only), the analogue of MPI_BYTE.
+// The two 16-bit floating types MPICH adds as MPIX_C_BF16 / MPIX_C_FLOAT16
+// (__nv_bfloat16, __half) have SUM kernels too: the rings round every add to the
+// 16-bit format, two-shot accumulates in fp32 and rounds once (docs/allreduce.md).
+// cuda_bf16.h / cuda_fp16.h also compile as plain host C++ (g++), so the host-only
+// users of this header need nothing beyond the CUDA include directory.
 #pragma once
+
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <cstddef>
 #include <cstdint>
@@ -49,6 +57,8 @@ HPCP_DTYPE(unsigned long long, "unsigned long", true, ElemType::kULong, "uint64"
 HPCP_DTYPE(short, "short", true, ElemType::kShort, "int16");
 HPCP_DTYPE(unsigned short, "unsigned short", true, ElemType::kUShort, "uint16");
 HPCP_DTYPE(unsigned char, "unsigned char", true, ElemType::kUChar, "uint8");
+HPCP_DTYPE(__nv_bfloat16, "bfloat16", true, ElemType::kBFloat16, "bfloat16");
+HPCP_DTYPE(__half, "half", true, ElemType::kHalf, "float16");
 #undef HPCP_DTYPE
 
 template <typename T>
@@ -76,6 +86,9 @@ inline bool elem_type_from_name(const std::string& name, ElemType* out) {
       {"u16", ElemType::kUShort},
       {"uchar", ElemType::kUChar},    {"unsigned char", ElemType::kUChar}, {"uint8", ElemType::kUChar},
       {"u8", ElemType::kUChar},
+      {"bfloat16", ElemType::kBFloat16}, {"bf16", ElemType::kBFloat16},
+      {"half", ElemType::kHalf},      {"float16", ElemType::kHalf},        {"f16", ElemType::kHalf},
+      {"fp16", ElemType::kHalf},
   };
   for (const Row& r : rows)
     if (name == r.name) {
@@ -95,6 +108,8 @@ inline const char* elem_type_name(ElemType t) {
     case ElemType::kShort: return "short";
     case ElemType::kUShort: return "ushort";
     case ElemType::kUChar: return "uchar";
+    case ElemType::kBFloat16: return "bfloat16";
+    case ElemType::kHalf: return "half";
   }
   return "?";
 }

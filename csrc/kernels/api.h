@@ -284,13 +284,15 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
 // ------------------------------------------------------ allreduce miniapp ----
 // Element types of the miniapp's arrays (↔ mpi::get_datatype<T>(), mpi_datatype.hpp:28-51: every one of them is usable
 // with MPI_SUM upstream).  Kernels are instantiated per ADDITION CLASS: signed and unsigned integers of one width share
-// the two's-complement add.
+// the two's-complement add.  kBFloat16 / kHalf (↔ MPICH's MPIX_C_BF16 / MPIX_C_FLOAT16) add with one round-to-nearest-even
+// per add in the 16-bit format (rings), or accumulate in fp32 and round once (two-shot).
 enum class ElemType : int {
-  kFloat = 0, kInt = 1, kUInt = 2, kDouble = 3, kLong = 4, kULong = 5, kShort = 6, kUShort = 7, kUChar = 8
+  kFloat = 0, kInt = 1, kUInt = 2, kDouble = 3, kLong = 4, kULong = 5, kShort = 6, kUShort = 7, kUChar = 8,
+  kBFloat16 = 9, kHalf = 10
 };
 constexpr size_t elem_size(ElemType t) {
   return t == ElemType::kDouble || t == ElemType::kLong || t == ElemType::kULong ? 8
-         : t == ElemType::kShort || t == ElemType::kUShort                       ? 2
+         : t == ElemType::kShort || t == ElemType::kUShort || t == ElemType::kBFloat16 || t == ElemType::kHalf ? 2
          : t == ElemType::kUChar                                                 ? 1
                                                                                  : 4;
 }

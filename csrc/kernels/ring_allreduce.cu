@@ -25,6 +25,9 @@
 // multicast mapping exists.
 #include "api.h"
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include <algorithm>
 #include <cstdlib>
 #include <initializer_list>
@@ -89,6 +92,79 @@ struct Vec4<unsigned char> {  // sixteen 8-bit lanes
     return make_uint4(__vadd4(a.x, b.x), __vadd4(a.y, b.y), __vadd4(a.z, b.z), __vadd4(a.w, b.w));
   }
 };
+// Eight 16-bit floating lanes, two per 32-bit word (H2 = __nv_bfloat162 / __half2): every lane is ONE add rounded to
+// nearest even in the 16-bit format, subnormal results kept (HFMA2.BF16_V2 a, 1, b / HFMA2 without .FTZ).
+template <typename H2>
+struct Vec4Pairs {
+  static __device__ __forceinline__ uint32_t add2(uint32_t a, uint32_t b) {
+    const H2 s = __hadd2_rn(*reinterpret_cast<const H2*>(&a), *reinterpret_cast<const H2*>(&b));
+    return *reinterpret_cast<const uint32_t*>(&s);
+  }
+  static __device__ __forceinline__ uint4 add(const uint4& a, const uint4& b) {
+    return make_uint4(add2(a.x, b.x), add2(a.y, b.y), add2(a.z, b.z), add2(a.w, b.w));
+  }
+};
+template <>
+struct Vec4<__nv_bfloat16> : Vec4Pairs<__nv_bfloat162> {};
+template <>
+struct Vec4<__half> : Vec4Pairs<__half2> {};
+
+// 16-bit floating types: two-shot accumulates them in fp32 and rounds once (two_shot_f32_kernel).
+template <typename T>
+constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
+
+// The eight lanes of a 16-byte vector of T (bf16 or fp16) as fp32 partial sums: set / add widen exactly, round()
+// rounds every lane once to nearest even in T (F2FP.*.F32.PACK_AB).  The fp32 adds are IEEE (no FTZ).
+template <typename T>
+struct Acc8;
+template <>
+struct Acc8<__nv_bfloat16> {
+  static __device__ __forceinline__ float2 widen(uint32_t u) {
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
+  }
+  static __device__ __forceinline__ uint32_t narrow(float lo, float hi) {
+    const __nv_bfloat162 r = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&r);
+  }
+};
+template <>
+struct Acc8<__half> {
+  static __device__ __forceinline__ float2 widen(uint32_t u) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&u));
+  }
+  static __device__ __forceinline__ uint32_t narrow(float lo, float hi) {
+    const __half2 r = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&r);
+  }
+};
+template <typename T>
+struct Sum8 {
+  float2 v[4];
+  __device__ __forceinline__ void set(const uint4& a) {
+    v[0] = Acc8<T>::widen(a.x), v[1] = Acc8<T>::widen(a.y), v[2] = Acc8<T>::widen(a.z), v[3] = Acc8<T>::widen(a.w);
+  }
+  __device__ __forceinline__ void add(const uint4& a) {
+    const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 f = Acc8<T>::widen(w[k]);
+      v[k].x = __fadd_rn(v[k].x, f.x);
+      v[k].y = __fadd_rn(v[k].y, f.y);
+    }
+  }
+  __device__ __forceinline__ uint4 round() const {
+    return make_uint4(Acc8<T>::narrow(v[0].x, v[0].y), Acc8<T>::narrow(v[1].x, v[1].y),
+                      Acc8<T>::narrow(v[2].x, v[2].y), Acc8<T>::narrow(v[3].x, v[3].y));
+  }
+};
+
+// Element -> double for the mismatch count (the 16-bit floats convert through their exact fp32 value).
+template <typename T>
+__device__ __forceinline__ double to_double(T x) {
+  return static_cast<double>(x);
+}
+__device__ __forceinline__ double to_double(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ double to_double(__half x) { return __half2float(x); }
 
 // C++ element type -> the addition class its kernels are instantiated for.
 template <typename T> struct AddClass { using type = T; };
@@ -109,9 +185,11 @@ void dispatch_elem(ElemType t, F&& f) {
     case ElemType::kShort: f(static_cast<short>(0)); break;
     case ElemType::kUShort: f(static_cast<unsigned short>(0)); break;
     case ElemType::kUChar: f(static_cast<unsigned char>(0)); break;
+    case ElemType::kBFloat16: f(__nv_bfloat16{}); break;
+    case ElemType::kHalf: f(__half{}); break;
   }
 }
-// Run f(C{}) with the addition class of `t` (six kernel instantiations instead of nine).
+// Run f(C{}) with the addition class of `t` (eight kernel instantiations instead of eleven).
 template <typename F>
 void dispatch_add_class(ElemType t, F&& f) {
   dispatch_elem(t, [&](auto tag) { f(typename AddClass<decltype(tag)>::type{}); });
@@ -143,7 +221,7 @@ __global__ void count_mismatch_kernel(const T* __restrict__ v, size_t n, double 
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   unsigned long long bad = 0;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const double d = static_cast<double>(__ldcg(v + i)) - expected;
+    const double d = to_double(__ldcg(v + i)) - expected;
     bad += !(d < 1e-6 && d > -1e-6);
   }
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
@@ -458,6 +536,54 @@ __global__ void __launch_bounds__(512) two_shot_kernel(const __grid_constant__ T
                          a.timeout_ns, a.status);
 }
 
+// Two-shot for the 16-bit floating types: same loads, stores and barrier as two_shot_kernel, but every lane is widened
+// to fp32 and the P inputs are added owner first, ((VA[s] + VA[s+1]) + ...) + VA[s+P-1] (ranks mod P), in the main
+// blocks and in the tail loop alike; the sum is rounded once to T.  One rounding instead of the ring's P-1.
+template <typename T, int W, int U>
+__global__ void __launch_bounds__(512) two_shot_f32_kernel(const __grid_constant__ TwoShotDev a) {
+  const size_t base = static_cast<size_t>(a.rank) * a.slice_vec;
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  const size_t block_vec = static_cast<size_t>(blockDim.x) * U;
+  const size_t n_blocks = a.slice_vec / block_vec;
+  for (size_t blk = blockIdx.x; blk < n_blocks; blk += gridDim.x) {
+    const size_t i = blk * block_vec + threadIdx.x;
+    uint4 x[W][U];
+#pragma unroll
+    for (int q = 0; q < W; ++q)
+      if (q < a.world) {
+        const int p = (a.rank + q) % a.world;  // owner first: the summation order
+#pragma unroll
+        for (int u = 0; u < U; ++u) x[q][u] = ptx::ld_peer_v4(a.va[p] + base + i + u * blockDim.x);
+      }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      Sum8<T> s;
+      s.set(x[0][u]);
+#pragma unroll
+      for (int q = 1; q < W; ++q)
+        if (q < a.world) s.add(x[q][u]);
+      x[0][u] = s.round();
+    }
+#pragma unroll
+    for (int q = 0; q < W; ++q)
+      if (q < a.world) {
+        const int p = (a.rank + q) % a.world;
+#pragma unroll
+        for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[p] + base + i + u * blockDim.x, x[0][u]);
+      }
+  }
+  size_t i = n_blocks * block_vec + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  for (; i < a.slice_vec; i += stride) {
+    Sum8<T> s;
+    s.set(ptx::ld_peer_v4(a.va[a.rank] + base + i));
+    for (int q = 1; q < a.world; ++q) s.add(ptx::ld_peer_v4(a.va[(a.rank + q) % a.world] + base + i));
+    const uint4 r = s.round();
+    for (int p = 0; p < a.world; ++p) ptx::st_stream_v4(a.vc[p] + base + i, r);
+  }
+  grid_then_node_barrier(a.ticket, a.ticket_target, a.pads, a.rank, a.world, a.barrier_epoch,
+                         a.timeout_ns, a.status);
+}
+
 // -------------------------------------------------------------------- NVLS ----
 struct NvlsDev {
   const unsigned char* va_mc;
@@ -739,11 +865,15 @@ int launch_allreduce_two_shot(const TwoShotArgs& args, ElemType type, int ctas, 
   const int sms = device_sm_count(device);
   const int grid = grid_for(std::max<size_t>(d.slice_vec, 1), 512, ctas > 0 ? ctas : sms * 2);
   d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
-#define HPCP_TWO_SHOT(W, U)                                          \
-  do {                                                               \
-    dispatch_add_class(type, [&](auto tag) {                         \
-      two_shot_kernel<decltype(tag), W, U><<<grid, 512, 0, stream>>>(d); \
-    });                                                              \
+#define HPCP_TWO_SHOT(W, U)                                                \
+  do {                                                                     \
+    dispatch_add_class(type, [&](auto tag) {                               \
+      using C = decltype(tag);                                             \
+      if constexpr (kSum16InF32<C>)                                        \
+        two_shot_f32_kernel<C, W, U><<<grid, 512, 0, stream>>>(d);         \
+      else                                                                 \
+        two_shot_kernel<C, W, U><<<grid, 512, 0, stream>>>(d);             \
+    });                                                                    \
   } while (0)
   if (args.world <= 2)
     HPCP_TWO_SHOT(2, 4);

@@ -10,6 +10,8 @@
 // float or int (upstream: compile-time APP_DATA_TYPE -> here --type or the
 // binary-name suffix `allreduce.float` / `allreduce.int`, like the upstream
 // target names `<app>.<type>`).  Output kept: `Passed <rank>` per rank, exit 0.
+// bfloat16 / half (`allreduce.bfloat16`, `allreduce.half`, ↔ MPIX_C_BF16 / MPIX_C_FLOAT16): the rings round every add to
+// the 16-bit format, -a runs two-shot with fp32 accumulation; the constant-data check stays exact up to P = 16.
 // Additions: the elapsed time the reference computes but never prints
 // (allreduce-mpi-sycl.cpp:185-190) is printed as max over ranks, with bus GB/s.
 //
@@ -90,7 +92,8 @@ void print_help() {
                "                       cudaProfilerStart/Stop: use with `ncu --profile-from-start off`\n"
                " -n N        ranks (one host thread + one GPU each; default: all GPUs;\n"
                "             more ranks than GPUs are placed round-robin)\n"
-               " --type T   element type: float int uint double long ulong short ushort uchar (default float, or binary-name suffix)\n"
+               " --type T   element type: float int uint double long ulong short ushort uchar bfloat16 half\n"
+               "            (default float, or binary-name suffix)\n"
                " --algo ring|ring-unfused|ring-rsag   fused persistent ring kernel (default),\n"
                "                            separate put + accumulate kernels per step, or the\n"
                "                            bandwidth-optimal reduce-scatter + all-gather ring\n"
@@ -120,8 +123,30 @@ struct Shared {
   unsigned long long total_bad = 0;
 };
 
+// Host arithmetic of the 16-bit floating types: exact widening to fp32, and an add that is one fp32 add rounded once to
+// nearest even in the 16-bit format (fp32 has more than 2p+2 bits, so that equals the correctly rounded 16-bit add the
+// ring kernels do).  Every other type keeps its own arithmetic.
+template <typename T>
+double host_to_double(T x) {
+  return static_cast<double>(x);
+}
+double host_to_double(__nv_bfloat16 x) { return __bfloat162float(x); }
+double host_to_double(__half x) { return __half2float(x); }
+template <typename T>
+T host_add(T a, T b) {
+  return static_cast<T>(a + b);
+}
+__nv_bfloat16 host_add(__nv_bfloat16 a, __nv_bfloat16 b) {
+  return __float2bfloat16_rn(__bfloat162float(a) + __bfloat162float(b));
+}
+__half host_add(__half a, __half b) { return __float2half_rn(__half2float(a) + __half2float(b)); }
+template <typename T>
+constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
+
 double first_element_as_double(const void* p, ElemType t) {
   switch (t) {
+    case ElemType::kBFloat16: return host_to_double(*static_cast<const __nv_bfloat16*>(p));
+    case ElemType::kHalf: return host_to_double(*static_cast<const __half*>(p));
     case ElemType::kFloat: return *static_cast<const float*>(p);
     case ElemType::kInt: return *static_cast<const int*>(p);
     case ElemType::kUInt: return *static_cast<const unsigned int*>(p);
@@ -140,13 +165,15 @@ unsigned long long count_mismatch_typed(const void* p, size_t n, double expected
   const T* v = static_cast<const T*>(p);
   unsigned long long bad = 0;
   for (size_t i = 0; i < n; ++i) {
-    const double d = static_cast<double>(v[i]) - expected;
+    const double d = host_to_double(v[i]) - expected;
     bad += !(d < 1e-6 && d > -1e-6);
   }
   return bad;
 }
 unsigned long long count_mismatch_on_host(const void* p, size_t n, double expected, ElemType t) {
   switch (t) {
+    case ElemType::kBFloat16: return count_mismatch_typed<__nv_bfloat16>(p, n, expected);
+    case ElemType::kHalf: return count_mismatch_typed<__half>(p, n, expected);
     case ElemType::kFloat: return count_mismatch_typed<float>(p, n, expected);
     case ElemType::kInt: return count_mismatch_typed<int>(p, n, expected);
     case ElemType::kUInt: return count_mismatch_typed<unsigned int>(p, n, expected);
@@ -402,9 +429,18 @@ int run_on_host_typed(const Config& cfg) {
     vc[me].assign(n, static_cast<T>(0));
     ctx.barrier();
     const auto t0 = std::chrono::steady_clock::now();
-    if (cfg.use_collective) {
+    if (cfg.use_collective && kSum16InF32<T>) {
+      // two-shot's 16-bit rule: element i belongs to slice s = i*P/n, whose owner s sums VA[s], VA[s+1], ... (ranks
+      // mod P) in fp32 and rounds once
+      for (size_t i = 0; i < n; ++i) {
+        const int s = static_cast<int>(i * P / n);
+        float acc = static_cast<float>(host_to_double(va[s][i]));
+        for (int q = 1; q < P; ++q) acc += static_cast<float>(host_to_double(va[(s + q) % P][i]));
+        vc[me][i] = static_cast<T>(acc);
+      }
+    } else if (cfg.use_collective) {
       for (int r = 0; r < P; ++r)
-        for (size_t i = 0; i < n; ++i) vc[me][i] += va[r][i];
+        for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[r][i]);
     } else if (rsag) {
       vb[me].resize(seg_n * std::max(P - 1, 1));  // receive slots
       ctx.barrier();
@@ -414,7 +450,7 @@ int run_on_host_typed(const Config& cfg) {
         const T* src = (rsag_reads_vc(h, P) ? vc[me].data() : va[me].data()) + seg;
         const int rs = rsag_src_slot(h, kRsAgAllreduce, P);
         for (size_t i = 0; i < seg_n; ++i)
-          x[i] = rs >= 0 ? static_cast<T>(vb[me][rs * seg_n + i] + src[i]) : src[i];
+          x[i] = rs >= 0 ? host_add(vb[me][rs * seg_n + i], src[i]) : src[i];
         if (rsag_writes_own_vc(h, P)) std::memcpy(vc[me].data() + seg, x.data(), seg_n * sizeof(T));
         if (rsag_forwards(h, kRsAgAllreduce, P)) {
           const int fs = rsag_fwd_slot(h, P);
@@ -424,13 +460,13 @@ int run_on_host_typed(const Config& cfg) {
         ctx.barrier();  // the hop has landed everywhere
       }
     } else {
-      for (size_t i = 0; i < n; ++i) vc[me][i] += va[me][i];
+      for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[me][i]);
       for (int s = 1; s < P; ++s) {
         std::memcpy(vb[right].data(), va[me].data(), n * sizeof(T));  // "send right"
         ctx.barrier();                                                 // everybody received
         va[me].swap(vb[me]);
         ctx.barrier();                                                 // nobody still reads the old VA
-        for (size_t i = 0; i < n; ++i) vc[me][i] += va[me][i];
+        for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[me][i]);
       }
     }
     const double ms =
@@ -438,7 +474,7 @@ int run_on_host_typed(const Config& cfg) {
     const double t = ctx.max(ms);
     const T want = static_cast<T>(P * (P - 1) / 2);
     unsigned long long bad = 0;
-    for (size_t i = 0; i < n; ++i) bad += std::abs(static_cast<double>(vc[me][i]) - static_cast<double>(want)) >= 1e-6;
+    for (size_t i = 0; i < n; ++i) bad += std::abs(host_to_double(vc[me][i]) - host_to_double(want)) >= 1e-6;
     const double all_bad = ctx.sum(static_cast<double>(bad));
     if (bad == 0)
       std::cout << "Passed " << me << std::endl;
@@ -481,6 +517,8 @@ int run_on_host(const Config& cfg) {
     case ElemType::kShort: return run_on_host_typed<short>(cfg);
     case ElemType::kUShort: return run_on_host_typed<unsigned short>(cfg);
     case ElemType::kUChar: return run_on_host_typed<unsigned char>(cfg);
+    case ElemType::kBFloat16: return run_on_host_typed<__nv_bfloat16>(cfg);
+    case ElemType::kHalf: return run_on_host_typed<__half>(cfg);
   }
   return 1;
 }

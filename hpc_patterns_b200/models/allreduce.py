@@ -34,9 +34,12 @@ ALGOS = ("ring", "ring-unfused", "twoshot", "nvls", "nccl", "ring-nccl", "ring-r
 VIRTUAL_ALGOS = ("ring", "ring-unfused", "twoshot", "ring-rsag")   # the ones whose peers are plain pointers (no NCCL, no multicast)
 # element types of the reference's datatype trait (mpi_datatype.hpp:28-51) -> the torch dtype whose add is bit-identical
 # (unsigned integers share the two's-complement add of the signed type of the same width; NCCL rows only)
+# bfloat16 / half (MPICH's MPIX_C_BF16 / MPIX_C_FLOAT16): the rings round every add to the 16-bit format, two-shot sums in
+# fp32 and rounds once (docs/allreduce.md)
 _TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32, "double": torch.float64,
                 "long": torch.int64, "ulong": torch.int64, "short": torch.int16, "ushort": torch.int16,
-                "uchar": torch.uint8}
+                "uchar": torch.uint8, "bfloat16": torch.bfloat16, "half": torch.float16}
+FLOAT16_TYPES = ("bfloat16", "half")
 
 
 def expected_value(world: int) -> float:
@@ -401,8 +404,12 @@ def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int):
     Decided BEFORE anything is allocated and agreed across ranks (min over ranks of the local probe), so ranks can
     neither diverge on the algorithm nor leak a half-built instance:
       * int:   two-shot — ``multimem.ld_reduce`` has no vector form for .s32 (one 4-byte request per thread), peer loads are 128-bit for every type;
+      * bfloat16 / half: two-shot — its fp32 accumulation rounds once, where the rings round P-1 times (the NVLS
+        kernel reduces fp32 and 32-bit integers only);
       * float: NVLS (in-switch reduction) when every rank reports multicast support, else two-shot."""
     C = native()
+    if dtype in FLOAT16_TYPES:
+        return "twoshot", "16-bit floats: two-shot sums in fp32 and rounds once"
     if dtype != "float":
         return "twoshot", "integer reductions use vector peer loads; multimem.ld_reduce.s32 is scalar"
     ok = comm.world >= 2 and bool(C.multicast_supported(device))

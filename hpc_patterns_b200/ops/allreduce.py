@@ -14,14 +14,14 @@ import torch
 from .. import native
 from ._util import current_stream, ptr
 
-_DTYPE_NAME = {torch.float32: "float", torch.int32: "int"}
+_DTYPE_NAME = {torch.float32: "float", torch.int32: "int", torch.bfloat16: "bfloat16", torch.float16: "half"}
 
 
 def dtype_name(t: torch.Tensor) -> str:
     try:
         return _DTYPE_NAME[t.dtype]
     except KeyError:
-        raise TypeError(f"allreduce kernels support float32 and int32, not {t.dtype}") from None
+        raise TypeError(f"allreduce kernels support float32, int32, bfloat16 and float16, not {t.dtype}") from None
 
 
 def accumulate(va: torch.Tensor, vc: torch.Tensor, stream: Optional[int] = None) -> torch.Tensor:
