@@ -24,6 +24,7 @@
 #include "concurency/driver.hpp"
 #include "kernels/api.h"
 #include "kernels/ring_order.h"
+#include "kernels/halo_columns.h"
 #include "kernels/tile_order.h"
 #include "p2p/topology_core.hpp"
 
@@ -75,8 +76,7 @@ HaloTuning halo_tuning_from(const py::dict& d) {
   HaloTuning t;
   if (d.contains("ctas")) t.ctas = d["ctas"].cast<int>();
   if (d.contains("tile_kb")) t.tile_kb = d["tile_kb"].cast<int>();
-  if (d.contains("stages")) t.stages = d["stages"].cast<int>();
-  if (d.contains("out_stages")) t.out_stages = d["out_stages"].cast<int>();
+  // "stages" / "out_stages" sized the shared-memory rings of the old TMA pipeline: accepted and ignored.
   return t;
 }
 
@@ -501,6 +501,26 @@ PYBIND11_MODULE(_C, m) {
       py::arg("ticket_base") = 0, py::arg("rank") = 0, py::arg("m"), py::arg("n"), py::arg("k"), py::arg("ctas") = 0,
       py::arg("device") = 0, py::arg("stream") = 0, py::arg("cluster") = 0,
       "wgmma GEMM whose epilogue stores row block q of the result into rank q's receive buffer (GEMM -> all-to-all).");
+  // K-halo column ownership (kernels/halo_columns.h), exposed for the CPU tests: the float4 columns thread `thread` of
+  // CTA `cta` visits, in the kernel's loop order, and the owner of one column ((-1, -1) outside the launch).
+  m.def("halo_thread_columns", [](uint64_t row_vec, uint32_t tile_vec, uint64_t tile_begin, uint64_t tile_end,
+                                  uint32_t ctas, uint32_t threads, uint32_t cta, uint32_t thread) {
+    const HaloColumns g{row_vec, tile_vec, tile_begin, tile_end, ctas, threads};
+    std::vector<uint64_t> out;
+    for (uint64_t jj = 0; jj < halo_cta_tiles(g, cta); ++jj) {
+      const uint64_t first = halo_tile_first(g, cta, jj);
+      for (uint64_t v = first + thread; v < halo_tile_end(g, first); v += threads) out.push_back(v);
+    }
+    return out;
+  });
+  m.def("halo_column_owner", [](uint64_t row_vec, uint32_t tile_vec, uint64_t tile_begin, uint64_t tile_end,
+                                uint32_t ctas, uint32_t threads, uint64_t v) {
+    const HaloColumns g{row_vec, tile_vec, tile_begin, tile_end, ctas, threads};
+    uint32_t cta = 0, thread = 0;
+    if (!halo_column_owner(g, v, &cta, &thread)) return std::make_pair(-1, -1);
+    return std::make_pair(static_cast<int>(cta), static_cast<int>(thread));
+  });
+  m.attr("HALO_THREADS") = kHaloThreads;
   // Tile / gather orderings of the tensor-core kernels (kernels/tile_order.h), exposed for the CPU tests.
   m.def("gemm_tile_coords", [](int tile, int tiles_m, int tiles_n) {
     int mb = 0, nb = 0;

@@ -116,10 +116,8 @@ constexpr int kHaloMaxCtas = 1024;   // flag words per side
 constexpr int kHaloFlagSets = 16;    // independent flag sets (chunked launches of one step use one set per chunk)
 constexpr size_t kHaloFlagBytes = static_cast<size_t>(kHaloFlagSets) * 2 * kHaloMaxCtas * kHaloFlagWords * 4;
 struct HaloTuning {
-  int ctas = 0;     // 0 -> every resident CTA slot (SMs x occupancy); always clamped to it
-  int tile_kb = 0;     // bytes of a row per shared-memory stage in KiB (<= 32); 0 -> 16
-  int stages = 0;      // shared-memory tile slots, input ring + output ring (>= 3); 0 -> 12
-  int out_stages = 0;  // of those, the output staging ring (>= 2); 0 -> max(2, stages / 4)
+  int ctas = 0;     // 0 -> every resident CTA slot (SMs x 2 CTAs of 512 threads); always clamped to it
+  int tile_kb = 0;  // column tile in KiB (1 .. 1024), the unit of CTA ownership and of tile_begin / tile_end; 0 -> 16
 };
 struct HaloStencilArgs {
   float* u[2] = {nullptr, nullptr};                 // local field, ping-pong: step g reads u[g&1], writes u[(g+1)&1]

@@ -14,85 +14,68 @@
 // Row -1 is the left neighbour's last row and row `rows` the right neighbour's first row of the
 // SAME step's input: the halo.  Two forms of the exchange, both inside the stencil kernel:
 //   pull  the kernel reads the neighbours' boundary rows straight out of their field over NVLink
-//         (cp.async.bulk global -> shared on a peer-mapped address).  No halo buffer exists, the
-//         halo costs no HBM write and no HBM read on the consumer.
+//         (128-bit loads from a peer-mapped address).  No halo buffer exists, the halo costs no HBM
+//         write and no HBM read on the consumer.
 //   push  the kernel stores its freshly computed boundary rows into halo buffers on the neighbours
-//         (cp.async.bulk shared -> peer global) next to the local store, from the same smem tile.
+//         (128-bit stores to a peer-mapped address) next to the local store, from the same registers.
 // `none` reads local halo buffers and talks to nobody: the compute kernel of the stock arm
 // (kernel -> cudaMemcpyAsync / NCCL send+recv -> host wait), which models/halo.py times next to it.
 //
-// Work split.  A CTA owns column tiles j = blockIdx.x + k * gridDim.x of EVERY row and marches down the rows of a column
-// tile.  Each input tile is fetched once into a shared-memory input ring and read once from there, by the math warps,
-// into a register row window; the result of row r is written to a separate output staging ring and leaves through the
-// TMA unit.  Because a column tile is owned by the same CTA index on every rank and in every step, the only cross-CTA
-// dependency of step g+1 is "CTA c of my two neighbours finished step g".  That is one monotonic word per
-// (neighbour, CTA):
+// Work split (halo_columns.h).  A CTA owns column tiles j = blockIdx.x + k * gridDim.x of EVERY row, and thread t of
+// the CTA the float4 columns t, t + kHaloThreads, ... of each of its tiles.  A thread loads all R + 2 input rows of
+// one of its columns into registers, computes the R outputs and stores them: a plain 128-bit ld/st stream, the engine
+// of the card's fastest copy, with no shared memory and no intra-CTA hand-off.  Because the map does not depend on the
+// rank or the step, a thread only reads what it wrote itself in the previous step (its own rows, and at N = 1 both
+// halos) or what a neighbour's CTA c published, so the only cross-CTA dependency of step g+1 is "CTA c of my two
+// neighbours finished step g".  That is one monotonic word per (neighbour, CTA):
 //   * RAW  my step g reads the neighbour's u_g boundary tile / my halo[g&1]: written in its step g-1;
 //   * WAR  my step g overwrites u[(g+1)&1] / the neighbour's halo[(g+1)&1]: last read in its step g-1.
-// Both are "neighbour's CTA c completed step g-1", i.e. flag >= g.  So K steps run in ONE launch
-// with no grid barrier, no host sync and no per-step launch (`steps` > 1), or one launch per step
-// (`steps` == 1) with the same words carrying the dependency across launches.
+// Both are "neighbour's CTA c completed step g-1", i.e. flag >= g.  Thread 0 waits for both words, then
+// __syncthreads(); after the CTA's last store of the step, __syncthreads(), fence.acq_rel.sys and st.release.sys of
+// g+1 to both neighbours (signal.cuh).  In pull and push mode the CTAs also pace each other through a rank-local
+// count of finished tiles (see the kernel), so that they stay within one wave of tiles.  So K steps run in ONE launch with no grid barrier, no host sync and no
+// per-step launch (`steps` > 1), or one launch per step (`steps` == 1) with the same words carrying the dependency
+// across launches.  Loads are never `.nc`: the kernel reads data that it or a peer wrote earlier in the same launch.
 //
-// Load order of a column tile: boundary rows first — own row R-1, up halo, own row 0, down halo, then rows 1 .. R-2
-// (R = 2: row 1, up, row 0, down; R = 1: row 0, up, down).  Every boundary row is read twice per step by somebody: by
-// its owner as a centre row and by a neighbour as its halo (at N = 1 the neighbour is the rank itself, so up halo = own
-// row R-1 and down halo = own row 0).  With this order the two reads of a row sit next to each other, and since ranks
-// run CTA by CTA in near lock-step the second one is served from L2: a step moves 2 * rows rows through HBM, not 2 *
-// rows + 2.  L2 policy by role: interior-row loads and the local stores stream with evict_first, boundary-row loads keep
-// the default policy so that the second read finds them.
-//
-// Warp roles (one CTA per SM):
-//   warp 0 / lane 0   producer: per step, waits until this CTA's previous-step stores are performed (`stored`, a
-//                     CTA-local mbarrier: step g+1 reads what step g wrote here, which the neighbour words do not
-//                     cover at N > 1) and for the two neighbour words, then streams tiles global -> smem into the input
-//                     ring (full / empty mbarriers).  It only ever blocks on `stored`, the words and `empty`.
-//   warp 1 / lane 0   store thread: waits for a finished output slot (`ofull`), stores it smem -> global (+ the peer
-//                     puts in push mode), keeps up to two stores reading shared memory and frees a slot once
-//                     bulk_wait_read has seen its store read (`oempty`); at the end of a step bulk_wait<0>,
-//                     fence.proxy.async, releases both step words and arrives on `stored`.
-//   warps 2..9        math: each thread owns the float4 columns v = t + k * 256 of the tile.  Per column it reads each
-//                     input tile once into registers (row R-1 and the down halo are kept aside), frees the slot, and
-//                     writes stencil1(up, ce, dn) of row r into the output ring, rows 0 .. R-1 in order.  An interior
-//                     lower row is read and consumed in the same pass, so only four rows are live per thread.
-// Ordering: every step-g load has been read by the math warps before the last step-g result exists, so before the last
-// step-g store is issued; step-g+1 loads are issued only after `stored` (own step-g stores performed) and the words.
+// Load order of a column: boundary rows first — own row R-1, up halo, own row 0, down halo, then rows 1 .. R-2
+// (R = 1: row 0, up, down).  Every boundary row is read twice per step by somebody: by its owner as a centre row and
+// by a neighbour as its halo (at N = 1 the neighbour is the rank itself, so up halo = own row R-1 and down halo = own
+// row 0).  With this order the two reads of a row sit next to each other, and since ranks run CTA by CTA in near
+// lock-step the second one is served from L2: a step moves 2 * rows rows through HBM, not 2 * rows + 2.  L2 policy by
+// role: interior-row loads and the local stores stream with evict_first, boundary-row loads keep the default policy so
+// that the second read finds them; nothing is allocated in L1.  The interior rows are loaded kHaloChunk at a time
+// ahead of their use, so at R = 8 all ten loads of a column are in flight at once.
 #include "api.h"
 
 #include <algorithm>
 #include <mutex>
-#include <vector>
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
+#include "halo_columns.h"
 
 namespace hpcp {
 
 namespace {
 
-constexpr int kHaloMathWarps = 8;
-constexpr int kHaloMathThreads = 32 * kHaloMathWarps;
-constexpr int kHaloThreads = 32 * (2 + kHaloMathWarps);
-constexpr int kHaloVec = 8;  // float4 per math thread and tile row: the register window covers tiles up to 32 KiB
-constexpr uint32_t kHaloMaxTileBytes = 16u * kHaloVec * kHaloMathThreads;
+constexpr int kHaloCtasPerSm = 2;  // 1024 threads per SM: <= 64 registers per thread
+constexpr int kHaloChunk = 6;      // interior rows loaded ahead of their use
 constexpr int kHaloDefaultTileKb = 16;
-constexpr int kHaloDefaultStages = 12;  // 9 input + 3 output slots of 16 KiB
 
 struct HaloParams {
-  unsigned char* u[2];
-  const unsigned char* up_src[2];   // row -1 of step parity p: pull = left neighbour's last row, else halo_lo[p]
-  const unsigned char* dn_src[2];   // row `rows`:              pull = right neighbour's row 0,   else halo_hi[p]
-  unsigned char* put_first[2];      // push: where my new row 0 goes on the left neighbour (its halo_hi[p])
-  unsigned char* put_last[2];       // push: where my new last row goes on the right neighbour (its halo_lo[p])
+  float4* u[2];
+  const float4* up_src[2];  // row -1 of step parity p: pull = left neighbour's last row, else halo_lo[p]
+  const float4* dn_src[2];  // row `rows`:              pull = right neighbour's row 0,   else halo_hi[p]
+  float4* put_first[2];     // push: where my new row 0 goes on the left neighbour (its halo_hi[p])
+  float4* put_last[2];      // push: where my new last row goes on the right neighbour (its halo_lo[p])
   // Flag arrays, one 32-byte sector per CTA (index blockIdx.x * kHaloFlagWords):
-  const uint32_t* wait_lo;          // local, written by the left neighbour's CTAs
-  const uint32_t* wait_hi;          // local, written by the right neighbour's CTAs
-  uint32_t* signal_lo;              // on the left neighbour (its wait_hi array)
-  uint32_t* signal_hi;              // on the right neighbour (its wait_lo array)
+  const uint32_t* wait_lo;  // local, written by the left neighbour's CTAs
+  const uint32_t* wait_hi;  // local, written by the right neighbour's CTAs
+  uint32_t* signal_lo;      // on the left neighbour (its wait_hi array)
+  uint32_t* signal_hi;      // on the right neighbour (its wait_lo array)
+  uint32_t* pace;           // local: column tiles of this flag set finished on this rank, counting up forever
   int rows;
-  size_t row_bytes;
-  size_t tile_begin, tile_end;      // column tiles [begin, end) of a row handled by this launch
-  uint32_t tile_bytes;
-  int in_stages, out_stages;        // input ring and output staging ring, in tiles
+  HaloColumns cols;
   float alpha, s;
   uint32_t step_base;
   int steps;
@@ -111,262 +94,116 @@ __device__ __forceinline__ float4 stencil4(const float4& up, const float4& ce, c
                      stencil1(up.z, ce.z, dn.z, alpha, s), stencil1(up.w, ce.w, dn.w, alpha, s));
 }
 
-// Row of the q-th load of a column tile (q = 0 .. R+1), boundary rows first; -1 is the up halo, R the down halo.
-__device__ __forceinline__ int halo_load_row(int q, int R) {
-  if (q == 0) return R - 1;
-  if (q == 1) return -1;
-  if (R == 1) return 1;  // q == 2: the down halo
-  if (q == 2) return 0;
-  if (q == 3) return R;
-  return q - 3;
+// 128-bit accesses of the stencil, all L1::no_allocate and never `.nc`.
+__device__ __forceinline__ float4 ld_keep(const float4* p) {  // boundary rows: read again right after, from L2
+  float4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(p)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ float4 ld_stream(const float4* p, uint64_t policy) {  // interior rows: read once
+  float4 v;
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(p), "l"(policy)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_stream(float4* p, const float4& v, uint64_t policy) {  // local field
+  asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(p), "f"(v.x),
+               "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy)
+               : "memory");
+}
+__device__ __forceinline__ void st_put(float4* p, const float4& v) {  // push: the neighbour's halo buffer
+  asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
+               "f"(v.w)
+               : "memory");
 }
 
-// Cursor into a ring of S mbarrier-guarded slots: slot index + the phase parity of its current use.
-struct Ring {
-  int slot;
-  uint32_t phase;
-  __device__ __forceinline__ void advance(int S) {
-    if (++slot == S) {
-      slot = 0;
-      phase ^= 1u;
+// One step of float4 column v: loads in boundary-first order, outputs rows 0 .. R-1 in order.
+template <int kMode>
+__device__ __forceinline__ void halo_column(const HaloParams& p, int in, uint64_t v) {
+  const uint64_t evict_first = ptx::l2_policy_evict_first();
+  const int R = p.rows;
+  const uint64_t rv = p.cols.row_vec;
+  const float alpha = p.alpha, s = p.s;
+  const float4* uin = p.u[in] + v;
+  float4* uout = p.u[in ^ 1] + v;
+  auto store = [&](int r, const float4& x) {
+    st_stream(uout + static_cast<uint64_t>(r) * rv, x, evict_first);
+    if (kMode == 2) {
+      if (r == 0) st_put(p.put_first[in ^ 1] + v, x);
+      if (r == R - 1) st_put(p.put_last[in ^ 1] + v, x);
     }
+  };
+  const float4 last = ld_keep(uin + static_cast<uint64_t>(R - 1) * rv);
+  float4 prev = ld_keep(p.up_src[in] + v);
+  if (R == 1) {
+    store(0, stencil4(prev, last, ld_keep(p.dn_src[in] + v), alpha, s));
+    return;
   }
-};
-
-// mbarrier wait that gives up when the producer reported a dead peer.
-__device__ __forceinline__ bool mbar_wait_or_abort(uint64_t* bar, uint32_t parity, const volatile int* abort_w) {
-  while (!ptx::mbar_try_wait(bar, parity)) {
-    if (*abort_w != 0) return false;
-  }
-  return true;
-}
-
-// One tile row of a math thread's columns, kept in registers.
-struct RowRegs {
-  float4 v[kHaloVec];
-};
-
-// The math warps' side of both rings.
-struct MathPipe {
-  unsigned char* in_base;
-  unsigned char* out_base;
-  uint64_t* full;
-  uint64_t* empty;
-  uint64_t* ofull;
-  uint64_t* oempty;
-  const volatile int* abort_w;
-  uint32_t T;
-  int S_in, S_out;
-  int mt;
-  Ring in, out;
-
-  // Wait for the next input tile, copy this thread's part into `dst`, free the slot.
-  __device__ __forceinline__ bool read(RowRegs& dst, uint32_t nv) {
-    if (!mbar_wait_or_abort(&full[in.slot], in.phase, abort_w)) return false;
-    const float4* t = reinterpret_cast<const float4*>(in_base + static_cast<size_t>(in.slot) * T);
+  float4 cur = ld_keep(uin);
+  const float4 dn = ld_keep(p.dn_src[in] + v);
+  for (int base = 1; base < R - 1; base += kHaloChunk) {  // interior rows: row base-1 .. base+kHaloChunk-2 out
+    float4 w[kHaloChunk];
 #pragma unroll
-    for (int k = 0; k < kHaloVec; ++k) {
-      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
-      if (v < nv) dst.v[k] = t[v];
-    }
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&empty[in.slot]);
-    in.advance(S_in);
-    return true;
-  }
-  // Wait for a free output slot.
-  __device__ __forceinline__ bool acquire_out() {
-    return mbar_wait_or_abort(&oempty[out.slot], out.phase ^ 1u, abort_w);
-  }
-  // The math warps' writes to the output slot -> visible to the TMA store; hand the slot to the store thread.
-  __device__ __forceinline__ void publish_out() {
-    ptx::fence_proxy_async_smem();
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&ofull[out.slot]);
-    out.advance(S_out);
-  }
-  __device__ __forceinline__ float4* out_tile() const {
-    return reinterpret_cast<float4*>(out_base + static_cast<size_t>(out.slot) * T);
-  }
-  // Output row from three rows held in registers.
-  __device__ __forceinline__ bool write(const RowRegs& up, const RowRegs& ce, const RowRegs& dn, uint32_t nv,
-                                        float alpha, float s) {
-    if (!acquire_out()) return false;
-    float4* t = out_tile();
+    for (int i = 0; i < kHaloChunk; ++i)
+      if (base + i < R - 1) w[i] = ld_stream(uin + static_cast<uint64_t>(base + i) * rv, evict_first);
 #pragma unroll
-    for (int k = 0; k < kHaloVec; ++k) {
-      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
-      if (v < nv) t[v] = stencil4(up.v[k], ce.v[k], dn.v[k], alpha, s);
-    }
-    publish_out();
-    return true;
-  }
-  // Output row whose lower neighbour is the next input tile, read straight into the window: up <- ce <- next tile.
-  // Only four rows are live in the math warps (up, ce and the two saved boundary rows).
-  __device__ __forceinline__ bool read_write(RowRegs& up, RowRegs& ce, uint32_t nv, float alpha, float s) {
-    if (!mbar_wait_or_abort(&full[in.slot], in.phase, abort_w) || !acquire_out()) return false;
-    const float4* src = reinterpret_cast<const float4*>(in_base + static_cast<size_t>(in.slot) * T);
-    float4* t = out_tile();
-#pragma unroll
-    for (int k = 0; k < kHaloVec; ++k) {
-      const uint32_t v = static_cast<uint32_t>(mt + k * kHaloMathThreads);
-      if (v < nv) {
-        const float4 dn = src[v];
-        t[v] = stencil4(up.v[k], ce.v[k], dn, alpha, s);
-        up.v[k] = ce.v[k];
-        ce.v[k] = dn;
+    for (int i = 0; i < kHaloChunk; ++i) {
+      if (base + i < R - 1) {
+        store(base + i - 1, stencil4(prev, cur, w[i], alpha, s));
+        prev = cur;
+        cur = w[i];
       }
     }
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) ptx::mbar_arrive(&empty[in.slot]);
-    in.advance(S_in);
-    publish_out();
-    return true;
   }
-};
+  store(R - 2, stencil4(prev, cur, last, alpha, s));
+  store(R - 1, stencil4(cur, last, dn, alpha, s));
+}
 
 // kMode: 0 none, 1 pull, 2 push.
 template <int kMode>
-__global__ void __launch_bounds__(kHaloThreads, 1) halo_stencil_kernel(const HaloParams p) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  const uint32_t T = p.tile_bytes;
-  const int S_in = p.in_stages, S_out = p.out_stages;
-  unsigned char* out_base = smem + static_cast<size_t>(S_in) * T;
-  uint64_t* full = reinterpret_cast<uint64_t*>(out_base + static_cast<size_t>(S_out) * T);
-  uint64_t* empty = full + S_in;
-  uint64_t* ofull = empty + S_in;
-  uint64_t* oempty = ofull + S_out;
-  uint64_t* stored = oempty + S_out;
-  volatile int* abort_w = reinterpret_cast<volatile int*>(stored + 1);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < S_in; ++i) {
-      ptx::mbar_init(&full[i], 1);
-      ptx::mbar_init(&empty[i], kHaloMathWarps);
-    }
-    for (int i = 0; i < S_out; ++i) {
-      ptx::mbar_init(&ofull[i], kHaloMathWarps);
-      ptx::mbar_init(&oempty[i], 1);
-    }
-    ptx::mbar_init(stored, 1);
-    *abort_w = 0;
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
-
-  const int R = p.rows;
-  const size_t n_tiles = p.tile_end - p.tile_begin;
-  const size_t ncols = n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  if (ncols == 0) return;  // same geometry on every rank: nobody waits for this CTA index
-  auto col_off = [&](size_t jj) { return (p.tile_begin + blockIdx.x + jj * gridDim.x) * static_cast<size_t>(T); };
-  auto col_len = [&](size_t off) {
-    return static_cast<uint32_t>(p.row_bytes - off < T ? p.row_bytes - off : T);
-  };
-
-  const int warp = threadIdx.x >> 5;
-  if (warp == 0) {
-    if (threadIdx.x != 0) return;
-    // ------------------------------------------------------------------ producer ----
-    const uint64_t evict_first = ptx::l2_policy_evict_first();
-    Ring ld{0, 0};
-    for (int si = 0; si < p.steps; ++si) {
-      const uint32_t g = p.step_base + static_cast<uint32_t>(si);
-      const int in = static_cast<int>(g & 1u);
-      if (si > 0) ptx::mbar_wait(stored, static_cast<uint32_t>(si - 1) & 1u);  // own step g-1 stores performed
+__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_kernel(const HaloParams p) {
+  __shared__ int abort_w;
+  const uint32_t ntiles = static_cast<uint32_t>(halo_cta_tiles(p.cols, blockIdx.x));  // < 2^32 float4 per row
+  if (ntiles == 0) return;  // same geometry on every rank: nobody waits for this CTA index
+  for (int si = 0; si < p.steps; ++si) {
+    const uint32_t g = p.step_base + static_cast<uint32_t>(si);
+    const int in = static_cast<int>(g & 1u);
+    for (uint32_t jj = 0; jj < ntiles; ++jj) {
       if (kMode != 0) {
-        const bool ok = wait_epoch(p.wait_lo + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status) &&
-                        wait_epoch(p.wait_hi + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status);
-        if (!ok) {
-          *abort_w = 1;
-          return;
+        // Tile jj of step g is ticket t = g * n + jj * G + c of this rank and flag set (dense over the n tiles of a
+        // step, in row order within a step).  Besides the neighbour words at the start of a step, the CTA waits until
+        // at least t - G tickets of this rank are finished: CTAs that run ahead are held to one wave of tiles, so the
+        // CTAs stream through a compact stretch of the rows together, as one-shot grids do.  On an H100 that is
+        // worth ~2 % of HBM throughput over free-running CTAs.  The wait only ever needs earlier tickets (or the
+        // neighbours' earlier steps), so it cannot deadlock; it is not needed for correctness.
+        if (threadIdx.x == 0) {
+          const uint32_t n = static_cast<uint32_t>(p.cols.tile_end - p.cols.tile_begin);
+          const uint32_t ticket = g * n + jj * gridDim.x + blockIdx.x;
+          abort_w = !((jj != 0 || (wait_epoch(p.wait_lo + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status) &&
+                                   wait_epoch(p.wait_hi + blockIdx.x * kHaloFlagWords, g, p.timeout_ns, p.status))) &&
+                      wait_epoch(p.pace, ticket - gridDim.x, p.timeout_ns, p.status));
         }
-        asm volatile("fence.proxy.async;" ::: "memory");  // acquired peer data -> visible to the bulk loads
+        __syncthreads();
+        if (abort_w) return;
       }
-      const unsigned char* uin = p.u[in];
-      for (size_t jj = 0; jj < ncols; ++jj) {
-        const size_t off = col_off(jj);
-        const uint32_t len = col_len(off);
-        for (int q = 0; q < R + 2; ++q) {
-          const int row = halo_load_row(q, R);
-          const unsigned char* src = row < 0    ? p.up_src[in] + off
-                                     : row == R ? p.dn_src[in] + off
-                                                : uin + static_cast<size_t>(row) * p.row_bytes + off;
-          ptx::mbar_wait(&empty[ld.slot], ld.phase ^ 1u);
-          unsigned char* dst = smem + static_cast<size_t>(ld.slot) * T;
-          ptx::mbar_arrive_expect_tx(&full[ld.slot], len);
-          if (row > 0 && row < R - 1)  // interior: read once per step, never again through L2
-            ptx::bulk_g2s_hint(dst, src, len, &full[ld.slot], evict_first);
-          else  // boundary rows: read twice per step, back to back
-            ptx::bulk_g2s(dst, src, len, &full[ld.slot]);
-          ld.advance(S_in);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (threadIdx.x != 32) return;
-    // ------------------------------------------------------------------ store thread ----
-    const uint64_t evict_first = ptx::l2_policy_evict_first();
-    // Store groups left reading shared memory after each commit; the math warps keep at least one free slot.
-    const int lag = S_out >= 3 ? 2 : 1;
-    Ring st{0, 0};
-    for (int si = 0; si < p.steps; ++si) {
-      const uint32_t g = p.step_base + static_cast<uint32_t>(si);
-      const int out = static_cast<int>(g & 1u) ^ 1;
-      unsigned char* uout = p.u[out];
-      uint64_t n = 0;  // stores issued in this step; slots are used in ring order
-      for (size_t jj = 0; jj < ncols; ++jj) {
-        const size_t off = col_off(jj);
-        const uint32_t len = col_len(off);
-        for (int r = 0; r < R; ++r) {
-          if (!mbar_wait_or_abort(&ofull[st.slot], st.phase, abort_w)) return;
-          const unsigned char* sa = out_base + static_cast<size_t>(st.slot) * T;
-          ptx::bulk_s2g_hint(uout + static_cast<size_t>(r) * p.row_bytes + off, sa, len, evict_first);
-          if (kMode == 2) {
-            if (r == 0) ptx::bulk_s2g(p.put_first[out] + off, sa, len);
-            if (r == R - 1) ptx::bulk_s2g(p.put_last[out] + off, sa, len);
+      const uint64_t first = halo_tile_first(p.cols, blockIdx.x, jj);
+      const uint64_t end = halo_tile_end(p.cols, first);
+      for (uint64_t v = first + threadIdx.x; v < end; v += kHaloThreads) halo_column<kMode>(p, in, v);
+      if (kMode != 0) {
+        __syncthreads();  // every store of the tile (local field and, in push mode, the peers' halos)
+        if (threadIdx.x == 0) {
+          ptx::red_release_gpu_add(p.pace, 1u);
+          if (jj + 1 == ntiles) {  // the step's last tile: publish the step to both neighbours
+            ptx::fence_acq_rel_sys();
+            ptx::st_release_sys(p.signal_hi + blockIdx.x * kHaloFlagWords, g + 1u);
+            ptx::st_release_sys(p.signal_lo + blockIdx.x * kHaloFlagWords, g + 1u);
           }
-          ptx::bulk_commit();
-          // every store group but the `lag` newest has left shared memory: free the slot of the one just before them
-          if (lag == 2)
-            ptx::bulk_wait_read<2>();
-          else
-            ptx::bulk_wait_read<1>();
-          if (n >= static_cast<uint64_t>(lag)) ptx::mbar_arrive(&oempty[(st.slot + S_out - lag) % S_out]);
-          ++n;
-          st.advance(S_out);
         }
-      }
-      ptx::bulk_wait<0>();  // this step's stores are performed (local field and, in push mode, the peers' halos)
-      for (int k = n < static_cast<uint64_t>(lag) ? static_cast<int>(n) : lag; k >= 1; --k)
-        ptx::mbar_arrive(&oempty[(st.slot + S_out - k) % S_out]);
-      asm volatile("fence.proxy.async;" ::: "memory");
-      if (kMode != 0) {
-        ptx::fence_acq_rel_sys();
-        ptx::st_release_sys(p.signal_hi + blockIdx.x * kHaloFlagWords, g + 1u);
-        ptx::st_release_sys(p.signal_lo + blockIdx.x * kHaloFlagWords, g + 1u);
-      }
-      ptx::mbar_arrive(stored);  // the producer may load what this step wrote
-    }
-  } else {
-    // ------------------------------------------------------------------ math warps ----
-    const float alpha = p.alpha, s = p.s;
-    MathPipe mp{smem, out_base, full, empty, ofull, oempty, abort_w, T, S_in, S_out,
-                static_cast<int>(threadIdx.x) - 64, {0, 0}, {0, 0}};
-    RowRegs last, up, ce, dnh;
-    for (int si = 0; si < p.steps; ++si) {
-      for (size_t jj = 0; jj < ncols; ++jj) {
-        const uint32_t nv = col_len(col_off(jj)) / 16;
-        // loads in halo_load_row order: row R-1 (row 0 when R == 1), up halo, [row 0,] down halo, rows 1 .. R-2
-        if (!mp.read(last, nv) || !mp.read(up, nv)) return;
-        if (R == 1) {
-          if (!mp.read(dnh, nv) || !mp.write(up, last, dnh, nv, alpha, s)) return;
-          continue;
-        }
-        if (!mp.read(ce, nv) || !mp.read(dnh, nv)) return;
-        for (int r = 0; r + 2 < R; ++r)  // rows 0 .. R-3: the lower neighbour is the next interior row
-          if (!mp.read_write(up, ce, nv, alpha, s)) return;
-        if (!mp.write(up, ce, last, nv, alpha, s)) return;   // row R-2
-        if (!mp.write(ce, last, dnh, nv, alpha, s)) return;  // row R-1
       }
     }
   }
@@ -451,61 +288,41 @@ __global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const f
 
 struct HaloGeometry {
   uint32_t tile_bytes;
-  int in_stages, out_stages;
-  size_t smem;
   int ctas;
 };
 
 template <int kMode>
-int occupancy_of(size_t smem) {
-  // One attribute + occupancy query per (mode, smem, device), not per launch (per-step launches come here K times).
-  // The dynamic shared-memory limit of the function is only ever RAISED: instances with different stage counts coexist.
-  struct Entry {
-    size_t smem;
-    int device, per_sm;
-  };
+int occupancy_of() {
+  // One occupancy query per (mode, device), not per launch (per-step launches come here K times).
   static std::mutex mu;
-  static std::vector<Entry> cache;
-  static size_t limit_set[64] = {0};
+  static int per_sm[64] = {0};
   int device = 0;
   HPCP_CUDA(cudaGetDevice(&device));
   std::lock_guard<std::mutex> lk(mu);
-  if (device >= 0 && device < 64 && smem > limit_set[device]) {
-    HPCP_ENABLE_SMEM(halo_stencil_kernel<kMode>, smem);
-    limit_set[device] = smem;
+  if (device < 0 || device >= 64 || per_sm[device] == 0) {
+    int n = 0;
+    HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, halo_stencil_kernel<kMode>, kHaloThreads, 0));
+    if (device < 0 || device >= 64) return n;
+    per_sm[device] = n;
   }
-  for (const Entry& e : cache)
-    if (e.smem == smem && e.device == device) return e.per_sm;
-  int per_sm = 0;
-  HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, halo_stencil_kernel<kMode>, kHaloThreads, smem));
-  cache.push_back({smem, device, per_sm});
-  return per_sm;
+  return per_sm[device];
 }
 
 HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device) {
   HaloGeometry g;
+  HPCP_REQUIRE(tune.tile_kb >= 0 && tune.tile_kb <= 1024, "halo_stencil: tile_kb in 1 .. 1024 (0 -> 16)");
   g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : kHaloDefaultTileKb) * 1024);
-  HPCP_REQUIRE(g.tile_bytes <= kHaloMaxTileBytes, "halo_stencil: tiles of at most 32 KiB (the math warps' registers)");
-  // `stages` counts every tile slot in shared memory: the input ring plus the output staging ring.
-  const int stages = tune.stages > 0 ? tune.stages : kHaloDefaultStages;
-  g.out_stages = tune.out_stages > 0 ? tune.out_stages : std::max(2, stages / 4);
-  g.in_stages = stages - g.out_stages;
-  // The store thread keeps its newest slot until the next store's bulk_wait_read: one output slot would deadlock.
-  HPCP_REQUIRE(g.out_stages >= 2 && g.in_stages >= 1,
-               "halo_stencil: needs >= 2 output and >= 1 input shared-memory stages");
-  g.smem = static_cast<size_t>(stages) * g.tile_bytes + static_cast<size_t>(2 * stages + 1) * 8 + 16;
-  HPCP_REQUIRE(g.smem <= 227 * 1024, "halo_stencil: stages * tile exceed 227 KiB of shared memory");
   const int sms = device_sm_count(device);
   int per_sm = 1;
   // Co-residency: a persistent multi-step launch spins on neighbour words, so every CTA must be resident.
   switch (mode) {
-    case HaloMode::kNone: per_sm = occupancy_of<0>(g.smem); break;
-    case HaloMode::kPull: per_sm = occupancy_of<1>(g.smem); break;
-    case HaloMode::kPush: per_sm = occupancy_of<2>(g.smem); break;
+    case HaloMode::kNone: per_sm = occupancy_of<0>(); break;
+    case HaloMode::kPull: per_sm = occupancy_of<1>(); break;
+    case HaloMode::kPush: per_sm = occupancy_of<2>(); break;
   }
   HPCP_REQUIRE(per_sm >= 1, "halo_stencil: kernel does not fit on an SM");
   const size_t tiles = (row_bytes + g.tile_bytes - 1) / g.tile_bytes;
-  const int resident = std::min(sms * per_sm, kHaloMaxCtas);  // one step word per CTA and side
+  const int resident = std::min(sms * std::min(per_sm, kHaloCtasPerSm), kHaloMaxCtas);  // one step word per CTA
   const int want = tune.ctas > 0 ? std::min(tune.ctas, resident) : resident;
   g.ctas = static_cast<int>(std::max<size_t>(1, std::min<size_t>(tiles, static_cast<size_t>(want))));
   HPCP_REQUIRE(g.ctas <= kHaloMaxCtas, "halo_stencil: more CTAs than flag words");
@@ -530,21 +347,21 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
   const size_t tiles_per_row = (row_bytes + g.tile_bytes - 1) / g.tile_bytes;
   HaloParams p{};
   for (int q = 0; q < 2; ++q) {
-    p.u[q] = reinterpret_cast<unsigned char*>(a.u[q]);
+    p.u[q] = reinterpret_cast<float4*>(a.u[q]);
     if (mode == HaloMode::kPull) {
       HPCP_REQUIRE(a.left_u[q] != nullptr && a.right_u[q] != nullptr, "halo_stencil: pull needs the neighbours' fields");
-      p.up_src[q] = reinterpret_cast<const unsigned char*>(a.left_u[q]) + static_cast<size_t>(a.rows - 1) * row_bytes;
-      p.dn_src[q] = reinterpret_cast<const unsigned char*>(a.right_u[q]);
+      p.up_src[q] = reinterpret_cast<const float4*>(a.left_u[q] + static_cast<size_t>(a.rows - 1) * a.row_elems);
+      p.dn_src[q] = reinterpret_cast<const float4*>(a.right_u[q]);
     } else {
       HPCP_REQUIRE(a.halo_lo[q] != nullptr && a.halo_hi[q] != nullptr, "halo_stencil: halo buffers are needed");
-      p.up_src[q] = reinterpret_cast<const unsigned char*>(a.halo_lo[q]);
-      p.dn_src[q] = reinterpret_cast<const unsigned char*>(a.halo_hi[q]);
+      p.up_src[q] = reinterpret_cast<const float4*>(a.halo_lo[q]);
+      p.dn_src[q] = reinterpret_cast<const float4*>(a.halo_hi[q]);
     }
     if (mode == HaloMode::kPush) {
       HPCP_REQUIRE(a.left_halo_hi[q] != nullptr && a.right_halo_lo[q] != nullptr,
                    "halo_stencil: push needs the neighbours' halo buffers");
-      p.put_first[q] = reinterpret_cast<unsigned char*>(a.left_halo_hi[q]);
-      p.put_last[q] = reinterpret_cast<unsigned char*>(a.right_halo_lo[q]);
+      p.put_first[q] = reinterpret_cast<float4*>(a.left_halo_hi[q]);
+      p.put_last[q] = reinterpret_cast<float4*>(a.right_halo_lo[q]);
     }
   }
   if (mode != HaloMode::kNone) {
@@ -553,13 +370,14 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
     HPCP_REQUIRE(a.flag_set >= 0 && a.flag_set < kHaloFlagSets, "halo_stencil: flag_set out of range");
   }
   p.rows = a.rows;
-  p.row_bytes = row_bytes;
-  p.tile_begin = a.tile_begin;
-  p.tile_end = a.tile_end == 0 ? tiles_per_row : a.tile_end;
-  HPCP_REQUIRE(p.tile_begin < p.tile_end && p.tile_end <= tiles_per_row, "halo_stencil: bad column-tile range");
-  p.tile_bytes = g.tile_bytes;
-  p.in_stages = g.in_stages;
-  p.out_stages = g.out_stages;
+  p.cols.row_vec = a.row_elems / 4;
+  p.cols.tile_vec = g.tile_bytes / 16;
+  p.cols.tile_begin = a.tile_begin;
+  p.cols.tile_end = a.tile_end == 0 ? tiles_per_row : a.tile_end;
+  HPCP_REQUIRE(p.cols.tile_begin < p.cols.tile_end && p.cols.tile_end <= tiles_per_row,
+               "halo_stencil: bad column-tile range");
+  p.cols.ctas = static_cast<uint32_t>(ctas);
+  p.cols.threads = kHaloThreads;
   p.alpha = a.alpha;
   p.s = a.s;
   p.step_base = a.step_base;
@@ -569,14 +387,13 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
   // Flag words: one 32-byte sector per (flag set, side, CTA); the kernel adds blockIdx.x * kHaloFlagWords.
   const size_t set_words = static_cast<size_t>(a.flag_set) * 2 * kHaloMaxCtas * kHaloFlagWords;
   const size_t side_words = static_cast<size_t>(kHaloMaxCtas) * kHaloFlagWords;
-  auto launch = [&](auto kernel) {  // the shared-memory attribute was set when the geometry was computed
-    kernel<<<ctas, kHaloThreads, g.smem, stream>>>(p);
-  };
+  auto launch = [&](auto kernel) { kernel<<<ctas, kHaloThreads, 0, stream>>>(p); };
   if (mode != HaloMode::kNone) {
     p.wait_lo = a.flags_local + set_words;
     p.wait_hi = a.flags_local + set_words + side_words;
     p.signal_lo = a.flags_left + set_words + side_words;  // I am the right neighbour of my left neighbour
     p.signal_hi = a.flags_right + set_words;              // and the left neighbour of my right neighbour
+    p.pace = a.flags_local + set_words + 1;               // word 1 of CTA 0's sector of the wait_lo side (unused)
   }
   switch (mode) {
     case HaloMode::kNone: launch(halo_stencil_kernel<0>); break;

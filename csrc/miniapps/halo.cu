@@ -63,7 +63,7 @@ void print_help() {
                "                    their halo buffers — both from inside the stencil kernel\n"
                " --per-step    one launch per step instead of one persistent K-step launch\n"
                " --stock memcpy     the reference's shape through stock calls: kernel; wait; copies; wait\n"
-               " --ctas N --tile-kb N --stages N --out-stages N   kernel geometry (stages: input + output ring)\n"
+               " --ctas N --tile-kb N   kernel geometry (--stages N / --out-stages N: accepted, ignored)\n"
                " --json FILE   append one JSON row\n"
                " --cpu         no GPU: ranks are host threads, the exchange is a memcpy into (push) or a read out of\n"
                "               (pull) the neighbours' arrays, one barrier per step: options, ring order, verification\n"
@@ -361,9 +361,9 @@ int main(int argc, char** argv) {
         case 8: cfg.stock = optarg; break;
         case 9: cfg.tune.ctas = std::atoi(optarg); break;
         case 10: cfg.tune.tile_kb = std::atoi(optarg); break;
-        case 11: cfg.tune.stages = std::atoi(optarg); break;
+        case 11: break;  // --stages / --out-stages sized the old TMA pipeline's rings: accepted, ignored
         case 12: cfg.json_path = optarg; break;
-        case 13: cfg.tune.out_stages = std::atoi(optarg); break;
+        case 13: break;
         case 14: cfg.cpu = true; break;
         case 15: cfg.dump_path = optarg; break;
         default: print_help(); return 1;

@@ -13,8 +13,8 @@ periodic neighbour exchange with a true step-to-step dependency and no overlap a
   a neighbour sum for ``c``); rows -1 / ``rows`` are the neighbours' boundary rows of the
   same step, so step g+1 consumes what step g produced on the neighbours;
 * the exchange happens INSIDE the stencil kernel (csrc/kernels/halo_stencil.cu): ``pull``
-  reads the boundary rows out of the neighbours' fields over NVLink with TMA bulk loads,
-  ``push`` stores the new boundary rows into the neighbours' halo buffers with TMA bulk
+  reads the boundary rows out of the neighbours' fields over NVLink with 128-bit loads,
+  ``push`` stores the new boundary rows into the neighbours' halo buffers with 128-bit
   stores; per-CTA step words keep it RAW/WAR safe without any barrier or host sync, and
   ``step(k)`` runs k steps in one persistent launch.
 
@@ -432,7 +432,7 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--stock", default=None, choices=("memcpy", "nccl"),
                     help="the reference's shape through stock calls instead: kernel; wait; library transfer; wait")
     ap.add_argument("--tile-kb", type=int, default=0)
-    ap.add_argument("--stages", type=int, default=0)
+    ap.add_argument("--stages", type=int, default=0, help="accepted for old command lines and ignored")
     ap.add_argument("--ctas", type=int, default=0)
     ap.add_argument("--l2-hint", action="store_true",
                     help="accepted for old command lines and ignored: the kernel always picks the L2 policy by row role")

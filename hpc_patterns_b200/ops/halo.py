@@ -28,7 +28,7 @@ def stencil_step_reference(u: torch.Tensor, lo: torch.Tensor, hi: torch.Tensor, 
 def stencil_step(u: torch.Tensor, lo: torch.Tensor, hi: torch.Tensor, out: Optional[torch.Tensor] = None,
                  alpha: float = 0.5, s: float = 0.25, tune: Optional[dict] = None) -> torch.Tensor:
     """``out[r] = alpha*u[r] + s*(u[r-1] + u[r+1])`` with ``u[-1] = lo``, ``u[rows] = hi`` (fp32, contiguous, row length
-    a multiple of 4) through the TMA-tiled sm_90a kernel on the current stream."""
+    a multiple of 4) through the sm_90a K-halo kernel on the current stream."""
     if u.dtype != torch.float32 or u.dim() != 2 or u.shape[1] % 4:
         raise ValueError("u must be fp32 [rows, row_elems] with row_elems a multiple of 4")
     rows, row_elems = u.shape
