@@ -46,6 +46,7 @@ aliases: $(CLIS)
 	          allreduce.bfloat16 allreduce.half \
 	          allreduce-mpi-sycl.float allreduce-mpi-sycl.int \
 	          allreduce-usm-mpi-omp-offload.float allreduce-map-mpi-omp-offload.float; do ln -sf allreduce bin/$$n; done
+	@for n in halo.float halo.double halo.bfloat16 halo.half; do ln -sf halo bin/$$n; done
 	@ln -sf peer2pear bin/peer2pear_i; ln -sf peer2pear bin/peer2pear_w
 	@ln -sf concurency bin/sycl_con; ln -sf omp_con bin/omp_host_threads; ln -sf omp_con bin/omp_nowait
 

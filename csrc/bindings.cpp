@@ -48,7 +48,8 @@ CopyEngine engine_from(const std::string& s) {
 ElemType elem_from(const std::string& s) {
   ElemType t;
   if (elem_type_from_name(s, &t)) return t;
-  throw std::invalid_argument("dtype must be one of float int uint double long ulong short ushort uchar");
+  throw std::invalid_argument(
+      "dtype must be one of float int uint double long ulong short ushort uchar bfloat16 half");
 }
 
 CopyTuning tuning_from(const py::dict& d) {
@@ -318,16 +319,20 @@ PYBIND11_MODULE(_C, m) {
   m.attr("HALO_FLAG_BYTES") = static_cast<size_t>(kHaloFlagBytes);
   m.attr("HALO_FLAG_SETS") = kHaloFlagSets;
   m.attr("HALO_MAX_CTAS") = kHaloMaxCtas;
+  // `dtype`: the field type (float, double, bfloat16 or half, spelled as elem_type_from_name accepts); default float.
   m.def(
       "halo_stencil_ctas",
-      [](size_t row_elems, const std::string& mode, const py::dict& tune, int device) {
-        return halo_stencil_ctas(row_elems, halo_tuning_from(tune), halo_mode_from(mode), device);
+      [](size_t row_elems, const std::string& mode, const py::dict& tune, int device, const std::string& dtype) {
+        return halo_stencil_ctas(row_elems, halo_tuning_from(tune), halo_mode_from(mode), device, elem_from(dtype));
       },
-      py::arg("row_elems"), py::arg("mode") = "pull", py::arg("tune") = py::dict(), py::arg("device") = 0);
+      py::arg("row_elems"), py::arg("mode") = "pull", py::arg("tune") = py::dict(), py::arg("device") = 0,
+      py::arg("dtype") = "float");
   m.def(
       "halo_stencil",
-      [](const py::dict& d, const std::string& mode, const py::dict& tune, int device, uintptr_t stream) {
+      [](const py::dict& d, const std::string& mode, const py::dict& tune, int device, uintptr_t stream,
+         const std::string& dtype) {
         HaloStencilArgs a;
+        a.type = elem_from(dtype);
         auto pair = [&](const char* key, auto& dst) {
           if (!d.contains(key)) return;
           const auto v = d[key].cast<std::vector<uintptr_t>>();
@@ -358,25 +363,37 @@ PYBIND11_MODULE(_C, m) {
         return launch_halo_stencil(a, halo_mode_from(mode), halo_tuning_from(tune), device, as_stream(stream));
       },
       py::arg("args"), py::arg("mode") = "pull", py::arg("tune") = py::dict(), py::arg("device") = 0,
-      py::arg("stream") = 0,
+      py::arg("stream") = 0, py::arg("dtype") = "float",
       "Fused 3-point slab stencil + halo exchange with both ring neighbours (pull / push / none); `steps` steps in one "
       "persistent launch.  Returns the number of CTAs.");
-  m.def("halo_init", [](uintptr_t u, uintptr_t halo_lo, uintptr_t halo_hi, int rows, size_t row_elems, int rank,
-                        int world, uintptr_t stream) {
-    launch_halo_init(as_ptr<float>(u), as_ptr<float>(halo_lo), as_ptr<float>(halo_hi), rows, row_elems, rank, world,
-                     as_stream(stream));
-  });
-  m.def("halo_verify_from_init", [](uintptr_t u, int rows, size_t row_elems, int rank, int world, uint32_t steps,
-                                    float alpha, float s, uintptr_t mismatch, uintptr_t stream) {
-    launch_halo_verify_from_init(as_ptr<const float>(u), rows, row_elems, rank, world, steps, alpha, s,
-                                 as_ptr<unsigned long long>(mismatch), as_stream(stream));
-  });
-  m.def("halo_verify_step", [](uintptr_t u_new, uintptr_t u_old, uintptr_t up_row, uintptr_t dn_row, int rows,
-                               size_t row_elems, float alpha, float s, uintptr_t mismatch, uintptr_t stream) {
-    launch_halo_verify_step(as_ptr<const float>(u_new), as_ptr<const float>(u_old), as_ptr<const float>(up_row),
-                            as_ptr<const float>(dn_row), rows, row_elems, alpha, s,
-                            as_ptr<unsigned long long>(mismatch), as_stream(stream));
-  });
+  m.def(
+      "halo_init",
+      [](uintptr_t u, uintptr_t halo_lo, uintptr_t halo_hi, int rows, size_t row_elems, int rank, int world,
+         uintptr_t stream, const std::string& dtype) {
+        launch_halo_init(as_ptr<void>(u), as_ptr<void>(halo_lo), as_ptr<void>(halo_hi), rows, row_elems, rank, world,
+                         as_stream(stream), elem_from(dtype));
+      },
+      py::arg("u"), py::arg("halo_lo"), py::arg("halo_hi"), py::arg("rows"), py::arg("row_elems"), py::arg("rank"),
+      py::arg("world"), py::arg("stream"), py::arg("dtype") = "float");
+  m.def(
+      "halo_verify_from_init",
+      [](uintptr_t u, int rows, size_t row_elems, int rank, int world, uint32_t steps, float alpha, float s,
+         uintptr_t mismatch, uintptr_t stream, const std::string& dtype) {
+        launch_halo_verify_from_init(as_ptr<const void>(u), rows, row_elems, rank, world, steps, alpha, s,
+                                     as_ptr<unsigned long long>(mismatch), as_stream(stream), elem_from(dtype));
+      },
+      py::arg("u"), py::arg("rows"), py::arg("row_elems"), py::arg("rank"), py::arg("world"), py::arg("steps"),
+      py::arg("alpha"), py::arg("s"), py::arg("mismatch"), py::arg("stream"), py::arg("dtype") = "float");
+  m.def(
+      "halo_verify_step",
+      [](uintptr_t u_new, uintptr_t u_old, uintptr_t up_row, uintptr_t dn_row, int rows, size_t row_elems, float alpha,
+         float s, uintptr_t mismatch, uintptr_t stream, const std::string& dtype) {
+        launch_halo_verify_step(as_ptr<const void>(u_new), as_ptr<const void>(u_old), as_ptr<const void>(up_row),
+                                as_ptr<const void>(dn_row), rows, row_elems, alpha, s,
+                                as_ptr<unsigned long long>(mismatch), as_stream(stream), elem_from(dtype));
+      },
+      py::arg("u_new"), py::arg("u_old"), py::arg("up_row"), py::arg("dn_row"), py::arg("rows"), py::arg("row_elems"),
+      py::arg("alpha"), py::arg("s"), py::arg("mismatch"), py::arg("stream"), py::arg("dtype") = "float");
 
   // ------------------------------------------------- concurrency payloads ----
   m.def("busy_wait", [](uintptr_t out, size_t n_items, size_t tripcount, uintptr_t stream) {

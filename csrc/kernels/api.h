@@ -103,6 +103,23 @@ void launch_fill_triad_inputs(float* b, float* c, size_t n, int rank, cudaStream
 void launch_verify_triad(const float* a, size_t n, int src_rank, float s,
                          unsigned long long* mismatch_count, cudaStream_t stream);
 
+// ------------------------------------------------------------ element types ----
+// Element types of the miniapp's arrays (↔ mpi::get_datatype<T>(), mpi_datatype.hpp:28-51: every one of them is usable
+// with MPI_SUM upstream).  Kernels are instantiated per ADDITION CLASS: signed and unsigned integers of one width share
+// the two's-complement add.  kBFloat16 / kHalf (↔ MPICH's MPIX_C_BF16 / MPIX_C_FLOAT16) add with one round-to-nearest-even
+// per add in the 16-bit format (rings), or accumulate in fp32 and round once (two-shot).  kFloat, kDouble, kBFloat16 and
+// kHalf are also the field types of the halo stencil below.
+enum class ElemType : int {
+  kFloat = 0, kInt = 1, kUInt = 2, kDouble = 3, kLong = 4, kULong = 5, kShort = 6, kUShort = 7, kUChar = 8,
+  kBFloat16 = 9, kHalf = 10
+};
+constexpr size_t elem_size(ElemType t) {
+  return t == ElemType::kDouble || t == ElemType::kLong || t == ElemType::kULong ? 8
+         : t == ElemType::kShort || t == ElemType::kUShort || t == ElemType::kBFloat16 || t == ElemType::kHalf ? 2
+         : t == ElemType::kUChar                                                 ? 1
+                                                                                 : 4;
+}
+
 // ------------------------------------- fused stencil + halo exchange (flagship) ----
 // One step: u'[r][j] = alpha*u[r][j] + s*(u[r-1][j] + u[r+1][j]) over this rank's slab [rows][row_elems] of a field
 // that is periodic in r and split over the ring of ranks; rows -1 / `rows` are the neighbours' boundary rows.
@@ -120,40 +137,45 @@ struct HaloTuning {
   int tile_kb = 0;  // column tile in KiB (1 .. 1024), the unit of CTA ownership and of tile_begin / tile_end; 0 -> 16
 };
 struct HaloStencilArgs {
-  float* u[2] = {nullptr, nullptr};                 // local field, ping-pong: step g reads u[g&1], writes u[(g+1)&1]
-  const float* left_u[2] = {nullptr, nullptr};      // pull: the left / right neighbour's u[0], u[1] (peer-mapped)
-  const float* right_u[2] = {nullptr, nullptr};
-  float* halo_lo[2] = {nullptr, nullptr};           // push / none: local halo rows by step parity (from the left ...
-  float* halo_hi[2] = {nullptr, nullptr};           // ... and from the right neighbour)
-  float* left_halo_hi[2] = {nullptr, nullptr};      // push: the left neighbour's halo_hi (receives my new row 0)
-  float* right_halo_lo[2] = {nullptr, nullptr};     // push: the right neighbour's halo_lo (receives my new last row)
+  // Field type: kFloat (default), kDouble, kBFloat16 or kHalf.  Every pointer below holds elements of this type.
+  ElemType type = ElemType::kFloat;
+  void* u[2] = {nullptr, nullptr};                  // local field, ping-pong: step g reads u[g&1], writes u[(g+1)&1]
+  const void* left_u[2] = {nullptr, nullptr};       // pull: the left / right neighbour's u[0], u[1] (peer-mapped)
+  const void* right_u[2] = {nullptr, nullptr};
+  void* halo_lo[2] = {nullptr, nullptr};            // push / none: local halo rows by step parity (from the left ...
+  void* halo_hi[2] = {nullptr, nullptr};            // ... and from the right neighbour)
+  void* left_halo_hi[2] = {nullptr, nullptr};       // push: the left neighbour's halo_hi (receives my new row 0)
+  void* right_halo_lo[2] = {nullptr, nullptr};      // push: the right neighbour's halo_lo (receives my new last row)
   uint32_t* flags_local = nullptr;                  // kHaloFlagBytes of zeroed words on every rank
   uint32_t* flags_left = nullptr;                   // the neighbours' flag buffers (peer-mapped)
   uint32_t* flags_right = nullptr;
   int flag_set = 0;
   int rows = 0;
-  size_t row_elems = 0;                             // multiple of 4
+  size_t row_elems = 0;                             // a row is a multiple of 16 bytes
   size_t tile_begin = 0, tile_end = 0;              // column tiles of a row to process; end 0 -> all
-  float alpha = 0.5f, s = 0.25f;
+  float alpha = 0.5f, s = 0.25f;                    // fp32 in every field type (widened exactly for double)
   uint32_t step_base = 0;                           // global index of the first step of this launch
   int steps = 1;
   uint64_t timeout_ns = 0;
   uint32_t* status = nullptr;
 };
 // CTAs a launch with this geometry uses (identical on every rank; the flag words are indexed by it).
-int halo_stencil_ctas(size_t row_elems, const HaloTuning& tune, HaloMode mode, int device);
+int halo_stencil_ctas(size_t row_elems, const HaloTuning& tune, HaloMode mode, int device,
+                      ElemType type = ElemType::kFloat);
 int launch_halo_stencil(const HaloStencilArgs& args, HaloMode mode, const HaloTuning& tune, int device,
                         cudaStream_t stream);
 // u[r][j] = u0(rank*rows + r, j); halo_lo / halo_hi (may be null) = the neighbours' boundary rows of the initial field.
-void launch_halo_init(float* u, float* halo_lo, float* halo_hi, int rows, size_t row_elems, int rank, int world,
-                      cudaStream_t stream);
+// u0 is an fp32 value, rounded to the field type (round-to-nearest-even).
+void launch_halo_init(void* u, void* halo_lo, void* halo_hi, int rows, size_t row_elems, int rank, int world,
+                      cudaStream_t stream, ElemType type = ElemType::kFloat);
 // Exact check of this rank's rows after `steps` steps against the closed-form initial field (world*rows <= 128).
-void launch_halo_verify_from_init(const float* u, int rows, size_t row_elems, int rank, int world, uint32_t steps,
-                                  float alpha, float s, unsigned long long* mismatch_count, cudaStream_t stream);
+void launch_halo_verify_from_init(const void* u, int rows, size_t row_elems, int rank, int world, uint32_t steps,
+                                  float alpha, float s, unsigned long long* mismatch_count, cudaStream_t stream,
+                                  ElemType type = ElemType::kFloat);
 // Exact check of one step: u_new against the stencil of u_old with the given boundary rows (any may be peer-mapped).
-void launch_halo_verify_step(const float* u_new, const float* u_old, const float* up_row, const float* dn_row,
-                             int rows, size_t row_elems, float alpha, float s, unsigned long long* mismatch_count,
-                             cudaStream_t stream);
+void launch_halo_verify_step(const void* u_new, const void* u_old, const void* up_row, const void* dn_row, int rows,
+                             size_t row_elems, float alpha, float s, unsigned long long* mismatch_count,
+                             cudaStream_t stream, ElemType type = ElemType::kFloat);
 
 // ------------------------------------------- fused concurrency "megakernel" ----
 // One persistent launch that executes a whole command group of the concurrency
@@ -280,21 +302,6 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
                        cudaStream_t stream);
 
 // ------------------------------------------------------ allreduce miniapp ----
-// Element types of the miniapp's arrays (↔ mpi::get_datatype<T>(), mpi_datatype.hpp:28-51: every one of them is usable
-// with MPI_SUM upstream).  Kernels are instantiated per ADDITION CLASS: signed and unsigned integers of one width share
-// the two's-complement add.  kBFloat16 / kHalf (↔ MPICH's MPIX_C_BF16 / MPIX_C_FLOAT16) add with one round-to-nearest-even
-// per add in the 16-bit format (rings), or accumulate in fp32 and round once (two-shot).
-enum class ElemType : int {
-  kFloat = 0, kInt = 1, kUInt = 2, kDouble = 3, kLong = 4, kULong = 5, kShort = 6, kUShort = 7, kUChar = 8,
-  kBFloat16 = 9, kHalf = 10
-};
-constexpr size_t elem_size(ElemType t) {
-  return t == ElemType::kDouble || t == ElemType::kLong || t == ElemType::kULong ? 8
-         : t == ElemType::kShort || t == ElemType::kUShort || t == ElemType::kBFloat16 || t == ElemType::kHalf ? 2
-         : t == ElemType::kUChar                                                 ? 1
-                                                                                 : 4;
-}
-
 // VA = a, VB = b, VC = c (↔ Initialize, allreduce-mpi-sycl.cpp:33-41). Any pointer may be null.
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
                   ElemType type, cudaStream_t stream);

@@ -4,7 +4,8 @@
 // neighbours; wait; swap; kernel" (allreduce-mpi-sycl.cpp:167-181: Accumulate().wait(),
 // SendRecvRing(VA -> right, VB <- left), swap, Accumulate().wait()): every step's compute
 // consumes what the previous step received, and nothing overlaps.  K-halo is that dependency
-// structure as an H100 kernel.  The global field is [world * rows][row_elems] floats, periodic in
+// structure as an H100 kernel.  The global field is [world * rows][row_elems] elements of one field type (float by
+// default; double, bfloat16 and half share the same body through a 16-byte vector type, below), periodic in
 // the row dimension and split into slabs of `rows` rows per GPU (one row = one message of the
 // p2p benchmark, 188 743 680 B by default, p2p/peer2pear.cpp:115-116).  One step is the stream
 // triad  a = b + s * c  with  b = alpha * u[r],  c = u[r-1] + u[r+1]:
@@ -48,7 +49,13 @@
 #include "api.h"
 
 #include <algorithm>
+#include <cstring>
 #include <mutex>
+#include <string>
+#include <type_traits>
+
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
@@ -59,7 +66,7 @@ namespace hpcp {
 namespace {
 
 constexpr int kHaloCtasPerSm = 2;  // 1024 threads per SM: <= 64 registers per thread
-constexpr int kHaloChunk = 6;      // interior rows loaded ahead of their use
+constexpr int kHaloChunk = 6;      // interior rows loaded ahead of their use (fp32, fp64; see Pair16Vec)
 constexpr int kHaloDefaultTileKb = 16;
 
 struct HaloParams {
@@ -121,52 +128,213 @@ __device__ __forceinline__ void st_put(float4* p, const float4& v) {  // push: t
                "f"(v.w)
                : "memory");
 }
+// The same four accesses on raw 16-byte words, for the double and 16-bit fields.
+__device__ __forceinline__ uint4 ld_keep(const uint4* p) {
+  uint4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ uint4 ld_stream(const uint4* p, uint64_t policy) {
+  uint4 v;
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p), "l"(policy)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_stream(uint4* p, const uint4& v, uint64_t policy) {
+  asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(p), "r"(v.x),
+               "r"(v.y), "r"(v.z), "r"(v.w), "l"(policy)
+               : "memory");
+}
+__device__ __forceinline__ void st_put(uint4* p, const uint4& v) {
+  asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),
+               "r"(v.w)
+               : "memory");
+}
 
-// One step of float4 column v: loads in boundary-first order, outputs rows 0 .. R-1 in order.
-template <int kMode>
+// ------------------------------------------------------- 16-byte vectors ----
+// A "16-byte vector of T" is what one thread moves per row and column: its raw register type (`Raw`), the interior
+// rows it keeps in flight (`kChunk`), the stencil on it, and the two helpers of the step check.  Every field type computes one step per element as: widen the three
+// inputs exactly to the compute type (fp32, or fp64 for double), alpha*u + s*(up + dn) one rounded operation at a time,
+// never contracted, then round once to T (round-to-nearest-even, subnormals kept).  alpha and s are fp32 values.
+struct F32Vec {  // 4 lanes: the fp32 kernels' float4 code
+  using Raw = float4;
+  static constexpr int kChunk = kHaloChunk;
+  __device__ static __forceinline__ Raw stencil(const Raw& up, const Raw& ce, const Raw& dn, float alpha, float s) {
+    return stencil4(up, ce, dn, alpha, s);
+  }
+  __device__ static __forceinline__ Raw from_bits(const uint4& w) {
+    return make_float4(__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w));
+  }
+  __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
+    return (got.x != want.x) + (got.y != want.y) + (got.z != want.z) + (got.w != want.w);
+  }
+};
+
+__device__ __forceinline__ double stencil1(double up, double ce, double dn, float alpha, float s) {
+  return __dadd_rn(__dmul_rn(static_cast<double>(alpha), ce), __dmul_rn(static_cast<double>(s), __dadd_rn(up, dn)));
+}
+
+// Element <-> compute type, and a 32-bit word <-> a pair of 16-bit elements (element 2i in the low half).
+template <class T>
+struct Elem;
+template <>
+struct Elem<float> {
+  using Compute = float;
+  __device__ static __forceinline__ float widen(float x) { return x; }
+  __device__ static __forceinline__ float narrow(float x) { return x; }
+};
+template <>
+struct Elem<double> {
+  using Compute = double;
+  __device__ static __forceinline__ double widen(double x) { return x; }
+  __device__ static __forceinline__ double narrow(double x) { return x; }
+};
+template <>
+struct Elem<__nv_bfloat16> {
+  using Compute = float;
+  __device__ static __forceinline__ float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+  __device__ static __forceinline__ __nv_bfloat16 narrow(float x) { return __float2bfloat16_rn(x); }
+  __device__ static __forceinline__ float2 widen2(uint32_t w) {  // bf16 is the high half of an fp32: one op per lane
+    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
+  }
+  __device__ static __forceinline__ uint32_t narrow2(float2 f) {
+    const __nv_bfloat162 h = __float22bfloat162_rn(f);
+    uint32_t w;
+    memcpy(&w, &h, 4);
+    return w;
+  }
+};
+template <>
+struct Elem<__half> {
+  using Compute = float;
+  __device__ static __forceinline__ float widen(__half x) { return __half2float(x); }
+  __device__ static __forceinline__ __half narrow(float x) { return __float2half_rn(x); }
+  __device__ static __forceinline__ float2 widen2(uint32_t w) {
+    __half2 h;
+    memcpy(&h, &w, 4);
+    return __half22float2(h);
+  }
+  __device__ static __forceinline__ uint32_t narrow2(float2 f) {
+    const __half2 h = __float22half2_rn(f);
+    uint32_t w;
+    memcpy(&w, &h, 4);
+    return w;
+  }
+};
+
+struct F64Vec {  // 2 lanes, each a pair of 32-bit words
+  using Raw = uint4;
+  static constexpr int kChunk = kHaloChunk;
+  __device__ static __forceinline__ double lane(uint32_t lo, uint32_t hi) {
+    return __hiloint2double(static_cast<int>(hi), static_cast<int>(lo));
+  }
+  __device__ static __forceinline__ Raw stencil(const Raw& up, const Raw& ce, const Raw& dn, float alpha, float s) {
+    const double a = stencil1(lane(up.x, up.y), lane(ce.x, ce.y), lane(dn.x, dn.y), alpha, s);
+    const double b = stencil1(lane(up.z, up.w), lane(ce.z, ce.w), lane(dn.z, dn.w), alpha, s);
+    return make_uint4(static_cast<uint32_t>(__double2loint(a)), static_cast<uint32_t>(__double2hiint(a)),
+                      static_cast<uint32_t>(__double2loint(b)), static_cast<uint32_t>(__double2hiint(b)));
+  }
+  __device__ static __forceinline__ Raw from_bits(const uint4& w) { return w; }
+  __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
+    return (lane(got.x, got.y) != lane(want.x, want.y)) + (lane(got.z, got.w) != lane(want.z, want.w));
+  }
+};
+
+template <class T>  // 8 lanes of __nv_bfloat16 or __half, converted one 32-bit pair at a time where it is used
+struct Pair16Vec {
+  using Raw = uint4;
+  // With six interior rows in flight the lane conversions push ptxas past 64 registers (an 8-byte spill inside the
+  // push kernel's column code); five fit.  At R = 8 that is nine of the ten loads of a column in flight at once.
+  static constexpr int kChunk = 5;
+  __device__ static __forceinline__ uint32_t pair(uint32_t up, uint32_t ce, uint32_t dn, float alpha, float s) {
+    const float2 u = Elem<T>::widen2(up), c = Elem<T>::widen2(ce), d = Elem<T>::widen2(dn);
+    return Elem<T>::narrow2(make_float2(stencil1(u.x, c.x, d.x, alpha, s), stencil1(u.y, c.y, d.y, alpha, s)));
+  }
+  __device__ static __forceinline__ Raw stencil(const Raw& up, const Raw& ce, const Raw& dn, float alpha, float s) {
+    return make_uint4(pair(up.x, ce.x, dn.x, alpha, s), pair(up.y, ce.y, dn.y, alpha, s),
+                      pair(up.z, ce.z, dn.z, alpha, s), pair(up.w, ce.w, dn.w, alpha, s));
+  }
+  __device__ static __forceinline__ Raw from_bits(const uint4& w) { return w; }
+  __device__ static __forceinline__ int lanes_differ(uint32_t a, uint32_t b) {
+    const float2 x = Elem<T>::widen2(a), y = Elem<T>::widen2(b);
+    return (x.x != y.x) + (x.y != y.y);
+  }
+  __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
+    return lanes_differ(got.x, want.x) + lanes_differ(got.y, want.y) + lanes_differ(got.z, want.z) +
+           lanes_differ(got.w, want.w);
+  }
+};
+
+template <class T>
+struct VecOf;
+template <>
+struct VecOf<float> {
+  using type = F32Vec;
+};
+template <>
+struct VecOf<double> {
+  using type = F64Vec;
+};
+template <>
+struct VecOf<__nv_bfloat16> {
+  using type = Pair16Vec<__nv_bfloat16>;
+};
+template <>
+struct VecOf<__half> {
+  using type = Pair16Vec<__half>;
+};
+
+// One step of 16-byte column v: loads in boundary-first order, outputs rows 0 .. R-1 in order.
+template <class V, int kMode>
 __device__ __forceinline__ void halo_column(const HaloParams& p, int in, uint64_t v) {
+  using Raw = typename V::Raw;
   const uint64_t evict_first = ptx::l2_policy_evict_first();
   const int R = p.rows;
   const uint64_t rv = p.cols.row_vec;
   const float alpha = p.alpha, s = p.s;
-  const float4* uin = p.u[in] + v;
-  float4* uout = p.u[in ^ 1] + v;
-  auto store = [&](int r, const float4& x) {
+  const Raw* uin = reinterpret_cast<const Raw*>(p.u[in]) + v;
+  Raw* uout = reinterpret_cast<Raw*>(p.u[in ^ 1]) + v;
+  auto store = [&](int r, const Raw& x) {
     st_stream(uout + static_cast<uint64_t>(r) * rv, x, evict_first);
     if (kMode == 2) {
-      if (r == 0) st_put(p.put_first[in ^ 1] + v, x);
-      if (r == R - 1) st_put(p.put_last[in ^ 1] + v, x);
+      if (r == 0) st_put(reinterpret_cast<Raw*>(p.put_first[in ^ 1]) + v, x);
+      if (r == R - 1) st_put(reinterpret_cast<Raw*>(p.put_last[in ^ 1]) + v, x);
     }
   };
-  const float4 last = ld_keep(uin + static_cast<uint64_t>(R - 1) * rv);
-  float4 prev = ld_keep(p.up_src[in] + v);
+  const Raw last = ld_keep(uin + static_cast<uint64_t>(R - 1) * rv);
+  Raw prev = ld_keep(reinterpret_cast<const Raw*>(p.up_src[in]) + v);
   if (R == 1) {
-    store(0, stencil4(prev, last, ld_keep(p.dn_src[in] + v), alpha, s));
+    store(0, V::stencil(prev, last, ld_keep(reinterpret_cast<const Raw*>(p.dn_src[in]) + v), alpha, s));
     return;
   }
-  float4 cur = ld_keep(uin);
-  const float4 dn = ld_keep(p.dn_src[in] + v);
-  for (int base = 1; base < R - 1; base += kHaloChunk) {  // interior rows: row base-1 .. base+kHaloChunk-2 out
-    float4 w[kHaloChunk];
+  Raw cur = ld_keep(uin);
+  const Raw dn = ld_keep(reinterpret_cast<const Raw*>(p.dn_src[in]) + v);
+  for (int base = 1; base < R - 1; base += V::kChunk) {  // interior rows: row base-1 .. base+V::kChunk-2 out
+    Raw w[V::kChunk];
 #pragma unroll
-    for (int i = 0; i < kHaloChunk; ++i)
+    for (int i = 0; i < V::kChunk; ++i)
       if (base + i < R - 1) w[i] = ld_stream(uin + static_cast<uint64_t>(base + i) * rv, evict_first);
 #pragma unroll
-    for (int i = 0; i < kHaloChunk; ++i) {
+    for (int i = 0; i < V::kChunk; ++i) {
       if (base + i < R - 1) {
-        store(base + i - 1, stencil4(prev, cur, w[i], alpha, s));
+        store(base + i - 1, V::stencil(prev, cur, w[i], alpha, s));
         prev = cur;
         cur = w[i];
       }
     }
   }
-  store(R - 2, stencil4(prev, cur, last, alpha, s));
-  store(R - 1, stencil4(cur, last, dn, alpha, s));
+  store(R - 2, V::stencil(prev, cur, last, alpha, s));
+  store(R - 1, V::stencil(cur, last, dn, alpha, s));
 }
 
-// kMode: 0 none, 1 pull, 2 push.
-template <int kMode>
-__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_kernel(const HaloParams p) {
+// The kernel body of every field type.  kMode: 0 none, 1 pull, 2 push.
+template <class V, int kMode>
+__device__ __forceinline__ void halo_body(const HaloParams& p) {
   __shared__ int abort_w;
   const uint32_t ntiles = static_cast<uint32_t>(halo_cta_tiles(p.cols, blockIdx.x));  // < 2^32 float4 per row
   if (ntiles == 0) return;  // same geometry on every rank: nobody waits for this CTA index
@@ -193,7 +361,7 @@ __global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_ker
       }
       const uint64_t first = halo_tile_first(p.cols, blockIdx.x, jj);
       const uint64_t end = halo_tile_end(p.cols, first);
-      for (uint64_t v = first + threadIdx.x; v < end; v += kHaloThreads) halo_column<kMode>(p, in, v);
+      for (uint64_t v = first + threadIdx.x; v < end; v += kHaloThreads) halo_column<V, kMode>(p, in, v);
       if (kMode != 0) {
         __syncthreads();  // every store of the tile (local field and, in push mode, the peers' halos)
         if (threadIdx.x == 0) {
@@ -209,75 +377,112 @@ __global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_ker
   }
 }
 
+// The fp32 kernels (their SASS is fingerprinted in docs/sass/VALIDATED.sha256) ...
+template <int kMode>
+__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_kernel(const HaloParams p) {
+  halo_body<F32Vec, kMode>(p);
+}
+// ... and the other field types: T = double, __nv_bfloat16, __half.
+template <class T, int kMode>
+__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_typed_kernel(const HaloParams p) {
+  halo_body<typename VecOf<T>::type, kMode>(p);
+}
+
 // ------------------------------------------------------------- field values ----
 // u0(global row, column): a hash folded to [-32, 32) with 10 fractional bits, reproducible on the host
-// (models/halo.py::initial_field).
+// (models/halo.py::initial_field).  A field of type T starts at u0 rounded to T (exact for float and double).
 __device__ __forceinline__ float halo_u0(uint32_t grow, uint64_t j) {
   const uint32_t jl = static_cast<uint32_t>(j);
   const uint32_t h = (grow * 2654435761u) ^ (jl * 40503u + (jl >> 11));
   return static_cast<float>(static_cast<int>(h & 0xFFFFu) - 32768) * (1.0f / 1024.0f);
 }
 
-__global__ void halo_init_kernel(float* __restrict__ u, float* __restrict__ halo_lo, float* __restrict__ halo_hi,
-                                 int rows, size_t row_elems, int rank, int world) {
+template <class T>
+__device__ __forceinline__ void halo_init_body(T* __restrict__ u, T* __restrict__ halo_lo, T* __restrict__ halo_hi,
+                                               int rows, size_t row_elems, int rank, int world) {
   const uint32_t grows = static_cast<uint32_t>(rows) * world;
   const uint32_t first = static_cast<uint32_t>(rank) * rows;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   for (size_t j = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j < row_elems; j += stride) {
-    for (int r = 0; r < rows; ++r) u[static_cast<size_t>(r) * row_elems + j] = halo_u0(first + r, j);
-    if (halo_lo != nullptr) halo_lo[j] = halo_u0((first + grows - 1) % grows, j);
-    if (halo_hi != nullptr) halo_hi[j] = halo_u0((first + rows) % grows, j);
+    for (int r = 0; r < rows; ++r) u[static_cast<size_t>(r) * row_elems + j] = Elem<T>::narrow(halo_u0(first + r, j));
+    if (halo_lo != nullptr) halo_lo[j] = Elem<T>::narrow(halo_u0((first + grows - 1) % grows, j));
+    if (halo_hi != nullptr) halo_hi[j] = Elem<T>::narrow(halo_u0((first + rows) % grows, j));
   }
+}
+__global__ void halo_init_kernel(float* __restrict__ u, float* __restrict__ halo_lo, float* __restrict__ halo_hi,
+                                 int rows, size_t row_elems, int rank, int world) {
+  halo_init_body(u, halo_lo, halo_hi, rows, row_elems, rank, world);
+}
+template <class T>
+__global__ void halo_init_typed_kernel(T* __restrict__ u, T* __restrict__ halo_lo, T* __restrict__ halo_hi, int rows,
+                                       size_t row_elems, int rank, int world) {
+  halo_init_body(u, halo_lo, halo_hi, rows, row_elems, rank, world);
 }
 
 // Independent check from the closed-form initial field: every thread owns one column of the GLOBAL
 // field (all world * rows rows), advances it `steps` times with the periodic stencil in the kernel's
-// operation order and compares this rank's rows exactly.
+// operation order and compares this rank's rows exactly.  The column is kept in the compute type, rounded to T after
+// every step as the field is.
 constexpr int kHaloMaxGlobalRows = 128;
-__global__ void halo_verify_init_kernel(const float* __restrict__ u, int rows, size_t row_elems, int rank, int world,
-                                        uint32_t steps, float alpha, float s, unsigned long long* mismatch_count) {
+template <class T>
+__device__ __forceinline__ void halo_verify_init_body(const T* __restrict__ u, int rows, size_t row_elems, int rank,
+                                                      int world, uint32_t steps, float alpha, float s,
+                                                      unsigned long long* mismatch_count) {
+  using C = typename Elem<T>::Compute;
   const int G = rows * world;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   unsigned long long bad = 0;
-  float v[kHaloMaxGlobalRows];
+  C v[kHaloMaxGlobalRows];
   for (size_t j = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j < row_elems; j += stride) {
-    for (int g = 0; g < G; ++g) v[g] = halo_u0(static_cast<uint32_t>(g), j);
+    for (int g = 0; g < G; ++g) v[g] = Elem<T>::widen(Elem<T>::narrow(halo_u0(static_cast<uint32_t>(g), j)));
     for (uint32_t k = 0; k < steps; ++k) {
-      const float first = v[0];
-      float prev = v[G - 1];
+      const C first = v[0];
+      C prev = v[G - 1];
       for (int g = 0; g < G; ++g) {
-        const float cur = v[g];
-        const float next = g + 1 < G ? v[g + 1] : first;
-        v[g] = stencil1(prev, cur, next, alpha, s);
+        const C cur = v[g];
+        const C next = g + 1 < G ? v[g + 1] : first;
+        v[g] = Elem<T>::widen(Elem<T>::narrow(stencil1(prev, cur, next, alpha, s)));
         prev = cur;
       }
     }
-    for (int r = 0; r < rows; ++r) bad += (__ldcg(u + static_cast<size_t>(r) * row_elems + j) != v[rank * rows + r]);
+    for (int r = 0; r < rows; ++r)
+      bad += (Elem<T>::widen(__ldcg(u + static_cast<size_t>(r) * row_elems + j)) != v[rank * rows + r]);
   }
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatch_count, bad);
 }
+__global__ void halo_verify_init_kernel(const float* __restrict__ u, int rows, size_t row_elems, int rank, int world,
+                                        uint32_t steps, float alpha, float s, unsigned long long* mismatch_count) {
+  halo_verify_init_body(u, rows, row_elems, rank, world, steps, alpha, s, mismatch_count);
+}
+template <class T>
+__global__ void halo_verify_init_typed_kernel(const T* __restrict__ u, int rows, size_t row_elems, int rank, int world,
+                                              uint32_t steps, float alpha, float s,
+                                              unsigned long long* mismatch_count) {
+  halo_verify_init_body(u, rows, row_elems, rank, world, steps, alpha, s, mismatch_count);
+}
 
 // Check of ONE step through an independent data path: plain (coherent) vector loads of the step's input,
 // including the neighbours' boundary rows wherever they live (peer-mapped field or local halo buffer).
-__global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const float* __restrict__ u_old,
-                                        const float* __restrict__ up_row, const float* __restrict__ dn_row, int rows,
-                                        size_t row_elems, float alpha, float s, unsigned long long* mismatch_count) {
-  const size_t nvec = row_elems / 4;
+template <class T>
+__device__ __forceinline__ void halo_verify_step_body(const T* __restrict__ u_new, const T* __restrict__ u_old,
+                                                      const T* __restrict__ up_row, const T* __restrict__ dn_row,
+                                                      int rows, size_t row_elems, float alpha, float s,
+                                                      unsigned long long* mismatch_count) {
+  using V = typename VecOf<T>::type;
+  using Raw = typename V::Raw;
+  const size_t nvec = row_elems / (16 / sizeof(T));
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   unsigned long long bad = 0;
-  auto ld = [](const float* base, size_t v) {
-    const uint4 w = ptx::ld_peer_v4(reinterpret_cast<const uint4*>(base) + v);
-    return make_float4(__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w));
-  };
+  auto ld = [](const T* base, size_t v) { return V::from_bits(ptx::ld_peer_v4(reinterpret_cast<const uint4*>(base) + v)); };
   for (size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < nvec; v += stride) {
-    float4 up = ld(up_row, v);
-    float4 ce = ld(u_old, v);
+    Raw up = ld(up_row, v);
+    Raw ce = ld(u_old, v);
     for (int r = 0; r < rows; ++r) {
-      const float4 dn = r + 1 < rows ? ld(u_old + static_cast<size_t>(r + 1) * row_elems, v) : ld(dn_row, v);
-      const float4 want = stencil4(up, ce, dn, alpha, s);
-      const float4 got = ld(u_new + static_cast<size_t>(r) * row_elems, v);
-      bad += (got.x != want.x) + (got.y != want.y) + (got.z != want.z) + (got.w != want.w);
+      const Raw dn = r + 1 < rows ? ld(u_old + static_cast<size_t>(r + 1) * row_elems, v) : ld(dn_row, v);
+      const Raw want = V::stencil(up, ce, dn, alpha, s);
+      const Raw got = ld(u_new + static_cast<size_t>(r) * row_elems, v);
+      bad += V::mismatches(got, want);
       up = ce;
       ce = dn;
     }
@@ -285,15 +490,52 @@ __global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const f
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatch_count, bad);
 }
+__global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const float* __restrict__ u_old,
+                                        const float* __restrict__ up_row, const float* __restrict__ dn_row, int rows,
+                                        size_t row_elems, float alpha, float s, unsigned long long* mismatch_count) {
+  halo_verify_step_body(u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch_count);
+}
+template <class T>
+__global__ void halo_verify_step_typed_kernel(const T* __restrict__ u_new, const T* __restrict__ u_old,
+                                              const T* __restrict__ up_row, const T* __restrict__ dn_row, int rows,
+                                              size_t row_elems, float alpha, float s,
+                                              unsigned long long* mismatch_count) {
+  halo_verify_step_body(u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch_count);
+}
 
 struct HaloGeometry {
   uint32_t tile_bytes;
   int ctas;
 };
 
-template <int kMode>
+template <class T>
+struct Tag {
+  using type = T;
+};
+// Calls f(Tag<T>{}) with the C++ type of a field type; any other type is an error.
+template <class F>
+void with_field_type(ElemType t, const char* what, F&& f) {
+  switch (t) {
+    case ElemType::kFloat: f(Tag<float>{}); return;
+    case ElemType::kDouble: f(Tag<double>{}); return;
+    case ElemType::kBFloat16: f(Tag<__nv_bfloat16>{}); return;
+    case ElemType::kHalf: f(Tag<__half>{}); return;
+    default: break;
+  }
+  HPCP_FAIL(std::string(what) + ": the field type must be float, double, bfloat16 or half");
+}
+
+template <class T, int kMode>
+constexpr auto stencil_kernel() {
+  if constexpr (std::is_same_v<T, float>)
+    return halo_stencil_kernel<kMode>;
+  else
+    return halo_stencil_typed_kernel<T, kMode>;
+}
+
+template <class T, int kMode>
 int occupancy_of() {
-  // One occupancy query per (mode, device), not per launch (per-step launches come here K times).
+  // One occupancy query per (type, mode, device), not per launch (per-step launches come here K times).
   static std::mutex mu;
   static int per_sm[64] = {0};
   int device = 0;
@@ -301,25 +543,28 @@ int occupancy_of() {
   std::lock_guard<std::mutex> lk(mu);
   if (device < 0 || device >= 64 || per_sm[device] == 0) {
     int n = 0;
-    HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, halo_stencil_kernel<kMode>, kHaloThreads, 0));
+    HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, stencil_kernel<T, kMode>(), kHaloThreads, 0));
     if (device < 0 || device >= 64) return n;
     per_sm[device] = n;
   }
   return per_sm[device];
 }
 
-HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device) {
+HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device, ElemType type) {
   HaloGeometry g;
   HPCP_REQUIRE(tune.tile_kb >= 0 && tune.tile_kb <= 1024, "halo_stencil: tile_kb in 1 .. 1024 (0 -> 16)");
   g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : kHaloDefaultTileKb) * 1024);
   const int sms = device_sm_count(device);
   int per_sm = 1;
   // Co-residency: a persistent multi-step launch spins on neighbour words, so every CTA must be resident.
-  switch (mode) {
-    case HaloMode::kNone: per_sm = occupancy_of<0>(); break;
-    case HaloMode::kPull: per_sm = occupancy_of<1>(); break;
-    case HaloMode::kPush: per_sm = occupancy_of<2>(); break;
-  }
+  with_field_type(type, "halo_stencil", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    switch (mode) {
+      case HaloMode::kNone: per_sm = occupancy_of<T, 0>(); break;
+      case HaloMode::kPull: per_sm = occupancy_of<T, 1>(); break;
+      case HaloMode::kPush: per_sm = occupancy_of<T, 2>(); break;
+    }
+  });
   HPCP_REQUIRE(per_sm >= 1, "halo_stencil: kernel does not fit on an SM");
   const size_t tiles = (row_bytes + g.tile_bytes - 1) / g.tile_bytes;
   const int resident = std::min(sms * std::min(per_sm, kHaloCtasPerSm), kHaloMaxCtas);  // one step word per CTA
@@ -331,37 +576,38 @@ HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mo
 
 }  // namespace
 
-int halo_stencil_ctas(size_t row_elems, const HaloTuning& tune, HaloMode mode, int device) {
-  return halo_geometry(row_elems * sizeof(float), tune, mode, device).ctas;
+int halo_stencil_ctas(size_t row_elems, const HaloTuning& tune, HaloMode mode, int device, ElemType type) {
+  return halo_geometry(row_elems * elem_size(type), tune, mode, device, type).ctas;
 }
 
 int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTuning& tune, int device,
                         cudaStream_t stream) {
-  HPCP_REQUIRE(a.rows >= 1 && a.row_elems > 0 && a.row_elems % 4 == 0,
-               "halo_stencil: rows >= 1 and row_elems a positive multiple of 4");
+  const size_t row_bytes = a.row_elems * elem_size(a.type);
+  HPCP_REQUIRE(a.rows >= 1 && a.row_elems > 0 && row_bytes % 16 == 0,
+               "halo_stencil: rows >= 1 and a row a positive multiple of 16 bytes");
   HPCP_REQUIRE(a.steps >= 1, "halo_stencil: steps >= 1");
   HPCP_REQUIRE(a.u[0] != nullptr && a.u[1] != nullptr, "halo_stencil: both field buffers are needed");
-  const size_t row_bytes = a.row_elems * sizeof(float);
-  const HaloGeometry g = halo_geometry(row_bytes, tune, mode, device);
+  const HaloGeometry g = halo_geometry(row_bytes, tune, mode, device, a.type);
   const int ctas = g.ctas;
   const size_t tiles_per_row = (row_bytes + g.tile_bytes - 1) / g.tile_bytes;
   HaloParams p{};
   for (int q = 0; q < 2; ++q) {
-    p.u[q] = reinterpret_cast<float4*>(a.u[q]);
+    p.u[q] = static_cast<float4*>(a.u[q]);
     if (mode == HaloMode::kPull) {
       HPCP_REQUIRE(a.left_u[q] != nullptr && a.right_u[q] != nullptr, "halo_stencil: pull needs the neighbours' fields");
-      p.up_src[q] = reinterpret_cast<const float4*>(a.left_u[q] + static_cast<size_t>(a.rows - 1) * a.row_elems);
-      p.dn_src[q] = reinterpret_cast<const float4*>(a.right_u[q]);
+      p.up_src[q] =
+          reinterpret_cast<const float4*>(static_cast<const char*>(a.left_u[q]) + static_cast<size_t>(a.rows - 1) * row_bytes);
+      p.dn_src[q] = static_cast<const float4*>(a.right_u[q]);
     } else {
       HPCP_REQUIRE(a.halo_lo[q] != nullptr && a.halo_hi[q] != nullptr, "halo_stencil: halo buffers are needed");
-      p.up_src[q] = reinterpret_cast<const float4*>(a.halo_lo[q]);
-      p.dn_src[q] = reinterpret_cast<const float4*>(a.halo_hi[q]);
+      p.up_src[q] = static_cast<const float4*>(a.halo_lo[q]);
+      p.dn_src[q] = static_cast<const float4*>(a.halo_hi[q]);
     }
     if (mode == HaloMode::kPush) {
       HPCP_REQUIRE(a.left_halo_hi[q] != nullptr && a.right_halo_lo[q] != nullptr,
                    "halo_stencil: push needs the neighbours' halo buffers");
-      p.put_first[q] = reinterpret_cast<float4*>(a.left_halo_hi[q]);
-      p.put_last[q] = reinterpret_cast<float4*>(a.right_halo_lo[q]);
+      p.put_first[q] = static_cast<float4*>(a.left_halo_hi[q]);
+      p.put_last[q] = static_cast<float4*>(a.right_halo_lo[q]);
     }
   }
   if (mode != HaloMode::kNone) {
@@ -370,7 +616,7 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
     HPCP_REQUIRE(a.flag_set >= 0 && a.flag_set < kHaloFlagSets, "halo_stencil: flag_set out of range");
   }
   p.rows = a.rows;
-  p.cols.row_vec = a.row_elems / 4;
+  p.cols.row_vec = row_bytes / 16;
   p.cols.tile_vec = g.tile_bytes / 16;
   p.cols.tile_begin = a.tile_begin;
   p.cols.tile_end = a.tile_end == 0 ? tiles_per_row : a.tile_end;
@@ -387,7 +633,6 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
   // Flag words: one 32-byte sector per (flag set, side, CTA); the kernel adds blockIdx.x * kHaloFlagWords.
   const size_t set_words = static_cast<size_t>(a.flag_set) * 2 * kHaloMaxCtas * kHaloFlagWords;
   const size_t side_words = static_cast<size_t>(kHaloMaxCtas) * kHaloFlagWords;
-  auto launch = [&](auto kernel) { kernel<<<ctas, kHaloThreads, 0, stream>>>(p); };
   if (mode != HaloMode::kNone) {
     p.wait_lo = a.flags_local + set_words;
     p.wait_hi = a.flags_local + set_words + side_words;
@@ -395,40 +640,69 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
     p.signal_hi = a.flags_right + set_words;              // and the left neighbour of my right neighbour
     p.pace = a.flags_local + set_words + 1;               // word 1 of CTA 0's sector of the wait_lo side (unused)
   }
-  switch (mode) {
-    case HaloMode::kNone: launch(halo_stencil_kernel<0>); break;
-    case HaloMode::kPull: launch(halo_stencil_kernel<1>); break;
-    case HaloMode::kPush: launch(halo_stencil_kernel<2>); break;
-  }
+  auto launch = [&](auto kernel) { kernel<<<ctas, kHaloThreads, 0, stream>>>(p); };
+  with_field_type(a.type, "halo_stencil", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    switch (mode) {
+      case HaloMode::kNone: launch(stencil_kernel<T, 0>()); break;
+      case HaloMode::kPull: launch(stencil_kernel<T, 1>()); break;
+      case HaloMode::kPush: launch(stencil_kernel<T, 2>()); break;
+    }
+  });
   HPCP_CUDA(cudaGetLastError());
   return ctas;
 }
 
-void launch_halo_init(float* u, float* halo_lo, float* halo_hi, int rows, size_t row_elems, int rank, int world,
-                      cudaStream_t stream) {
+void launch_halo_init(void* u, void* halo_lo, void* halo_hi, int rows, size_t row_elems, int rank, int world,
+                      cudaStream_t stream, ElemType type) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 8));
-  halo_init_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u, halo_lo, halo_hi, rows, row_elems, rank, world);
+  const int ctas = std::max(static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 8)), 1);
+  with_field_type(type, "halo_init", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    T *pu = static_cast<T*>(u), *lo = static_cast<T*>(halo_lo), *hi = static_cast<T*>(halo_hi);
+    if constexpr (std::is_same_v<T, float>)
+      halo_init_kernel<<<ctas, threads, 0, stream>>>(pu, lo, hi, rows, row_elems, rank, world);
+    else
+      halo_init_typed_kernel<T><<<ctas, threads, 0, stream>>>(pu, lo, hi, rows, row_elems, rank, world);
+  });
   HPCP_CUDA(cudaGetLastError());
 }
 
-void launch_halo_verify_from_init(const float* u, int rows, size_t row_elems, int rank, int world, uint32_t steps,
-                                  float alpha, float s, unsigned long long* mismatch_count, cudaStream_t stream) {
+void launch_halo_verify_from_init(const void* u, int rows, size_t row_elems, int rank, int world, uint32_t steps,
+                                  float alpha, float s, unsigned long long* mismatch_count, cudaStream_t stream,
+                                  ElemType type) {
   HPCP_REQUIRE(rows * world <= kHaloMaxGlobalRows, "halo verify: world * rows exceeds 128 global rows");
   const int threads = 128;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 16));
-  halo_verify_init_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u, rows, row_elems, rank, world, steps, alpha, s,
-                                                                    mismatch_count);
+  const int ctas = std::max(static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 16)), 1);
+  with_field_type(type, "halo_verify_from_init", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    const T* pu = static_cast<const T*>(u);
+    if constexpr (std::is_same_v<T, float>)
+      halo_verify_init_kernel<<<ctas, threads, 0, stream>>>(pu, rows, row_elems, rank, world, steps, alpha, s,
+                                                            mismatch_count);
+    else
+      halo_verify_init_typed_kernel<T><<<ctas, threads, 0, stream>>>(pu, rows, row_elems, rank, world, steps, alpha,
+                                                                     s, mismatch_count);
+  });
   HPCP_CUDA(cudaGetLastError());
 }
 
-void launch_halo_verify_step(const float* u_new, const float* u_old, const float* up_row, const float* dn_row,
-                             int rows, size_t row_elems, float alpha, float s, unsigned long long* mismatch_count,
-                             cudaStream_t stream) {
+void launch_halo_verify_step(const void* u_new, const void* u_old, const void* up_row, const void* dn_row, int rows,
+                             size_t row_elems, float alpha, float s, unsigned long long* mismatch_count,
+                             cudaStream_t stream, ElemType type) {
   const int threads = 256;
-  const int ctas = static_cast<int>(std::min<size_t>((row_elems / 4 + threads - 1) / threads, 132 * 8));
-  halo_verify_step_kernel<<<std::max(ctas, 1), threads, 0, stream>>>(u_new, u_old, up_row, dn_row, rows, row_elems,
-                                                                    alpha, s, mismatch_count);
+  const size_t nvec = row_elems * elem_size(type) / 16;
+  const int ctas = std::max(static_cast<int>(std::min<size_t>((nvec + threads - 1) / threads, 132 * 8)), 1);
+  with_field_type(type, "halo_verify_step", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    auto c = [](const void* q) { return static_cast<const T*>(q); };
+    if constexpr (std::is_same_v<T, float>)
+      halo_verify_step_kernel<<<ctas, threads, 0, stream>>>(c(u_new), c(u_old), c(up_row), c(dn_row), rows,
+                                                            row_elems, alpha, s, mismatch_count);
+    else
+      halo_verify_step_typed_kernel<T><<<ctas, threads, 0, stream>>>(c(u_new), c(u_old), c(up_row), c(dn_row), rows,
+                                                                     row_elems, alpha, s, mismatch_count);
+  });
   HPCP_CUDA(cudaGetLastError());
 }
 

@@ -14,6 +14,12 @@
 //   halo -n 8                       # 8 GPUs, pull mode, 8 rows of 188 743 680 B, 20 steps per iteration
 //   halo -n 2 --mode push --rows 1  # NVLink-bound: every computed row is exchanged
 //   halo -n 4 --stock memcpy        # the stock shape instead: kernel, wait, cudaMemcpyAsync to peers, wait
+//   halo -n 4 --type bfloat16       # a bf16 field (also: halo.bfloat16); float (default), double, bfloat16, half
+//
+// Field types: every type computes a step per element as widen the three inputs exactly to the compute type (fp32, or
+// fp64 for double), alpha*u + s*(up + dn) one rounded operation at a time, round once to the type (round-to-nearest-even,
+// subnormals kept).  The initial field is the fp32 closed form rounded to the type.  `--bytes` stays the row size, so a
+// row holds bytes / sizeof(T) elements.
 #include <getopt.h>
 
 #include <algorithm>
@@ -26,6 +32,7 @@
 #include <vector>
 
 #include "../common/cuda_check.h"
+#include "../common/dtype_traits.h"
 #include "../common/nvtx.h"
 #include "../common/peer_mem.h"
 #include "../common/rank_runtime.h"
@@ -50,7 +57,8 @@ struct Config {
   uint64_t timeout_ns = 30ull * 1000 * 1000 * 1000;
   std::string json_path;
   bool cpu = false;                      // host-only plumbing run: ranks are threads, rows live in host vectors
-  std::string dump_path;                 // --cpu only: the final field, rank after rank, raw fp32
+  std::string dump_path;                 // --cpu only: the final field, rank after rank, raw elements of the type
+  ElemType type = ElemType::kFloat;      // --type, or the program-name suffix (halo.bfloat16)
 };
 
 void print_help() {
@@ -63,12 +71,13 @@ void print_help() {
                "                    their halo buffers — both from inside the stencil kernel\n"
                " --per-step    one launch per step instead of one persistent K-step launch\n"
                " --stock memcpy     the reference's shape through stock calls: kernel; wait; copies; wait\n"
+               " --type T      field type: float (default) double bfloat16 half (or the program-name suffix, halo.half)\n"
                " --ctas N --tile-kb N   kernel geometry (--stages N / --out-stages N: accepted, ignored)\n"
                " --json FILE   append one JSON row\n"
                " --cpu         no GPU: ranks are host threads, the exchange is a memcpy into (push) or a read out of\n"
                "               (pull) the neighbours' arrays, one barrier per step: options, ring order, verification\n"
                "               and output of the program on a machine without a device (default 4 ranks)\n"
-               " --dump FILE   with --cpu: the final field (rank after rank, raw fp32), for comparison with an\n"
+               " --dump FILE   with --cpu: the final field (rank after rank, raw elements of the type), for comparison with an\n"
                "               independent implementation\n";
 }
 
@@ -95,12 +104,10 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   cudaStream_t stream;
   HPCP_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   const int left = (me - 1 + P) % P, right = (me + 1) % P;
-  const size_t row_elems = cfg.bytes / 4, slab = static_cast<size_t>(cfg.rows) * cfg.bytes;
-  auto u = [&](int r, int parity) {
-    return reinterpret_cast<float*>(static_cast<char*>(sh.field.ptr[r]) + parity * slab);
-  };
+  const size_t row_elems = cfg.bytes / elem_size(cfg.type), slab = static_cast<size_t>(cfg.rows) * cfg.bytes;
+  auto u = [&](int r, int parity) { return static_cast<char*>(sh.field.ptr[r]) + parity * slab; };
   auto halo = [&](int r, int side, int parity) {
-    return reinterpret_cast<float*>(static_cast<char*>(sh.halo.ptr[r]) + (side * 2 + parity) * cfg.bytes);
+    return static_cast<char*>(sh.halo.ptr[r]) + (side * 2 + parity) * cfg.bytes;
   };
   uint32_t* my_pad = static_cast<uint32_t*>(sh.pads.ptr[me]);
   uint32_t* status = my_pad + kPadWords;
@@ -109,6 +116,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   const HaloMode mode = !cfg.stock.empty() ? HaloMode::kNone : cfg.mode == "push" ? HaloMode::kPush : HaloMode::kPull;
 
   HaloStencilArgs a;
+  a.type = cfg.type;
   for (int q = 0; q < 2; ++q) {
     a.u[q] = u(me, q);
     a.left_u[q] = u(left, q);
@@ -126,7 +134,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   a.timeout_ns = cfg.timeout_ns;
   a.status = status;
 
-  launch_halo_init(u(me, 0), halo(me, 0, 0), halo(me, 1, 0), cfg.rows, row_elems, me, P, stream);
+  launch_halo_init(u(me, 0), halo(me, 0, 0), halo(me, 1, 0), cfg.rows, row_elems, me, P, stream, cfg.type);
   HPCP_CUDA(cudaStreamSynchronize(stream));
   ctx.barrier();
 
@@ -152,7 +160,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
         HPCP_CUDA(cudaStreamSynchronize(stream));                                   // Accumulate(...).wait()
         trace(me, "kernel done", it, k);
         HPCP_CUDA(cudaMemcpyAsync(halo(left, 1, out), u(me, out), cfg.bytes, cudaMemcpyDefault, stream));
-        HPCP_CUDA(cudaMemcpyAsync(halo(right, 0, out), u(me, out) + static_cast<size_t>(cfg.rows - 1) * row_elems,
+        HPCP_CUDA(cudaMemcpyAsync(halo(right, 0, out), u(me, out) + static_cast<size_t>(cfg.rows - 1) * cfg.bytes,
                                   cfg.bytes, cudaMemcpyDefault, stream));
         HPCP_CUDA(cudaStreamSynchronize(stream));                                   // the blocking Send/Recv pair
         trace(me, "copies done", it, k);
@@ -185,7 +193,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   unsigned long long* count = nullptr;
   HPCP_CUDA(cudaMalloc(&count, sizeof *count));
   HPCP_CUDA(cudaMemsetAsync(count, 0, sizeof *count, stream));
-  launch_halo_verify_from_init(u(me, g & 1), cfg.rows, row_elems, me, P, g, a.alpha, a.s, count, stream);
+  launch_halo_verify_from_init(u(me, g & 1), cfg.rows, row_elems, me, P, g, a.alpha, a.s, count, stream, cfg.type);
   unsigned long long bad = 0;
   HPCP_CUDA(cudaMemcpyAsync(&bad, count, sizeof bad, cudaMemcpyDeviceToHost, stream));
   HPCP_CUDA(cudaStreamSynchronize(stream));
@@ -217,6 +225,12 @@ __attribute__((noinline)) float host_stencil1(float prev, float cur, float next,
   const float mid = alpha * cur;
   return mid + side;
 }
+__attribute__((noinline)) double host_stencil1(double prev, double cur, double next, float alpha, float s) {
+  const double sum = prev + next;
+  const double side = static_cast<double>(s) * sum;
+  const double mid = static_cast<double>(alpha) * cur;
+  return mid + side;
+}
 
 float host_u0(uint32_t grow, uint64_t j) {  // halo_u0 of kernels/halo_stencil.cu
   const uint32_t jl = static_cast<uint32_t>(j);
@@ -224,14 +238,46 @@ float host_u0(uint32_t grow, uint64_t j) {  // halo_u0 of kernels/halo_stencil.c
   return static_cast<float>(static_cast<int>(h & 0xFFFFu) - 32768) * (1.0f / 1024.0f);
 }
 
+// Element type <-> compute type on the host, the same roundings as the kernels (cuda_bf16.h / cuda_fp16.h conversions
+// are host functions too).
+template <class T>
+struct HostElem {  // float, double
+  static T widen(T x) { return x; }
+  static T narrow(T x) { return x; }
+};
+template <>
+struct HostElem<__nv_bfloat16> {
+  static float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+  static __nv_bfloat16 narrow(float x) { return __float2bfloat16_rn(x); }
+};
+template <>
+struct HostElem<__half> {
+  static float widen(__half x) { return __half2float(x); }
+  static __half narrow(float x) { return __float2half_rn(x); }
+};
+template <class T>
+T host_stencil(T prev, T cur, T next, float alpha, float s) {
+  using E = HostElem<T>;
+  return E::narrow(host_stencil1(E::widen(prev), E::widen(cur), E::widen(next), alpha, s));
+}
+template <class T>
+T host_init(uint32_t grow, uint64_t j) {
+  return HostElem<T>::narrow(host_u0(grow, j));
+}
+template <class T>
+bool host_same(T a, T b) {
+  return HostElem<T>::widen(a) == HostElem<T>::widen(b);
+}
+
+template <class T>
 int run_on_host(const Config& cfg) {
   const int P = cfg.ranks > 0 ? cfg.ranks : 4;
   HPCP_REQUIRE(P >= 1 && P <= kMaxRanks, "ranks out of range");
   const int R = cfg.rows;
-  const size_t n = cfg.bytes / 4;
+  const size_t n = cfg.bytes / sizeof(T);
   const bool push = cfg.mode == "push" || !cfg.stock.empty();  // the stock shape is a push with host waits
   const float alpha = HaloStencilArgs{}.alpha, sc = HaloStencilArgs{}.s;
-  std::vector<std::vector<float>> u[2], lo[2], hi[2];
+  std::vector<std::vector<T>> u[2], lo[2], hi[2];
   for (int q = 0; q < 2; ++q) {
     u[q].resize(P);
     lo[q].resize(P);
@@ -244,14 +290,14 @@ int run_on_host(const Config& cfg) {
     const int me = ctx.rank, left = (me - 1 + P) % P, right = (me + 1) % P;
     const uint32_t G = static_cast<uint32_t>(P) * R, first = static_cast<uint32_t>(me) * R;
     for (int q = 0; q < 2; ++q) {
-      u[q][me].assign(static_cast<size_t>(R) * n, 0.f);
-      lo[q][me].assign(n, 0.f);
-      hi[q][me].assign(n, 0.f);
+      u[q][me].assign(static_cast<size_t>(R) * n, T{});
+      lo[q][me].assign(n, T{});
+      hi[q][me].assign(n, T{});
     }
     for (size_t j = 0; j < n; ++j) {
-      for (int r = 0; r < R; ++r) u[0][me][static_cast<size_t>(r) * n + j] = host_u0(first + r, j);
-      lo[0][me][j] = host_u0((first + G - 1) % G, j);
-      hi[0][me][j] = host_u0((first + R) % G, j);
+      for (int r = 0; r < R; ++r) u[0][me][static_cast<size_t>(r) * n + j] = host_init<T>(first + r, j);
+      lo[0][me][j] = host_init<T>((first + G - 1) % G, j);
+      hi[0][me][j] = host_init<T>((first + R) % G, j);
     }
     uint32_t g = 0;
     double best = std::numeric_limits<double>::max();
@@ -261,16 +307,16 @@ int run_on_host(const Config& cfg) {
       for (int k = 0; k < cfg.steps; ++k, ++g) {
         const int in = g & 1, out = in ^ 1;
         ctx.barrier();  // every rank finished step g-1: its rows (pull) / my halo arrays (push) hold step g's inputs
-        const float* below = push ? lo[in][me].data() : u[in][left].data() + static_cast<size_t>(R - 1) * n;
-        const float* above = push ? hi[in][me].data() : u[in][right].data();
-        const float* src = u[in][me].data();
-        float* dst = u[out][me].data();
+        const T* below = push ? lo[in][me].data() : u[in][left].data() + static_cast<size_t>(R - 1) * n;
+        const T* above = push ? hi[in][me].data() : u[in][right].data();
+        const T* src = u[in][me].data();
+        T* dst = u[out][me].data();
         for (int r = 0; r < R; ++r) {
-          const float* dn = r == 0 ? below : src + static_cast<size_t>(r - 1) * n;
-          const float* up = r == R - 1 ? above : src + static_cast<size_t>(r + 1) * n;
-          const float* ce = src + static_cast<size_t>(r) * n;
-          float* o = dst + static_cast<size_t>(r) * n;
-          for (size_t j = 0; j < n; ++j) o[j] = host_stencil1(dn[j], ce[j], up[j], alpha, sc);
+          const T* dn = r == 0 ? below : src + static_cast<size_t>(r - 1) * n;
+          const T* up = r == R - 1 ? above : src + static_cast<size_t>(r + 1) * n;
+          const T* ce = src + static_cast<size_t>(r) * n;
+          T* o = dst + static_cast<size_t>(r) * n;
+          for (size_t j = 0; j < n; ++j) o[j] = host_stencil(dn[j], ce[j], up[j], alpha, sc);
         }
         if (push) {  // my new first row is the left neighbour's upper halo, my new last row the right one's lower halo
           std::copy(dst, dst + n, hi[out][left].begin());
@@ -284,15 +330,15 @@ int run_on_host(const Config& cfg) {
     }
     // every column of the whole ring from the closed form, advanced g steps; compare this rank's rows exactly
     unsigned long long bad = 0;
-    std::vector<float> v(G), w(G);
-    const float* mine = u[g & 1][me].data();
+    std::vector<T> v(G), w(G);
+    const T* mine = u[g & 1][me].data();
     for (size_t j = 0; j < n; ++j) {
-      for (uint32_t q = 0; q < G; ++q) v[q] = host_u0(q, j);
+      for (uint32_t q = 0; q < G; ++q) v[q] = host_init<T>(q, j);
       for (uint32_t k = 0; k < g; ++k) {
-        for (uint32_t q = 0; q < G; ++q) w[q] = host_stencil1(v[(q + G - 1) % G], v[q], v[(q + 1) % G], alpha, sc);
+        for (uint32_t q = 0; q < G; ++q) w[q] = host_stencil(v[(q + G - 1) % G], v[q], v[(q + 1) % G], alpha, sc);
         v.swap(w);
       }
-      for (int r = 0; r < R; ++r) bad += mine[static_cast<size_t>(r) * n + j] != v[first + r];
+      for (int r = 0; r < R; ++r) bad += !host_same(mine[static_cast<size_t>(r) * n + j], v[first + r]);
     }
     const double all_bad = ctx.sum(static_cast<double>(bad));
     if (bad == 0)
@@ -308,23 +354,24 @@ int run_on_host(const Config& cfg) {
   if (!cfg.dump_path.empty()) {
     FILE* f = std::fopen(cfg.dump_path.c_str(), "wb");
     HPCP_REQUIRE(f != nullptr, "cannot open --dump file");
-    for (int r = 0; r < P; ++r) std::fwrite(u[final_parity][r].data(), sizeof(float), u[final_parity][r].size(), f);
+    for (int r = 0; r < P; ++r) std::fwrite(u[final_parity][r].data(), sizeof(T), u[final_parity][r].size(), f);
     std::fclose(f);
   }
   const double ms_per_step = best_ms / cfg.steps;
   const double bus = static_cast<double>(P) * 2.0 * static_cast<double>(cfg.bytes) / (ms_per_step * 1e6);
   const std::string what = std::string(!cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode) + "/host-threads";
+  const char* type = elem_type_name(cfg.type);
   std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << best_ms << " ms for " << cfg.steps
             << " steps = " << ms_per_step << " ms/step | halo " << what << " P=" << P << " rows=" << R
-            << " bytes=" << cfg.bytes << " ctas=0 | " << bus << " GB/s P2P bus (aggregate), " << bus / P / 2.0
-            << " GB/s per GPU per direction" << std::endl;
+            << " bytes=" << cfg.bytes << " ctas=0 type=" << type << " | " << bus << " GB/s P2P bus (aggregate), "
+            << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
   if (!cfg.json_path.empty()) {
     if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
       std::fprintf(f,
                    "{\"pattern\":\"halo\",\"variant\":\"%s\",\"ranks\":%d,\"rows\":%d,\"bytes\":%zu,\"steps\":%d,"
                    "\"ms_per_step\":%.6f,\"bus_GBps\":%.3f,\"per_gpu_per_dir_GBps\":%.3f,\"ctas\":0,"
-                   "\"mismatches\":%llu}\n",
-                   what.c_str(), P, R, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, total_bad);
+                   "\"mismatches\":%llu,\"type\":\"%s\"}\n",
+                   what.c_str(), P, R, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, total_bad, type);
       std::fclose(f);
     }
   }
@@ -337,6 +384,11 @@ int main(int argc, char** argv) {
   hpcp::prefer_eager_module_loading();  // spin-waiting kernels + lazy module loading can deadlock (cuda_check.h)
   try {
     Config cfg;
+    {  // type from the program-name suffix (`halo.bfloat16`), like allreduce.<type>
+      const std::string self = argv[0];
+      const auto dot = self.rfind('.');
+      if (dot != std::string::npos) (void)elem_type_from_name(self.substr(dot + 1), &cfg.type);
+    }
     static const option long_opts[] = {
         {"rows", required_argument, nullptr, 1}, {"bytes", required_argument, nullptr, 2},
         {"steps", required_argument, nullptr, 3}, {"iters", required_argument, nullptr, 4},
@@ -345,7 +397,8 @@ int main(int argc, char** argv) {
         {"ctas", required_argument, nullptr, 9}, {"tile-kb", required_argument, nullptr, 10},
         {"stages", required_argument, nullptr, 11}, {"json", required_argument, nullptr, 12},
         {"out-stages", required_argument, nullptr, 13}, {"cpu", no_argument, nullptr, 14},
-        {"dump", required_argument, nullptr, 15}, {"help", no_argument, nullptr, 'h'}, {nullptr, 0, nullptr, 0}};
+        {"dump", required_argument, nullptr, 15}, {"type", required_argument, nullptr, 16},
+        {"help", no_argument, nullptr, 'h'}, {nullptr, 0, nullptr, 0}};
     int opt;
     while ((opt = getopt_long(argc, argv, "hn:", long_opts, nullptr)) != -1) {
       switch (opt) {
@@ -366,6 +419,13 @@ int main(int argc, char** argv) {
         case 13: break;
         case 14: cfg.cpu = true; break;
         case 15: cfg.dump_path = optarg; break;
+        case 16:
+          if (!elem_type_from_name(optarg, &cfg.type)) {
+            std::cerr << "Error: unsupported --type " << optarg << "\n";
+            print_help();
+            return 1;
+          }
+          break;
         default: print_help(); return 1;
       }
     }
@@ -373,7 +433,20 @@ int main(int argc, char** argv) {
     HPCP_REQUIRE(cfg.stock.empty() || cfg.stock == "memcpy", "--stock accepts memcpy");
     HPCP_REQUIRE(cfg.rows >= 1 && cfg.bytes >= 16 && cfg.bytes % 16 == 0, "--rows >= 1, --bytes a multiple of 16");
     HPCP_REQUIRE(cfg.dump_path.empty() || cfg.cpu, "--dump belongs to --cpu");
-    if (cfg.cpu) return run_on_host(cfg);
+    if (cfg.type != ElemType::kFloat && cfg.type != ElemType::kDouble && cfg.type != ElemType::kBFloat16 &&
+        cfg.type != ElemType::kHalf) {
+      std::cerr << "Error: --type must be float, double, bfloat16 or half\n";
+      print_help();
+      return 1;
+    }
+    if (cfg.cpu) {
+      switch (cfg.type) {
+        case ElemType::kDouble: return run_on_host<double>(cfg);
+        case ElemType::kBFloat16: return run_on_host<__nv_bfloat16>(cfg);
+        case ElemType::kHalf: return run_on_host<__half>(cfg);
+        default: return run_on_host<float>(cfg);
+      }
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
       (void)cudaGetLastError();
@@ -390,12 +463,12 @@ int main(int argc, char** argv) {
     if (ranks_per_dev > 1) {  // co-residency of the spinning persistent kernels that share a GPU
       HaloTuning all = cfg.tune;
       all.ctas = 0;
-      const int full = halo_stencil_ctas(cfg.bytes / 4, all, geo_mode, devices[0]);
+      const int full = halo_stencil_ctas(cfg.bytes / elem_size(cfg.type), all, geo_mode, devices[0], cfg.type);
       const int share = std::max(1, full / ranks_per_dev);
       cfg.tune.ctas = cfg.tune.ctas > 0 ? std::min(cfg.tune.ctas, share) : share;
     }
     // the same grid on every rank and in every launch: the step words are indexed by CTA
-    cfg.tune.ctas = halo_stencil_ctas(cfg.bytes / 4, cfg.tune, geo_mode, devices[0]);
+    cfg.tune.ctas = halo_stencil_ctas(cfg.bytes / elem_size(cfg.type), cfg.tune, geo_mode, devices[0], cfg.type);
 
     Shared sh;
     sh.cfg = cfg;
@@ -413,18 +486,19 @@ int main(int argc, char** argv) {
     const double bus = static_cast<double>(P) * 2.0 * static_cast<double>(cfg.bytes) / (ms_per_step * 1e6);
     const std::string what =
         !cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode + (cfg.per_step ? "/per-step" : "/persistent");
+    const char* type = elem_type_name(cfg.type);
     std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << sh.best_ms << " ms for " << cfg.steps
               << " steps = " << ms_per_step << " ms/step | halo " << what << " P=" << P << " rows=" << cfg.rows
-              << " bytes=" << cfg.bytes << " ctas=" << sh.ctas << " | " << bus << " GB/s P2P bus (aggregate), "
-              << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
+              << " bytes=" << cfg.bytes << " ctas=" << sh.ctas << " type=" << type << " | " << bus
+              << " GB/s P2P bus (aggregate), " << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
     if (!cfg.json_path.empty()) {
       if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
         std::fprintf(f,
                      "{\"pattern\":\"halo\",\"variant\":\"%s\",\"ranks\":%d,\"rows\":%d,\"bytes\":%zu,\"steps\":%d,"
                      "\"ms_per_step\":%.6f,\"bus_GBps\":%.3f,\"per_gpu_per_dir_GBps\":%.3f,\"ctas\":%d,"
-                     "\"mismatches\":%llu}\n",
+                     "\"mismatches\":%llu,\"type\":\"%s\"}\n",
                      what.c_str(), P, cfg.rows, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, sh.ctas,
-                     sh.total_bad);
+                     sh.total_bad, type);
         std::fclose(f);
       }
     }

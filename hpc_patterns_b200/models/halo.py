@@ -20,6 +20,12 @@ periodic neighbour exchange with a true step-to-step dependency and no overlap a
 
 ``stock_step`` is the reference's shape through library calls (the thing to beat):
 compute kernel, host wait, ``cudaMemcpyAsync`` to the peers or NCCL send/recv, host wait.
+
+Field types (``dtype``): float32 (default), float64, bfloat16 and float16.  A row stays ``message_bytes`` long, so it
+holds ``message_bytes // itemsize`` elements.  One step per element widens the three inputs exactly to the compute type
+(fp32, or fp64 for float64), evaluates ``alpha*u + s*(up + dn)`` one rounded operation at a time and rounds once to the
+field type (round-to-nearest-even, subnormals kept); ``alpha`` and ``s`` are fp32 values in every type.  The initial
+field is the fp32 closed form rounded to the type.  ``reference_steps`` is that contract in plain PyTorch.
 """
 from __future__ import annotations
 
@@ -34,6 +40,25 @@ from ..parallel.symmetric import SignalPads, SymmetricBuffer, tensor_from_ptr
 REFERENCE_MESSAGE_BYTES = 1179648 * 40 * 4  # 188 743 680, p2p/peer2pear.cpp:115-116
 DEFAULT_ROWS = 8
 MODES = ("pull", "push", "none")
+# field dtype -> the element-type name of the native launchers
+DTYPES = {torch.float32: "float", torch.float64: "double", torch.bfloat16: "bfloat16", torch.float16: "half"}
+# --type spellings (csrc/common/dtype_traits.h::elem_type_from_name) of the four field types
+TYPE_NAMES = {"float": torch.float32, "float32": torch.float32, "f32": torch.float32,
+              "double": torch.float64, "float64": torch.float64, "f64": torch.float64,
+              "bfloat16": torch.bfloat16, "bf16": torch.bfloat16,
+              "half": torch.float16, "float16": torch.float16, "f16": torch.float16, "fp16": torch.float16}
+
+
+def compute_dtype(dtype: torch.dtype) -> torch.dtype:
+    """The type a step of a ``dtype`` field computes in: fp64 for float64, fp32 otherwise."""
+    return torch.float64 if dtype == torch.float64 else torch.float32
+
+
+def _native_type(dtype: torch.dtype) -> dict:
+    """Keyword arguments that select the field type in the native calls: none for fp32, whose calls keep their shape."""
+    if dtype not in DTYPES:
+        raise ValueError(f"dtype must be one of {[str(d) for d in DTYPES]}")
+    return {} if dtype == torch.float32 else {"dtype": DTYPES[dtype]}
 
 
 def balanced_rows(hbm_gbs: float, nvlink_gbs: float) -> int:
@@ -49,21 +74,27 @@ def balanced_rows(hbm_gbs: float, nvlink_gbs: float) -> int:
     return max(1, int(rows))
 
 
-def initial_field(world: int, rows: int, row_elems: int) -> torch.Tensor:
-    """The closed-form initial field of the kernels (halo_u0 in halo_stencil.cu), fp32 [world*rows, row_elems]."""
+def initial_field(world: int, rows: int, row_elems: int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """The closed-form initial field of the kernels (halo_u0 in halo_stencil.cu), [world*rows, row_elems]: fp32 values
+    rounded to ``dtype`` (round-to-nearest-even; exact for float32 and float64)."""
     g = torch.arange(world * rows, dtype=torch.int64).unsqueeze(1)
     j = torch.arange(row_elems, dtype=torch.int64).unsqueeze(0)
     h = ((g * 2654435761) & 0xFFFFFFFF) ^ ((j * 40503 + (j >> 11)) & 0xFFFFFFFF)
-    return (((h & 0xFFFF) - 32768).to(torch.float32)) * (1.0 / 1024.0)
+    u = (((h & 0xFFFF) - 32768).to(torch.float32)) * (1.0 / 1024.0)
+    return u if dtype == torch.float32 else u.to(dtype)
 
 
 def reference_steps(field: torch.Tensor, steps: int, alpha: float = 0.5, s: float = 0.25) -> torch.Tensor:
-    """Plain PyTorch fp32 reference of the whole (undecomposed) periodic stencil, operation by operation."""
+    """Plain PyTorch reference of the whole (undecomposed) periodic stencil, operation by operation in the compute type
+    of ``field.dtype`` (fp64 for float64, else fp32; ``alpha`` and ``s`` are fp32 values), rounded to ``field.dtype``
+    after every step."""
+    ct = compute_dtype(field.dtype)
     u = field.clone()
-    a = torch.tensor(alpha, dtype=torch.float32)
-    b = torch.tensor(s, dtype=torch.float32)
+    a = torch.tensor(alpha, dtype=torch.float32).to(ct)
+    b = torch.tensor(s, dtype=torch.float32).to(ct)
     for _ in range(steps):
-        u = a * u + b * (torch.roll(u, 1, 0) + torch.roll(u, -1, 0))
+        w = u.to(ct)
+        u = (a * w + b * (torch.roll(w, 1, 0) + torch.roll(w, -1, 0))).to(field.dtype)
     return u
 
 
@@ -73,18 +104,22 @@ class HaloStencil:
 
     def __init__(self, comm: Comm, device: int, message_bytes: int = REFERENCE_MESSAGE_BYTES,
                  rows: int = DEFAULT_ROWS, mode: str = "pull", alpha: float = 0.5, s: float = 0.25,
-                 tune: Optional[dict] = None, timeout_s: float = 30.0, _shared: Optional[dict] = None):
+                 tune: Optional[dict] = None, timeout_s: float = 30.0, _shared: Optional[dict] = None,
+                 dtype: torch.dtype = torch.float32):
         if mode not in MODES:
             raise ValueError(f"mode must be one of {MODES}")
         if message_bytes % 16 or message_bytes <= 0:
             raise ValueError("message size (one row) must be a positive multiple of 16 bytes")
         if rows < 1:
             raise ValueError("rows must be >= 1")
+        self._dt = _native_type(dtype)
+        self.dtype = dtype
         self.C = native()
         self.comm, self.device = comm, device
         self.rank, self.world = comm.rank, comm.world
         self.mode, self.alpha, self.s = mode, float(alpha), float(s)
-        self.rows, self.row_bytes, self.row_elems = int(rows), int(message_bytes), int(message_bytes) // 4
+        self.itemsize = torch.empty(0, dtype=dtype).element_size()
+        self.rows, self.row_bytes, self.row_elems = int(rows), int(message_bytes), int(message_bytes) // self.itemsize
         self.tune = dict(tune or {})
         self.left = (self.rank - 1) % self.world
         self.right = (self.rank + 1) % self.world
@@ -97,7 +132,8 @@ class HaloStencil:
             self.field = SymmetricBuffer(comm, 2 * slab, device, zero=False)        # u[0] | u[1]
             self.halo = SymmetricBuffer(comm, 4 * self.row_bytes, device, zero=False)  # lo[0] lo[1] hi[0] hi[1]
             self.flags = SymmetricBuffer(comm, self.C.HALO_FLAG_BYTES, device, zero=True)
-        self.ctas = self.C.halo_stencil_ctas(self.row_elems, "pull" if mode == "none" else mode, self.tune, device)
+        self.ctas = self.C.halo_stencil_ctas(self.row_elems, "pull" if mode == "none" else mode, self.tune, device,
+                                             **self._dt)
         if "ctas" in self.tune:
             self.ctas = min(self.ctas, int(self.tune["ctas"]))
         self.tune["ctas"] = self.ctas   # identical grid in every launch: flag words are indexed by CTA
@@ -116,10 +152,10 @@ class HaloStencil:
         return self.halo.ptrs[rank] + ((0 if side == "lo" else 2) + parity) * self.row_bytes
 
     def u_tensor(self, parity: Optional[int] = None) -> torch.Tensor:
-        """This rank's current field (or the given parity) as a [rows, row_elems] fp32 view."""
+        """This rank's current field (or the given parity) as a [rows, row_elems] view of the field type."""
         parity = self.g & 1 if parity is None else parity
         return tensor_from_ptr(self.u_ptr(self.rank, parity), self.rows * self.row_bytes, self.device,
-                               torch.float32).view(self.rows, self.row_elems)
+                               self.dtype).view(self.rows, self.row_elems)
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -149,7 +185,8 @@ class HaloStencil:
         st = self._stream()
         self.C.memset_async(self.flags.local_ptr, 0, self.C.HALO_FLAG_BYTES, st)
         self.C.halo_init(self.u_ptr(self.rank, 0), self.halo_ptr(self.rank, "lo", 0),
-                         self.halo_ptr(self.rank, "hi", 0), self.rows, self.row_elems, self.rank, self.world, st)
+                         self.halo_ptr(self.rank, "hi", 0), self.rows, self.row_elems, self.rank, self.world, st,
+                         **self._dt)
         self.g = 0
         self._flag_layout = None
         torch.cuda.synchronize(self.device)
@@ -169,7 +206,7 @@ class HaloStencil:
     def step(self, steps: int = 1) -> None:
         """``steps`` time steps, exchange included, in ONE kernel launch on the current stream."""
         self._use_layout(1)
-        self.C.halo_stencil(self._args(steps), self.mode, self.tune, self.device, self._stream())
+        self.C.halo_stencil(self._args(steps), self.mode, self.tune, self.device, self._stream(), **self._dt)
         self.g += steps
         self.launches += 1
 
@@ -177,7 +214,7 @@ class HaloStencil:
     def compute_only(self) -> None:
         """The stencil kernel alone: reads the local halo buffers, exchanges nothing, does not advance the step
         counter (timing only: the field is no longer a valid time series afterwards — reset() before verifying)."""
-        self.C.halo_stencil(self._args(1), "none", self.tune, self.device, self._stream())
+        self.C.halo_stencil(self._args(1), "none", self.tune, self.device, self._stream(), **self._dt)
         self.launches += 1
 
     def exchange_only(self, engine: str = "tma") -> None:
@@ -207,7 +244,7 @@ class HaloStencil:
         stream = torch.cuda.current_stream(self.device)
         st = stream.cuda_stream
         out = (self.g + 1) & 1
-        C.halo_stencil(self._args(1), "none", self.tune, self.device, st)
+        C.halo_stencil(self._args(1), "none", self.tune, self.device, st, **self._dt)
         self.launches += 1
         if host_wait:
             stream.synchronize()                                       # Accumulate(...).wait()
@@ -224,10 +261,10 @@ class HaloStencil:
         elif how == "nccl":
             import torch.distributed as dist
             row = self.row_bytes
-            t_first = tensor_from_ptr(first, row, self.device, torch.float32)
-            t_last = tensor_from_ptr(last, row, self.device, torch.float32)
-            r_lo = tensor_from_ptr(self.halo_ptr(self.rank, "lo", out), row, self.device, torch.float32)
-            r_hi = tensor_from_ptr(self.halo_ptr(self.rank, "hi", out), row, self.device, torch.float32)
+            t_first = tensor_from_ptr(first, row, self.device, self.dtype)
+            t_last = tensor_from_ptr(last, row, self.device, self.dtype)
+            r_lo = tensor_from_ptr(self.halo_ptr(self.rank, "lo", out), row, self.device, self.dtype)
+            r_hi = tensor_from_ptr(self.halo_ptr(self.rank, "hi", out), row, self.device, self.dtype)
             if self.world == 1:
                 r_hi.copy_(t_first)
                 r_lo.copy_(t_last)
@@ -253,7 +290,7 @@ class HaloStencil:
         self._counter.zero_()
         self.C.halo_verify_from_init(self.u_ptr(self.rank, self.g & 1), self.rows, self.row_elems, self.rank,
                                      self.world, self.g & 0xFFFFFFFF, self.alpha, self.s,
-                                     self._counter.data_ptr(), self._stream())
+                                     self._counter.data_ptr(), self._stream(), **self._dt)
         return self._count()
 
     def verify_last_step(self) -> int:
@@ -266,7 +303,7 @@ class HaloStencil:
         self.C.halo_verify_step(self.u_ptr(self.rank, new), self.u_ptr(self.rank, old),
                                 self.u_ptr(self.left, old, self.rows - 1), self.u_ptr(self.right, old, 0),
                                 self.rows, self.row_elems, self.alpha, self.s, self._counter.data_ptr(),
-                                self._stream())
+                                self._stream(), **self._dt)
         return self._count()
 
     def check(self) -> None:
@@ -275,7 +312,7 @@ class HaloStencil:
     # ---- end to end through host memory ------------------------------------------------------
     def make_host_buffers(self) -> List[torch.Tensor]:
         """Two pinned host fields [rows, row_elems]; [0] holds this rank's slab of the current step."""
-        bufs = [torch.empty(self.rows, self.row_elems, dtype=torch.float32).pin_memory() for _ in range(2)]
+        bufs = [torch.empty(self.rows, self.row_elems, dtype=self.dtype).pin_memory() for _ in range(2)]
         bufs[0].copy_(self.u_tensor())
         torch.cuda.synchronize(self.device)
         return bufs
@@ -314,7 +351,7 @@ class HaloStencil:
             up.record(h2d)
             main.wait_event(up)
             C.halo_stencil(self._args(1, flag_set=k, tile_begin=t0, tile_end=t1), self.mode, self.tune, self.device,
-                           main.cuda_stream)
+                           main.cuda_stream, **self._dt)
             self.launches += 1
             done = torch.cuda.Event()
             done.record(main)
@@ -364,15 +401,19 @@ class VirtualRing:
     grids sized so that every CTA of every rank sharing a GPU is resident."""
 
     def __init__(self, world: int, message_bytes: int, rows: int, mode: str = "pull", devices: Optional[List[int]] = None,
-                 alpha: float = 0.5, s: float = 0.25, tune: Optional[dict] = None, timeout_s: float = 20.0):
+                 alpha: float = 0.5, s: float = 0.25, tune: Optional[dict] = None, timeout_s: float = 20.0,
+                 dtype: torch.dtype = torch.float32):
         from ..parallel.local import LocalGroup
 
+        dt = _native_type(dtype)
+        itemsize = torch.empty(0, dtype=dtype).element_size()
         self.group = LocalGroup(world, devices)
         C = native()
         tune = dict(tune or {})
         share = max(self.group.ranks_on(d) for d in set(self.group.devices))
         if share > 1:   # co-residency of the spinning persistent kernels that share a GPU
-            full = C.halo_stencil_ctas(message_bytes // 4, "pull" if mode == "none" else mode, tune, self.group.devices[0])
+            full = C.halo_stencil_ctas(message_bytes // itemsize, "pull" if mode == "none" else mode, tune,
+                                       self.group.devices[0], **dt)
             tune["ctas"] = max(1, min(tune.get("ctas") or full, full // share))
         fields = self.group.symmetric(2 * rows * message_bytes, zero=False)
         halos = self.group.symmetric(4 * message_bytes, zero=False)
@@ -384,7 +425,7 @@ class VirtualRing:
             with torch.cuda.device(dev):
                 self.ranks.append(HaloStencil(self.group.comms[r], dev, message_bytes, rows, mode, alpha, s, tune,
                                               timeout_s, _shared={"pads": pads[r], "field": fields[r],
-                                                                  "halo": halos[r], "flags": flags[r]}))
+                                                                  "halo": halos[r], "flags": flags[r]}, dtype=dtype))
         self.streams = [torch.cuda.Stream(self.group.devices[r]) for r in range(world)]
 
     def step(self, steps: int = 1, persistent: bool = False) -> None:
@@ -415,7 +456,8 @@ class VirtualRing:
 
 
 def main(argv: Optional[List[str]] = None) -> int:
-    """``torchrun --nproc-per-node N -m hpc_patterns_b200 halo [--rows R] [--bytes B] [--steps K] [--mode pull|push]``
+    """``torchrun --nproc-per-node N -m hpc_patterns_b200 halo [--rows R] [--bytes B] [--steps K] [--mode pull|push]
+    [--type float|double|bfloat16|half]``
     — process-per-GPU twin of ``bin/halo``: same report lines (``Passed <rank>``, elapsed, bus GB/s)."""
     import argparse
     import json
@@ -436,13 +478,16 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--ctas", type=int, default=0)
     ap.add_argument("--l2-hint", action="store_true",
                     help="accepted for old command lines and ignored: the kernel always picks the L2 policy by row role")
+    ap.add_argument("--type", default="float", choices=sorted(TYPE_NAMES),
+                    help="field type (default float); a row stays --bytes long")
     ap.add_argument("--json", default=None)
     args = ap.parse_args(argv)
+    dtype = TYPE_NAMES[args.type]
     comm = Comm()
     dev = comm.device
     torch.cuda.set_device(dev)
     tune = {k: v for k, v in (("tile_kb", args.tile_kb), ("stages", args.stages), ("ctas", args.ctas)) if v}
-    hs = HaloStencil(comm, dev, args.bytes, args.rows, args.mode, tune=tune)
+    hs = HaloStencil(comm, dev, args.bytes, args.rows, args.mode, tune=tune, dtype=dtype)
     if args.stock:
         enqueue = lambda: [hs.stock_step(args.stock) for _ in range(args.steps)]      # noqa: E731
     elif args.per_step:
@@ -458,14 +503,15 @@ def main(argv: Optional[List[str]] = None) -> int:
         bus = comm.world * 2 * args.bytes / (m["ms"] * 1e6)
         what = f"stock-{args.stock}" if args.stock else args.mode + ("/per-step" if args.per_step else "/persistent")
         print(f"Elapsed (max over ranks, min of {args.iters}): {m['ms'] * args.steps:.4f} ms for {args.steps} steps = "
-              f"{m['ms']:.5f} ms/step | halo {what} P={comm.world} rows={args.rows} bytes={args.bytes} ctas={hs.ctas} | "
+              f"{m['ms']:.5f} ms/step | halo {what} P={comm.world} rows={args.rows} bytes={args.bytes} ctas={hs.ctas} "
+              f"type={DTYPES[dtype]} | "
               f"{bus:.1f} GB/s P2P bus (aggregate), {bus / comm.world / 2:.1f} GB/s per GPU per direction", flush=True)
         if args.json:
             with open(args.json, "a") as f:
                 f.write(json.dumps({"pattern": "halo", "variant": what, "ranks": comm.world, "rows": args.rows,
                                     "bytes": args.bytes, "steps": args.steps, "ms_per_step": m["ms"],
                                     "bus_GBps": bus, "per_gpu_per_dir_GBps": bus / comm.world / 2, "ctas": hs.ctas,
-                                    "mismatches": total_bad}) + "\n")
+                                    "mismatches": total_bad, "type": DTYPES[dtype]}) + "\n")
     hs.close()
     comm.close()
     return 0 if total_bad == 0 else 1
