@@ -52,6 +52,12 @@ ElemType elem_from(const std::string& s) {
       "dtype must be one of float int uint double long ulong short ushort uchar bfloat16 half");
 }
 
+ReduceOp op_from(const std::string& s) {
+  ReduceOp op;
+  if (reduce_op_from_name(s, &op)) return op;
+  throw std::invalid_argument("op must be one of sum prod product min max, not '" + s + "'");
+}
+
 CopyTuning tuning_from(const py::dict& d) {
   CopyTuning t;
   if (d.contains("ctas")) t.ctas = d["ctas"].cast<int>();
@@ -613,9 +619,14 @@ PYBIND11_MODULE(_C, m) {
     launch_init3(as_ptr<void>(va), as_ptr<void>(vb), as_ptr<void>(vc), n, a, b, c, elem_from(dtype),
                  as_stream(stream));
   });
-  m.def("accumulate", [](uintptr_t va, uintptr_t vc, size_t n, const std::string& dtype, uintptr_t stream) {
-    launch_accumulate(as_ptr<const void>(va), as_ptr<void>(vc), n, elem_from(dtype), as_stream(stream));
-  });
+  m.def(
+      "accumulate",
+      [](uintptr_t va, uintptr_t vc, size_t n, const std::string& dtype, uintptr_t stream, const std::string& op) {
+        launch_accumulate(as_ptr<const void>(va), as_ptr<void>(vc), n, elem_from(dtype), as_stream(stream),
+                          op_from(op));
+      },
+      py::arg("va"), py::arg("vc"), py::arg("n"), py::arg("dtype"), py::arg("stream"), py::arg("op") = "sum",
+      "VC += VA (op=sum), else VC = op(VC, VA); op = sum | prod | product | min | max.");
   m.def("count_mismatch", [](uintptr_t v, size_t n, double expected, const std::string& dtype,
                              uintptr_t count, uintptr_t stream) {
     launch_count_mismatch(as_ptr<const void>(v), n, expected, elem_from(dtype),
@@ -656,8 +667,9 @@ PYBIND11_MODULE(_C, m) {
          uintptr_t arrived_local, uintptr_t arrived_right, int world, size_t n, size_t chunk_elems,
          uint32_t epoch_base, uint64_t timeout_ns, uintptr_t status, const std::string& dtype, int ctas,
          int device, uintptr_t stream, int n_slots, uintptr_t ack_local, uintptr_t ack_left, bool pull,
-         uintptr_t va_left, uintptr_t slots_left) {
+         uintptr_t va_left, uintptr_t slots_left, const std::string& op) {
         RingArgs a;
+        a.op = op_from(op);
         a.pull = pull;
         a.va_left = as_ptr<const void>(va_left);
         a.slots_left = as_ptr<const void>(slots_left);
@@ -683,14 +695,15 @@ PYBIND11_MODULE(_C, m) {
       py::arg("chunk_elems") = 0, py::arg("epoch_base") = 0, py::arg("timeout_ns") = 0,
       py::arg("status") = 0, py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0,
       py::arg("stream") = 0, py::arg("n_slots") = 0, py::arg("ack_local") = 0, py::arg("ack_left") = 0,
-      py::arg("pull") = false, py::arg("va_left") = 0, py::arg("slots_left") = 0);
+      py::arg("pull") = false, py::arg("va_left") = 0, py::arg("slots_left") = 0, py::arg("op") = "sum");
   m.def(
       "ring_rsag",
       [](uintptr_t va, uintptr_t vc, uintptr_t slots_local, uintptr_t slots_right, uintptr_t vc_right,
          uintptr_t arrived_local, uintptr_t arrived_right, int rank, int world, size_t n, size_t chunk_elems,
          uint32_t epoch_base, uint64_t timeout_ns, uintptr_t status, const std::string& dtype, int ctas, int device,
-         uintptr_t stream, const std::string& phases) {
+         uintptr_t stream, const std::string& phases, const std::string& op) {
         RingRsAgArgs a;
+        a.op = op_from(op);
         a.va = as_ptr<const void>(va);
         a.vc = as_ptr<void>(vc);
         a.slots_local = as_ptr<void>(slots_local);
@@ -719,16 +732,17 @@ PYBIND11_MODULE(_C, m) {
       py::arg("arrived_local"), py::arg("arrived_right"), py::arg("rank"), py::arg("world"), py::arg("n"),
       py::arg("chunk_elems") = 0, py::arg("epoch_base") = 0, py::arg("timeout_ns") = 0, py::arg("status") = 0,
       py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0,
-      py::arg("phases") = "allreduce",
+      py::arg("phases") = "allreduce", py::arg("op") = "sum",
       "Reduce-scatter + all-gather ring in one launch per rank (kernels/ring_order.h: rsag_*); "
-      "phases = allreduce | reduce_scatter | all_gather.");
+      "phases = allreduce | reduce_scatter | all_gather; op = sum | prod | product | min | max.");
   m.def(
       "allreduce_two_shot",
       [](const std::vector<uintptr_t>& va, const std::vector<uintptr_t>& vc,
          const std::vector<uintptr_t>& pads, uintptr_t ticket, uint32_t ticket_base, int rank, size_t n,
          uint32_t barrier_epoch, uint64_t timeout_ns, uintptr_t status, const std::string& dtype,
-         int ctas, int device, uintptr_t stream) {
+         int ctas, int device, uintptr_t stream, const std::string& op) {
         TwoShotArgs a;
+        a.op = op_from(op);
         a.world = static_cast<int>(va.size());
         HPCP_REQUIRE(a.world <= kApiMaxRanks && vc.size() == va.size() && pads.size() == va.size(),
                      "two-shot: inconsistent rank lists");
@@ -749,13 +763,15 @@ PYBIND11_MODULE(_C, m) {
       py::arg("va"), py::arg("vc"), py::arg("pads"), py::arg("ticket"), py::arg("ticket_base"),
       py::arg("rank"), py::arg("n"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0,
       py::arg("status") = 0, py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0,
-      py::arg("stream") = 0);
+      py::arg("stream") = 0, py::arg("op") = "sum");
   m.def(
       "allreduce_nvls",
       [](uintptr_t va_mc, uintptr_t vc_mc, const std::vector<uintptr_t>& pads, uintptr_t ticket,
          uint32_t ticket_base, int rank, size_t n, uint32_t barrier_epoch, uint64_t timeout_ns,
-         uintptr_t status, const std::string& dtype, int ctas, int device, uintptr_t stream) {
+         uintptr_t status, const std::string& dtype, int ctas, int device, uintptr_t stream,
+         const std::string& op) {
         NvlsArgs a;
+        a.op = op_from(op);
         a.world = static_cast<int>(pads.size());
         HPCP_REQUIRE(a.world <= kApiMaxRanks, "nvls: too many ranks");
         a.va_mc = as_ptr<const void>(va_mc);
@@ -773,7 +789,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("va_mc"), py::arg("vc_mc"), py::arg("pads"), py::arg("ticket"), py::arg("ticket_base"),
       py::arg("rank"), py::arg("n"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0,
       py::arg("status") = 0, py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0,
-      py::arg("stream") = 0);
+      py::arg("stream") = 0, py::arg("op") = "sum", "In-switch sum; any other op raises.");
 
   // ------------------------------------------------------------- topology ----
   m.def("topology_merge_planes", [](int n_gpus, const std::vector<std::vector<std::string>>& links) {

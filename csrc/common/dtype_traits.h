@@ -114,4 +114,23 @@ inline const char* elem_type_name(ElemType t) {
   return "?";
 }
 
+// Reduction by name: sum, prod (or product), min, max; false if unknown.
+inline bool reduce_op_from_name(const std::string& name, ReduceOp* out) {
+  if (name == "sum") *out = ReduceOp::kSum;
+  else if (name == "prod" || name == "product") *out = ReduceOp::kProd;
+  else if (name == "min") *out = ReduceOp::kMin;
+  else if (name == "max") *out = ReduceOp::kMax;
+  else return false;
+  return true;
+}
+inline const char* reduce_op_name(ReduceOp op) {
+  switch (op) {
+    case ReduceOp::kSum: return "sum";
+    case ReduceOp::kProd: return "prod";
+    case ReduceOp::kMin: return "min";
+    case ReduceOp::kMax: return "max";
+  }
+  return "?";
+}
+
 }  // namespace hpcp

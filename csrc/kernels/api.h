@@ -302,11 +302,16 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
                        cudaStream_t stream);
 
 // ------------------------------------------------------ allreduce miniapp ----
+// The reduction of an allreduce (↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX).  kSum accumulates into VC as the
+// reference does; the other ops overwrite VC (docs/allreduce.md has their semantics per type).  NVLS is sum-only.
+enum class ReduceOp : int { kSum = 0, kProd = 1, kMin = 2, kMax = 3 };
+
 // VA = a, VB = b, VC = c (↔ Initialize, allreduce-mpi-sycl.cpp:33-41). Any pointer may be null.
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
                   ElemType type, cudaStream_t stream);
-// VC += VA, the unfused kernel of the reference pattern (↔ Accumulate, :26-31).
-void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaStream_t stream);
+// VC += VA, the unfused kernel of the reference pattern (↔ Accumulate, :26-31); VC = op(VC, VA) for the other ops.
+void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaStream_t stream,
+                       ReduceOp op = ReduceOp::kSum);
 // Counts elements with |v - expected| >= 1e-6 (↔ the assert loop, :192-204).
 void launch_count_mismatch(const void* v, size_t n, double expected, ElemType type,
                            unsigned long long* count, cudaStream_t stream);
@@ -343,6 +348,7 @@ struct RingArgs {
   bool pull = false;
   const void* va_left = nullptr;
   const void* slots_left = nullptr;
+  ReduceOp op = ReduceOp::kSum;   // not sum: hop 0 overwrites VC, VC = VA[r] o VA[r-1] o ...
 };
 size_t ring_num_chunks(size_t n, size_t chunk_elems, size_t elem_bytes = 4);
 void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int device,
@@ -370,6 +376,7 @@ struct RingRsAgArgs {
   uint64_t timeout_ns = 0;
   uint32_t* status = nullptr;
   int phases = 0;                     // RsAgPhase (ring_order.h)
+  ReduceOp op = ReduceOp::kSum;       // the all-gather phase copies and ignores it
 };
 void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int device, cudaStream_t stream);
 
@@ -388,6 +395,7 @@ struct TwoShotArgs {
   uint32_t barrier_epoch = 0;
   uint64_t timeout_ns = 0;
   uint32_t* status = nullptr;
+  ReduceOp op = ReduceOp::kSum;              // not sum: owner first in every element, ((VA[s] o VA[s+1]) o ...)
 };
 int launch_allreduce_two_shot(const TwoShotArgs& args, ElemType type, int ctas, int device,
                               cudaStream_t stream);
@@ -405,6 +413,7 @@ struct NvlsArgs {
   uint32_t barrier_epoch = 0;
   uint64_t timeout_ns = 0;
   uint32_t* status = nullptr;
+  ReduceOp op = ReduceOp::kSum;  // only kSum: any other op is refused
 };
 int launch_allreduce_nvls(const NvlsArgs& args, ElemType type, int ctas, int device,
                           cudaStream_t stream);

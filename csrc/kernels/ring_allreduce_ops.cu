@@ -1,0 +1,317 @@
+// Allreduce kernels for the reductions other than the sum: prod, min and max (↔ MPI_PROD / MPI_MIN / MPI_MAX).
+//
+// The bodies are the sum kernels' (ring_allreduce.cuh): the same loads, stores, arrival / ack words and barriers, in
+// the same combine order, with a different combine policy.  Two differences on purpose:
+//   * the rings OVERWRITE VC (hop 0 stores VA[r] without reading VC), as MPI_Allreduce does; the sum accumulates;
+//   * two-shot combines owner first, ((VA[s] o VA[s+1]) o ...), in its tail loop too, so every element has one order.
+// Semantics per type (docs/allreduce.md):
+//   min / max   integers compare signed or unsigned by type; floats follow IEEE 754-2019 minimum / maximum (any NaN
+//               gives NaN, -0 < +0), 16-bit floats in their own format (the result is one of the inputs);
+//   prod        integers wrap modulo 2^w (signed and unsigned share the bits, as for the sum); floats round every
+//               product to nearest even without FTZ; two-shot multiplies the 16-bit types in fp32 and rounds once.
+// A NaN result is the type's canonical quiet NaN (all bits set but the sign), the same bits on every rank.
+#include "ring_allreduce.cuh"
+
+namespace hpcp {
+
+namespace {
+
+constexpr uint32_t kNaN32 = 0x7fffffffu;
+constexpr unsigned long long kNaN64 = 0x7fffffffffffffffull;
+
+__device__ __forceinline__ unsigned long long lane64(uint32_t lo, uint32_t hi) {
+  return (static_cast<unsigned long long>(hi) << 32) | lo;
+}
+
+// A combine policy from a function of one 32-bit word (L::f) or of one 64-bit lane (L::f64).
+template <class L>
+struct Words {
+  static __device__ __forceinline__ uint4 combine(const uint4& a, const uint4& b) {
+    return make_uint4(L::f(a.x, b.x), L::f(a.y, b.y), L::f(a.z, b.z), L::f(a.w, b.w));
+  }
+};
+template <class L>
+struct DWords {
+  static __device__ __forceinline__ uint4 combine(const uint4& a, const uint4& b) {
+    const unsigned long long lo = L::f64(lane64(a.x, a.y), lane64(b.x, b.y));
+    const unsigned long long hi = L::f64(lane64(a.z, a.w), lane64(b.z, b.w));
+    return make_uint4(static_cast<uint32_t>(lo), static_cast<uint32_t>(lo >> 32), static_cast<uint32_t>(hi),
+                      static_cast<uint32_t>(hi >> 32));
+  }
+};
+
+// Two 16-bit floating lanes: every NaN lane becomes the canonical 0x7fff (kInf = the +inf bits of the format).
+template <uint32_t kInf>
+__device__ __forceinline__ uint32_t canonical_nan16x2(uint32_t r) {
+  const uint32_t nan = __vcmpgtu2(r & 0x7fff7fffu, kInf * 0x10001u);  // 0xffff in every NaN lane
+  return (r & ~nan) | (0x7fff7fffu & nan);
+}
+template <typename H2>
+constexpr uint32_t kInf16 = std::is_same<H2, __half2>::value ? 0x7c00u : 0x7f80u;
+
+// ------------------------------------------------------------- min / max ----
+// Equal inputs give their bitwise AND (max) or OR (min): the same bits unless they are +0 and -0, and then +0 (max) or
+// -0 (min), the order IEEE maximum / minimum demand and the hardware min / max do not promise.
+template <bool kMax>
+struct MnMxF32 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    float r;  // max.NaN / min.NaN: the canonical NaN if either input is NaN
+    if (kMax)
+      asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(__uint_as_float(a)), "f"(__uint_as_float(b)));
+    else
+      asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(__uint_as_float(a)), "f"(__uint_as_float(b)));
+    return __uint_as_float(a) == __uint_as_float(b) ? (kMax ? a & b : a | b) : __float_as_uint(r);
+  }
+};
+template <typename H2, bool kMax>
+struct MnMxH2 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    const H2 x = *reinterpret_cast<const H2*>(&a), y = *reinterpret_cast<const H2*>(&b);
+    const H2 m = kMax ? __hmax2_nan(x, y) : __hmin2_nan(x, y);  // canonical NaN if either lane input is NaN
+    const uint32_t eq = __heq2_mask(x, y);
+    return (*reinterpret_cast<const uint32_t*>(&m) & ~eq) | ((kMax ? a & b : a | b) & eq);
+  }
+};
+template <bool kMax>
+struct MnMxF64 {
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) {
+    const double x = __longlong_as_double(static_cast<long long>(a));
+    const double y = __longlong_as_double(static_cast<long long>(b));
+    if (x != x || y != y) return kNaN64;
+    if (x == y) return kMax ? a & b : a | b;
+    return (kMax ? x > y : x < y) ? a : b;
+  }
+};
+template <bool kMax>
+struct MnMxS32 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    const int x = static_cast<int>(a), y = static_cast<int>(b);
+    return static_cast<uint32_t>(kMax ? max(x, y) : min(x, y));
+  }
+};
+template <bool kMax>
+struct MnMxU32 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return kMax ? max(a, b) : min(a, b); }
+};
+template <bool kMax>
+struct MnMxS64 {
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) {
+    const long long x = static_cast<long long>(a), y = static_cast<long long>(b);
+    return (kMax ? x > y : x < y) ? a : b;
+  }
+};
+template <bool kMax>
+struct MnMxU64 {
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) {
+    return (kMax ? a > b : a < b) ? a : b;
+  }
+};
+template <bool kMax>
+struct MnMxS16x2 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return kMax ? __vmaxs2(a, b) : __vmins2(a, b); }
+};
+template <bool kMax>
+struct MnMxU16x2 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return kMax ? __vmaxu2(a, b) : __vminu2(a, b); }
+};
+template <bool kMax>
+struct MnMxU8x4 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return kMax ? __vmaxu4(a, b) : __vminu4(a, b); }
+};
+
+// min / max need one class per element type: signed and unsigned integers compare differently.
+template <typename T, bool kMax> struct MinMax;
+template <bool kMax> struct MinMax<float, kMax> : Words<MnMxF32<kMax>> {};
+template <bool kMax> struct MinMax<double, kMax> : DWords<MnMxF64<kMax>> {};
+template <bool kMax> struct MinMax<int, kMax> : Words<MnMxS32<kMax>> {};
+template <bool kMax> struct MinMax<unsigned int, kMax> : Words<MnMxU32<kMax>> {};
+template <bool kMax> struct MinMax<long long, kMax> : DWords<MnMxS64<kMax>> {};
+template <bool kMax> struct MinMax<unsigned long long, kMax> : DWords<MnMxU64<kMax>> {};
+template <bool kMax> struct MinMax<short, kMax> : Words<MnMxS16x2<kMax>> {};
+template <bool kMax> struct MinMax<unsigned short, kMax> : Words<MnMxU16x2<kMax>> {};
+template <bool kMax> struct MinMax<unsigned char, kMax> : Words<MnMxU8x4<kMax>> {};
+template <bool kMax> struct MinMax<__nv_bfloat16, kMax> : Words<MnMxH2<__nv_bfloat162, kMax>> {};
+template <bool kMax> struct MinMax<__half, kMax> : Words<MnMxH2<__half2, kMax>> {};
+template <typename T> struct Max : MinMax<T, true> {};
+template <typename T> struct Min : MinMax<T, false> {};
+
+// ------------------------------------------------------------------ prod ----
+struct MulF32 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    const float r = __fmul_rn(__uint_as_float(a), __uint_as_float(b));
+    return r != r ? kNaN32 : __float_as_uint(r);
+  }
+};
+struct MulF64 {
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) {
+    const double r = __dmul_rn(__longlong_as_double(static_cast<long long>(a)),
+                               __longlong_as_double(static_cast<long long>(b)));
+    return r != r ? kNaN64 : static_cast<unsigned long long>(__double_as_longlong(r));
+  }
+};
+template <typename H2>
+struct MulH2 {  // one product rounded to nearest even in the 16-bit format per lane, subnormals kept
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    const H2 r = __hmul2_rn(*reinterpret_cast<const H2*>(&a), *reinterpret_cast<const H2*>(&b));
+    return canonical_nan16x2<kInf16<H2>>(*reinterpret_cast<const uint32_t*>(&r));
+  }
+};
+struct MulI32 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return a * b; }
+};
+struct MulI64 {
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) { return a * b; }
+};
+// The low w bits of a product depend only on the low w bits of its factors.
+struct MulI16x2 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    return ((a >> 16) * (b >> 16)) << 16 | ((a * b) & 0xffffu);
+  }
+};
+struct MulU8x4 {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) {
+    return ((a >> 24) * (b >> 24)) << 24 | (((a >> 16) * (b >> 16)) & 0xffu) << 16 |
+           (((a >> 8) * (b >> 8)) & 0xffu) << 8 | ((a * b) & 0xffu);
+  }
+};
+
+// prod per addition class (AddClass): signed and unsigned integers share the wrapping product.
+template <typename C> struct Prod;
+template <> struct Prod<float> : Words<MulF32> {};
+template <> struct Prod<double> : DWords<MulF64> {};
+template <> struct Prod<int> : Words<MulI32> {};
+template <> struct Prod<long long> : DWords<MulI64> {};
+template <> struct Prod<short> : Words<MulI16x2> {};
+template <> struct Prod<unsigned char> : Words<MulU8x4> {};
+template <> struct Prod<__nv_bfloat16> : Words<MulH2<__nv_bfloat162>> {};
+template <> struct Prod<__half> : Words<MulH2<__half2>> {};
+
+// Two-shot's 16-bit prod: fp32 products, owner first, rounded once to T, NaN lanes canonical.
+struct MulF32Raw {
+  static __device__ __forceinline__ float apply(float a, float b) { return __fmul_rn(a, b); }
+};
+template <typename T>
+struct Prod8 : Wide8<T, MulF32Raw> {
+  __device__ __forceinline__ uint4 round() const {
+    constexpr uint32_t inf = std::is_same<T, __half>::value ? 0x7c00u : 0x7f80u;
+    const uint4 r = Wide8<T, MulF32Raw>::round();
+    return make_uint4(canonical_nan16x2<inf>(r.x), canonical_nan16x2<inf>(r.y), canonical_nan16x2<inf>(r.z),
+                      canonical_nan16x2<inf>(r.w));
+  }
+};
+template <class Op> struct TwoShotInF32 : std::false_type {};
+template <> struct TwoShotInF32<Prod<__nv_bfloat16>> : std::true_type { using acc = Prod8<__nv_bfloat16>; };
+template <> struct TwoShotInF32<Prod<__half>> : std::true_type { using acc = Prod8<__half>; };
+
+// ---------------------------------------------------------------- kernels ----
+template <class Op, bool kAck>
+__global__ void __launch_bounds__(512) ring_push_op_kernel(const __grid_constant__ RingDev a) {
+  ring_push_body<Op, kAck, true>(a);
+}
+
+template <class Op, bool kTwoSlots>
+__global__ void __launch_bounds__(512) ring_pull_op_kernel(const __grid_constant__ RingPullDev a) {
+  ring_pull_body<Op, kTwoSlots, true>(a);
+}
+
+template <class Op>
+__global__ void __launch_bounds__(512) ring_rsag_op_kernel(const __grid_constant__ RingRsAgDev a) {
+  ring_rsag_body<Op>(a);
+}
+
+template <class Op, int W, int U>
+__global__ void __launch_bounds__(512) two_shot_op_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_body<Op, W, U, true>(a);
+}
+
+template <class Acc, int W, int U>
+__global__ void __launch_bounds__(512) two_shot_f32_op_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_f32_body<Acc, W, U>(a);
+}
+
+// VC = op(VC, VA) over whole vectors; block 0's thread 0 combines the last partial vector in registers and writes back
+// only its tail_bytes.
+template <class Op>
+__global__ void __launch_bounds__(512) combine_kernel(const uint4* __restrict__ va, uint4* __restrict__ vc,
+                                                      size_t nvec, const unsigned char* va_tail,
+                                                      unsigned char* vc_tail, size_t tail_bytes) {
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec; i += stride)
+    vc[i] = Op::combine(vc[i], ptx::ld_weak_v4(va + i));
+  if (blockIdx.x == 0 && threadIdx.x == 0 && tail_bytes > 0) {
+    uint4 x = make_uint4(0, 0, 0, 0), acc = x;
+    unsigned char* xb = reinterpret_cast<unsigned char*>(&x);
+    unsigned char* ab = reinterpret_cast<unsigned char*>(&acc);
+    for (size_t k = 0; k < tail_bytes; ++k) xb[k] = va_tail[k], ab[k] = vc_tail[k];
+    const uint4 r = Op::combine(acc, x);
+    const unsigned char* rb = reinterpret_cast<const unsigned char*>(&r);
+    for (size_t k = 0; k < tail_bytes; ++k) vc_tail[k] = rb[k];
+  }
+}
+
+// Run f(Op{}) with the combine policy of (type, op).
+template <typename F>
+void dispatch_op(ElemType type, ReduceOp op, F&& f) {
+  dispatch_elem(type, [&](auto tag) {
+    using T = decltype(tag);
+    switch (op) {
+      case ReduceOp::kMax: f(Max<T>{}); break;
+      case ReduceOp::kMin: f(Min<T>{}); break;
+      case ReduceOp::kProd: f(Prod<typename AddClass<T>::type>{}); break;
+      case ReduceOp::kSum: HPCP_FAIL("allreduce ops: the sum has its own kernels"); break;
+    }
+  });
+}
+
+template <int W, int U>
+const void* two_shot_op_for(ElemType type, ReduceOp op) {
+  const void* k = nullptr;
+  dispatch_op(type, op, [&](auto tag) {
+    using Op = decltype(tag);
+    if constexpr (TwoShotInF32<Op>::value)
+      k = reinterpret_cast<const void*>(two_shot_f32_op_kernel<typename TwoShotInF32<Op>::acc, W, U>);
+    else
+      k = reinterpret_cast<const void*>(two_shot_op_kernel<Op, W, U>);
+  });
+  return k;
+}
+
+}  // namespace
+
+const void* select_ring_op(ElemType type, ReduceOp op, bool pull, bool two_slots) {
+  const void* k = nullptr;
+  dispatch_op(type, op, [&](auto tag) {
+    using Op = decltype(tag);
+    if (pull)
+      k = two_slots ? reinterpret_cast<const void*>(ring_pull_op_kernel<Op, true>)
+                    : reinterpret_cast<const void*>(ring_pull_op_kernel<Op, false>);
+    else
+      k = two_slots ? reinterpret_cast<const void*>(ring_push_op_kernel<Op, true>)
+                    : reinterpret_cast<const void*>(ring_push_op_kernel<Op, false>);
+  });
+  return k;
+}
+
+const void* select_rsag_op(ElemType type, ReduceOp op) {
+  const void* k = nullptr;
+  dispatch_op(type, op, [&](auto tag) { k = reinterpret_cast<const void*>(ring_rsag_op_kernel<decltype(tag)>); });
+  return k;
+}
+
+// <W, U> as the sum's two-shot: 2/4, 4/4, 8/2, 16/1.
+const void* select_two_shot_op(ElemType type, ReduceOp op, int w) {
+  switch (w) {
+    case 2: return two_shot_op_for<2, 4>(type, op);
+    case 4: return two_shot_op_for<4, 4>(type, op);
+    case 8: return two_shot_op_for<8, 2>(type, op);
+    default: return two_shot_op_for<16, 1>(type, op);
+  }
+}
+
+const void* select_combine_op(ElemType type, ReduceOp op) {
+  const void* k = nullptr;
+  dispatch_op(type, op, [&](auto tag) { k = reinterpret_cast<const void*>(combine_kernel<decltype(tag)>); });
+  return k;
+}
+
+}  // namespace hpcp

@@ -23,6 +23,10 @@
 //                 2(P-1)/P of the block sent per rank (n padded to whole 16-byte vectors x P)
 //   (with -a)     nvls when NVSwitch multicast is available, else two-shot P2P;
 //                 force with --coll nvls|twoshot
+// Reductions (--op, ↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX): sum (default) accumulates into VC; prod, min and max
+// overwrite VC and run on every algorithm except nvls (sum-only; -a picks two-shot for them).  Each op has its own
+// constant-data check, exact in every type up to P = 16: max (rank r holds r) -> P-1, min (P-r) -> 1, prod (2 on the
+// odd ranks below 8, else 1) -> 2^min(P/2, 4).
 #include <cuda_profiler_api.h>
 #include <getopt.h>
 
@@ -57,6 +61,7 @@ struct Config {
   bool use_collective = false;
   AllocKind kind = AllocKind::kDevice;
   ElemType type = ElemType::kFloat;
+  ReduceOp op = ReduceOp::kSum;
   std::string algo = "ring";
   std::string coll = "auto";
   int iters = 5;
@@ -98,6 +103,7 @@ void print_help() {
                "                            separate put + accumulate kernels per step, or the\n"
                "                            bandwidth-optimal reduce-scatter + all-gather ring\n"
                " --coll auto|nvls|twoshot   collective used with -a\n"
+               " --op sum|prod|min|max      reduction (default sum; nvls is sum-only, -a uses two-shot for the others)\n"
                " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
                " --ctas N --chunk N    kernel tuning (CTAs per rank, elements per ring chunk)\n"
                " --pull                fused ring, receiver-driven: every block is LOADED from the left neighbour's\n"
@@ -142,6 +148,79 @@ __nv_bfloat16 host_add(__nv_bfloat16 a, __nv_bfloat16 b) {
 __half host_add(__half a, __half b) { return __float2half_rn(__half2float(a) + __half2float(b)); }
 template <typename T>
 constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
+template <typename T>
+T host_from_float(float x) {
+  return static_cast<T>(x);
+}
+template <>
+__nv_bfloat16 host_from_float(float x) { return __float2bfloat16_rn(x); }
+template <>
+__half host_from_float(float x) { return __float2half_rn(x); }
+
+// The kernels' NaN result: all bits set but the sign (little-endian: the sign bit is in the last byte).
+template <typename T>
+T host_canonical_nan() {
+  T x;
+  std::memset(static_cast<void*>(&x), 0xff, sizeof x);
+  reinterpret_cast<unsigned char*>(&x)[sizeof x - 1] = 0x7f;
+  return x;
+}
+
+// op(a, b) with the kernels' semantics (docs/allreduce.md): integers compare by their own signedness and multiply
+// modulo 2^w; floats follow IEEE maximum / minimum (NaN wins, -0 < +0) and round every product once; the 16-bit floats
+// compare exactly and round every product to their format (from its exact fp64 value); NaN results are canonical.
+template <typename T>
+T host_combine(ReduceOp op, T a, T b) {
+  if (op == ReduceOp::kSum) return host_add(a, b);
+  if constexpr (std::is_integral<T>::value) {
+    if (op == ReduceOp::kProd)
+      return static_cast<T>(static_cast<unsigned long long>(a) * static_cast<unsigned long long>(b));
+    return op == ReduceOp::kMax ? std::max(a, b) : std::min(a, b);
+  } else {
+    const double x = host_to_double(a), y = host_to_double(b);
+    if (std::isnan(x) || std::isnan(y)) return host_canonical_nan<T>();
+    if (op == ReduceOp::kProd) {
+      T r;
+      if constexpr (std::is_same<T, __nv_bfloat16>::value)
+        r = __double2bfloat16(x * y);
+      else if constexpr (std::is_same<T, __half>::value)
+        r = __double2half(x * y);
+      else
+        r = a * b;
+      return std::isnan(host_to_double(r)) ? host_canonical_nan<T>() : r;
+    }
+    if (x == y) return (std::signbit(x) == (op == ReduceOp::kMax)) ? b : a;  // +-0: max takes +0, min -0
+    return (op == ReduceOp::kMax) == (x > y) ? a : b;
+  }
+}
+
+// Constant-data check of every op: what rank r holds and what every element of the result must equal (exact up to
+// P = 16 in every type).
+double op_input(ReduceOp op, int r, int P) {
+  switch (op) {
+    case ReduceOp::kSum: return r;
+    case ReduceOp::kMax: return r;
+    case ReduceOp::kMin: return P - r;
+    case ReduceOp::kProd: return r % 2 == 1 && r < 8 ? 2 : 1;
+  }
+  return 0;
+}
+double op_expected(ReduceOp op, int P) {
+  switch (op) {
+    case ReduceOp::kSum: return 0.5 * P * (P - 1);
+    case ReduceOp::kMax: return P - 1;
+    case ReduceOp::kMin: return 1;
+    case ReduceOp::kProd: return std::ldexp(1.0, std::min(P / 2, 4));
+  }
+  return 0;
+}
+// VC before the run: 0 for the sum, which accumulates into it; for the other ops a value that would change the result
+// if a kernel read VC instead of overwriting it.
+double op_vc_init(ReduceOp op, int P) { return op == ReduceOp::kMax ? P : 0; }
+// The JSON rows carry "op" only when it is not the sum (sum rows keep their shape).
+std::string op_json(ReduceOp op) {
+  return op == ReduceOp::kSum ? std::string() : std::string(",\"op\":\"") + reduce_op_name(op) + "\"";
+}
 
 double first_element_as_double(const void* p, ElemType t) {
   switch (t) {
@@ -231,6 +310,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
         a.barrier_epoch = barrier_epoch;
         a.timeout_ns = cfg.timeout_ns;
         a.status = status;
+        a.op = cfg.op;
         ticket_issued += launch_allreduce_nvls(a, cfg.type, cfg.ctas, dev, stream);
       } else {
         TwoShotArgs a;
@@ -247,6 +327,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
         a.barrier_epoch = barrier_epoch;
         a.timeout_ns = cfg.timeout_ns;
         a.status = status;
+        a.op = cfg.op;
         ticket_issued += launch_allreduce_two_shot(a, cfg.type, cfg.ctas, dev, stream);
       }
     } else if (cfg.algo == "ring") {
@@ -264,6 +345,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       a.timeout_ns = cfg.timeout_ns;
       a.status = status;
       a.n_slots = cfg.slots;
+      a.op = cfg.op;
       if (cfg.pull) {  // receiver-driven: load from the left neighbour instead of being stored into
         a.pull = true;
         a.va_left = sh.va.ptr[left];
@@ -292,6 +374,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       a.timeout_ns = cfg.timeout_ns;
       a.status = status;
       a.phases = kRsAgAllreduce;
+      a.op = cfg.op;
       if (!replay) ring_epoch += sh.epoch_advance;
       launch_ring_rsag(a, cfg.type, cfg.ctas, dev, stream);
     } else {  // ring-unfused: the reference's step structure with separate kernels
@@ -300,7 +383,10 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       void* other = sh.vb.ptr[me];
       void* right_cur = sh.va.ptr[right];     // what the right neighbour currently calls VA
       void* right_other = sh.vb.ptr[right];   // ... and VB (where my block must land)
-      launch_accumulate(cur, vc, sh.n, cfg.type, stream);
+      if (cfg.op == ReduceOp::kSum)
+        launch_accumulate(cur, vc, sh.n, cfg.type, stream);
+      else  // the other ops overwrite VC: step 0 is VC = VA
+        HPCP_CUDA(cudaMemcpyAsync(vc, cur, sh.n * esz, cudaMemcpyDeviceToDevice, stream));
       for (int s = 1; s < P; ++s) {
         ++step_epoch;
         // Post the receive: my VB is free (my previous put from it has completed in-stream).
@@ -321,7 +407,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
         launch_wait(my_pad + kPadDone + left, step_epoch, cfg.timeout_ns, status, stream);
         std::swap(cur, other);
         std::swap(right_cur, right_other);
-        launch_accumulate(cur, vc, sh.n, cfg.type, stream);
+        launch_accumulate(cur, vc, sh.n, cfg.type, stream, cfg.op);
       }
     }
 
@@ -329,9 +415,10 @@ void rank_main(RankCtx& ctx, Shared& sh) {
 
   for (int it = 0; it < cfg.warmup + cfg.iters; ++it) {
     NvtxRange iter_range(it < cfg.warmup ? "allreduce warm-up" : "allreduce timed");
-    // (Re-)initialise outside the timed region: VA = VB = rank, VC = 0.
+    // (Re-)initialise outside the timed region: VA = VB = rank (the op's input), VC = 0 (sum) or a poison value.
+    const double x = op_input(cfg.op, me, P);
     launch_init3(va, cfg.algo == "ring-unfused" && !cfg.use_collective ? sh.vb.ptr[me] : nullptr, vc,
-                 sh.n, me, me, 0, cfg.type, stream);
+                 sh.n, x, x, op_vc_init(cfg.op, P), cfg.type, stream);
     HPCP_CUDA(cudaStreamSynchronize(stream));
     ctx.barrier();
     launch_barrier_all(pad_list.data(), me, P, ++barrier_epoch, cfg.timeout_ns, status, stream);
@@ -350,7 +437,8 @@ void rank_main(RankCtx& ctx, Shared& sh) {
     if (it >= cfg.warmup) best_ms = std::min(best_ms, t);
   }
 
-  // Verify: every element of VC equals P(P-1)/2.
+  // Verify: every element of VC equals P(P-1)/2 (sum), or the op's constant result.
+  const double want = op_expected(cfg.op, P);
   unsigned long long bad = 0;
   const bool mapped_copy = !sh.host_vc.empty();
   if (mapped_copy) {
@@ -358,12 +446,12 @@ void rank_main(RankCtx& ctx, Shared& sh) {
     // own array (:163-164) and prints "<rank> <VC[0]>" (:161).
     HPCP_CUDA(cudaMemcpyAsync(sh.host_vc[me], vc, sh.n * esz, cudaMemcpyDeviceToHost, stream));
     HPCP_CUDA(cudaStreamSynchronize(stream));
-    bad = count_mismatch_on_host(sh.host_vc[me], sh.n, 0.5 * P * (P - 1), cfg.type);
+    bad = count_mismatch_on_host(sh.host_vc[me], sh.n, want, cfg.type);
   } else {
     unsigned long long* count = nullptr;
     HPCP_CUDA(cudaMalloc(&count, sizeof *count));
     HPCP_CUDA(cudaMemsetAsync(count, 0, sizeof *count, stream));
-    launch_count_mismatch(vc, sh.n, 0.5 * P * (P - 1), cfg.type, count, stream);
+    launch_count_mismatch(vc, sh.n, want, cfg.type, count, stream);
     HPCP_CUDA(cudaMemcpyAsync(&bad, count, sizeof bad, cudaMemcpyDeviceToHost, stream));
     HPCP_CUDA(cudaStreamSynchronize(stream));
     (void)cudaFree(count);
@@ -422,14 +510,32 @@ int run_on_host_typed(const Config& cfg) {
   std::vector<std::vector<T>> va(P), vb(P), vc(P);
   double elapsed_ms = 0;
   unsigned long long total_bad = 0;
+  const ReduceOp op = cfg.op;
   run_ranks(P, [&](RankCtx& ctx) {
     const int me = ctx.rank, right = (me + 1) % P;
-    va[me].assign(n, static_cast<T>(me));
-    vb[me].assign(n, static_cast<T>(me));
-    vc[me].assign(n, static_cast<T>(0));
+    va[me].assign(n, static_cast<T>(op_input(op, me, P)));
+    vb[me].assign(n, static_cast<T>(op_input(op, me, P)));
+    vc[me].assign(n, static_cast<T>(op_vc_init(op, P)));
     ctx.barrier();
     const auto t0 = std::chrono::steady_clock::now();
-    if (cfg.use_collective && kSum16InF32<T>) {
+    if (cfg.use_collective && op != ReduceOp::kSum) {
+      // two-shot's op rule: element i belongs to slice s = i*P/n, whose owner combines VA[s], VA[s+1], ... (ranks mod
+      // P) in that order; the 16-bit prod multiplies in fp32 and rounds once
+      for (size_t i = 0; i < n; ++i) {
+        const int s = static_cast<int>(i * P / n);
+        if constexpr (kSum16InF32<T>) {
+          if (op == ReduceOp::kProd) {
+            float acc = static_cast<float>(host_to_double(va[s][i]));
+            for (int q = 1; q < P; ++q) acc *= static_cast<float>(host_to_double(va[(s + q) % P][i]));
+            vc[me][i] = std::isnan(acc) ? host_canonical_nan<T>() : host_from_float<T>(acc);
+            continue;
+          }
+        }
+        T acc = va[s][i];
+        for (int q = 1; q < P; ++q) acc = host_combine(op, acc, va[(s + q) % P][i]);
+        vc[me][i] = acc;
+      }
+    } else if (cfg.use_collective && kSum16InF32<T>) {
       // two-shot's 16-bit rule: element i belongs to slice s = i*P/n, whose owner s sums VA[s], VA[s+1], ... (ranks
       // mod P) in fp32 and rounds once
       for (size_t i = 0; i < n; ++i) {
@@ -450,7 +556,7 @@ int run_on_host_typed(const Config& cfg) {
         const T* src = (rsag_reads_vc(h, P) ? vc[me].data() : va[me].data()) + seg;
         const int rs = rsag_src_slot(h, kRsAgAllreduce, P);
         for (size_t i = 0; i < seg_n; ++i)
-          x[i] = rs >= 0 ? host_add(vb[me][rs * seg_n + i], src[i]) : src[i];
+          x[i] = rs >= 0 ? host_combine(op, vb[me][rs * seg_n + i], src[i]) : src[i];
         if (rsag_writes_own_vc(h, P)) std::memcpy(vc[me].data() + seg, x.data(), seg_n * sizeof(T));
         if (rsag_forwards(h, kRsAgAllreduce, P)) {
           const int fs = rsag_fwd_slot(h, P);
@@ -460,19 +566,22 @@ int run_on_host_typed(const Config& cfg) {
         ctx.barrier();  // the hop has landed everywhere
       }
     } else {
-      for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[me][i]);
+      if (op == ReduceOp::kSum)
+        for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[me][i]);
+      else  // the other ops overwrite VC
+        vc[me] = va[me];
       for (int s = 1; s < P; ++s) {
         std::memcpy(vb[right].data(), va[me].data(), n * sizeof(T));  // "send right"
         ctx.barrier();                                                 // everybody received
         va[me].swap(vb[me]);
         ctx.barrier();                                                 // nobody still reads the old VA
-        for (size_t i = 0; i < n; ++i) vc[me][i] = host_add(vc[me][i], va[me][i]);
+        for (size_t i = 0; i < n; ++i) vc[me][i] = host_combine(op, vc[me][i], va[me][i]);
       }
     }
     const double ms =
         std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     const double t = ctx.max(ms);
-    const T want = static_cast<T>(P * (P - 1) / 2);
+    const T want = static_cast<T>(op_expected(op, P));
     unsigned long long bad = 0;
     for (size_t i = 0; i < n; ++i) bad += std::abs(host_to_double(vc[me][i]) - host_to_double(want)) >= 1e-6;
     const double all_bad = ctx.sum(static_cast<double>(bad));
@@ -488,6 +597,7 @@ int run_on_host_typed(const Config& cfg) {
   std::cout << "Elapsed (max over ranks): " << elapsed_ms << " ms | "
             << (cfg.use_collective ? "collective" : rsag ? "host-ring-rsag" : "ring") << " " << elem_type_name(cfg.type)
             << " host-threads P=" << P << " N=2^" << cfg.log2_elems << " arrays=" << alloc_kind_name(cfg.kind)
+            << (op != ReduceOp::kSum ? std::string(" op=") + reduce_op_name(op) : std::string())
             << " (host vectors in this mode)" << std::endl;
   if (!cfg.json_path.empty()) {  // same row shape as the GPU path; the algo name marks the plumbing run
     if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
@@ -496,10 +606,10 @@ int run_on_host_typed(const Config& cfg) {
                                              : static_cast<double>(P - 1) * n * sizeof(T);
       std::fprintf(f,
                    "{\"pattern\":\"allreduce\",\"algo\":\"%s\",\"type\":\"%s\",\"alloc\":\"host-vectors\","
-                   "\"ranks\":%d,\"elements\":%zu,\"ms\":%.6f,\"GBps_sent_per_rank\":%.3f,\"mismatches\":%llu}\n",
+                   "\"ranks\":%d,\"elements\":%zu,\"ms\":%.6f,\"GBps_sent_per_rank\":%.3f,\"mismatches\":%llu%s}\n",
                    cfg.use_collective ? "host-collective" : rsag ? "host-ring-rsag" : "host-ring",
                    elem_type_name(cfg.type), P, n, elapsed_ms,
-                   elapsed_ms > 0 ? sent / (elapsed_ms * 1e6) : 0.0, total_bad);
+                   elapsed_ms > 0 ? sent / (elapsed_ms * 1e6) : 0.0, total_bad, op_json(op).c_str());
       std::fclose(f);
     }
   }
@@ -556,6 +666,7 @@ int main(int argc, char** argv) {
                                        {"pull", no_argument, nullptr, 11},
                                        {"map-alias", no_argument, nullptr, 12},
                                        {"profile-relaunch", no_argument, nullptr, 13},
+                                       {"op", required_argument, nullptr, 14},
                                        {"help", no_argument, nullptr, 'h'},
                                        {nullptr, 0, nullptr, 0}};
     int opt;
@@ -582,6 +693,9 @@ int main(int argc, char** argv) {
         case 9: cfg.cpu = true; break;
         case 12: cfg.map_alias = true; break;
         case 13: cfg.profile_relaunch = true; break;
+        case 14:
+          if (!reduce_op_from_name(optarg, &cfg.op)) HPCP_FAIL(std::string("unknown --op ") + optarg + " (sum|prod|min|max)");
+          break;
         case 10: cfg.slots = std::atoi(optarg); break;
         case 11: cfg.pull = true; break;
         default: print_help(); return 1;
@@ -593,6 +707,8 @@ int main(int argc, char** argv) {
     HPCP_REQUIRE(cfg.slots == 0 || cfg.slots == 2, "--slots must be 2 (or omitted)");
     HPCP_REQUIRE(cfg.algo != "ring-rsag" || (cfg.slots == 0 && !cfg.pull),
                  "--slots 2 and --pull are variants of --algo ring, not of ring-rsag");
+    HPCP_REQUIRE(cfg.op == ReduceOp::kSum || !cfg.use_collective || cfg.coll != "nvls",
+                 std::string("--coll nvls is sum-only: --op ") + reduce_op_name(cfg.op) + " needs --coll twoshot or auto");
 
     if (cfg.cpu) return run_on_host(cfg);
     const int ndev = visible_device_count();
@@ -636,6 +752,11 @@ int main(int argc, char** argv) {
         // float: in-switch reduction where multicast exists.
         want_nvls = ranks_per_dev == 1 && cfg.kind == AllocKind::kDevice && cfg.type == ElemType::kFloat;
         for (int d : devices) want_nvls = want_nvls && NodeMemory::multicast_supported(d);
+        if (cfg.op != ReduceOp::kSum) {
+          want_nvls = false;
+          std::cout << "# -a --op " << reduce_op_name(cfg.op) << ": NVLS reduces sums only; using two-shot P2P"
+                    << std::endl;
+        }
       }
       if (want_nvls) {
         try {
@@ -688,7 +809,8 @@ int main(int argc, char** argv) {
     const double gbps = sent / (sh.best_ms * 1e-3) * 1e-9;
     std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << sh.best_ms << " ms | "
               << algo_name << " " << elem_type_name(cfg.type) << " " << alloc_kind_name(cfg.kind)
-              << " P=" << P << " N=2^" << cfg.log2_elems << " | " << gbps
+              << " P=" << P << " N=2^" << cfg.log2_elems
+              << (cfg.op != ReduceOp::kSum ? std::string(" op=") + reduce_op_name(cfg.op) : std::string()) << " | " << gbps
               << " GB/s sent per rank (" << gbps / 450.0 * 100.0 << "% of the 450 GB/s NVLink 4 nominal per direction)"
               << std::endl;
     if (!cfg.json_path.empty()) {
@@ -697,9 +819,9 @@ int main(int argc, char** argv) {
         std::fprintf(f,
                      "{\"pattern\":\"allreduce\",\"algo\":\"%s\",\"type\":\"%s\",\"alloc\":\"%s\","
                      "\"ranks\":%d,\"elements\":%zu,\"ms\":%.6f,\"GBps_sent_per_rank\":%.3f,"
-                     "\"mismatches\":%llu}\n",
+                     "\"mismatches\":%llu%s}\n",
                      algo_name.c_str(), elem_type_name(cfg.type), alloc_kind_name(cfg.kind), P, sh.n,
-                     sh.best_ms, gbps, sh.total_bad);
+                     sh.best_ms, gbps, sh.total_bad, op_json(cfg.op).c_str());
         std::fclose(f);
       }
     }

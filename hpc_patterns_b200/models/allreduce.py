@@ -16,6 +16,10 @@ element of VC equals P(P-1)/2.  Algorithms:
   ring-nccl     the reference pattern verbatim through stock calls: accumulate kernel,
                 NCCL send/recv, host wait, P-1 times — the baseline K-ring must beat
 
+Reductions (``op``, ↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX): ``sum`` (default) accumulates into VC; ``prod``, ``min``
+and ``max`` overwrite it, on every algorithm but nvls (sum-only).  Each op has its own constant-data check: max (rank r
+holds r) -> P-1, min (P-r) -> 1, prod (2 on the odd ranks below 8, else 1) -> 2^min(P/2, 4).
+
 The native single-process CLI twin is ``bin/allreduce`` (csrc/miniapps/allreduce.cu).
 """
 from __future__ import annotations
@@ -40,10 +44,43 @@ _TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32,
                 "long": torch.int64, "ulong": torch.int64, "short": torch.int16, "ushort": torch.int16,
                 "uchar": torch.uint8, "bfloat16": torch.bfloat16, "half": torch.float16}
 FLOAT16_TYPES = ("bfloat16", "half")
+OPS = ("sum", "prod", "min", "max")
+_OP_ALIASES = {"product": "prod"}
+UNSIGNED_TYPES = ("uint", "ulong", "ushort")   # torch stand-ins are signed: NCCL min/max would compare them signed
 
 
-def expected_value(world: int) -> float:
+def reduce_op(op: str) -> str:
+    """The canonical name of a reduction (``product`` is ``prod``); ValueError if unknown."""
+    op = _OP_ALIASES.get(op, op)
+    if op not in OPS:
+        raise ValueError(f"op must be one of {OPS} (or 'product'), not {op!r}")
+    return op
+
+
+def expected_value(world: int, op: str = "sum") -> float:
+    """Every element of VC after the constant-data run of ``op`` (see ``op_input``)."""
+    if op == "max":
+        return world - 1.0
+    if op == "min":
+        return 1.0
+    if op == "prod":
+        return 2.0 ** min(world // 2, 4)
     return world * (world - 1) / 2.0
+
+
+def op_input(op: str, rank: int, world: int) -> float:
+    """What ``rank`` holds in the constant-data run of ``op`` (exact in every type up to 16 ranks)."""
+    if op == "min":
+        return float(world - rank)
+    if op == "prod":
+        return 2.0 if rank % 2 == 1 and rank < 8 else 1.0
+    return float(rank)
+
+
+def _nccl_op(op: str):
+    import torch.distributed as dist
+    return {"sum": dist.ReduceOp.SUM, "prod": dist.ReduceOp.PRODUCT, "min": dist.ReduceOp.MIN,
+            "max": dist.ReduceOp.MAX}[op]
 
 
 def bytes_sent_per_rank(algo: str, nbytes: int, world: int) -> float:
@@ -65,14 +102,19 @@ class AllreduceResult:
     ms: float
     mismatches: int
     elem_bytes: int = 4
+    op: str = "sum"
 
     def row(self) -> dict:
+        """One JSON row; ``"op"`` only when it is not the sum (sum rows keep their shape)."""
         nbytes = self.elements * self.elem_bytes
         sent = bytes_sent_per_rank(self.algo, nbytes, self.world)
         gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
-        return {"pattern": "allreduce", "algo": self.algo, "type": self.dtype, "ranks": self.world,
-                "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
-                "frac_of_450GBps": gbps / 450.0, "mismatches": self.mismatches}
+        row = {"pattern": "allreduce", "algo": self.algo, "type": self.dtype, "ranks": self.world,
+               "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
+               "frac_of_450GBps": gbps / 450.0, "mismatches": self.mismatches}
+        if self.op != "sum":
+            row["op"] = self.op
+        return row
 
 
 def element_count(elem_bytes: int, world: int, log2_elems: int = 25, n_elems: int = 0) -> int:
@@ -112,17 +154,26 @@ def _layout(algo: str, C, n: int, esz: int, world: int, chunk_elems: int, slots_
 class AllreduceMiniapp:
     def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float",
                  algo: str = "ring", chunk_elems: int = 0, ctas: int = 0, timeout_s: float = 30.0,
-                 slots: int = 0, pull: bool = False, n_elems: int = 0, _shared: Optional[dict] = None):
+                 slots: int = 0, pull: bool = False, n_elems: int = 0, op: str = "sum",
+                 _shared: Optional[dict] = None):
         """``slots=2`` (fused ring only): two receive slots + per-chunk acks — the reference's VA/VB double
         buffer — instead of ``world-1`` slots without flow control.  ``pull=True`` (fused ring only): receiver-driven,
         every block is loaded from the left neighbour's memory instead of being stored into the right neighbour's.
         ``n_elems``: exact element count per rank instead of 2^log2_elems.  ``_shared``: buffers made by an
         in-process group (``VirtualAllreduce``): ``pads``, ``va``, ``vc`` and, where the algorithm uses them, ``vb`` and
-        ``slots``."""
+        ``slots``.  ``op``: sum (default), prod / product, min or max; nvls is sum-only, and the NCCL algorithms refuse
+        min / max on unsigned types (their torch stand-ins are signed)."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
         if dtype not in _TORCH_DTYPE:
             raise ValueError(f"dtype must be one of {sorted(_TORCH_DTYPE)}")
+        op = reduce_op(op)
+        if op != "sum" and algo == "nvls":
+            raise ValueError(f"nvls reduces sums only: op={op} needs twoshot or a ring")
+        if op in ("min", "max") and algo in ("nccl", "ring-nccl") and dtype in UNSIGNED_TYPES:
+            raise ValueError(f"{algo} compares {dtype} as a signed torch type: op={op} is refused")
+        self.op = op
+        self._op_kw = {} if op == "sum" else {"op": op}   # sum calls stay exactly as they were
         if _shared is not None and algo not in VIRTUAL_ALGOS:
             raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
         self.C = native()
@@ -191,7 +242,10 @@ class AllreduceMiniapp:
     def initialize(self) -> None:
         va, vc = self._ptrs()
         vb = self.vb.local_ptr if self.vb is not None else 0
-        self.C.init3(va, vb, vc, self.n, float(self.rank), float(self.rank), 0.0, self.dtype, self._stream())
+        x = op_input(self.op, self.rank, self.world)
+        # VC: 0 for the sum, which accumulates into it; the other ops must overwrite it whatever it holds
+        self.C.init3(va, vb, vc, self.n, x, x, float(self.world) if self.op == "max" else 0.0, self.dtype,
+                     self._stream())
 
     def run_once(self) -> None:
         """Enqueue one allreduce on the current stream (no host sync except for ring-nccl).
@@ -210,7 +264,7 @@ class AllreduceMiniapp:
                              pads.chunk_word(me, self.n_chunks) if self.slots_policy == 2 else 0,
                              pads.chunk_word(self.left, self.n_chunks) if self.slots_policy == 2 else 0,
                              self.pull, self.va.ptrs[self.left] if self.pull else 0,
-                             self.slots.ptrs[self.left] if self.pull else 0)
+                             self.slots.ptrs[self.left] if self.pull else 0, **self._op_kw)
             self.ring_epoch += P
             self.launches += 1
         elif self.algo == "ring-rsag":
@@ -219,7 +273,7 @@ class AllreduceMiniapp:
                         arrived_right=pads.chunk_word(self.right), rank=me, world=P, n=self.n,
                         chunk_elems=self.chunk_elems, epoch_base=self.ring_epoch, timeout_ns=pads.timeout_ns,
                         status=pads.status_ptr, dtype=self.dtype, ctas=self.ctas, device=self.device, stream=st,
-                        phases="allreduce")
+                        phases="allreduce", **self._op_kw)
             self.ring_epoch += C.rsag_epoch_advance(C.RSAG_ALLREDUCE, P)
             self.launches += 1
         elif self.algo == "twoshot":
@@ -227,7 +281,7 @@ class AllreduceMiniapp:
             ctas = C.allreduce_two_shot(self.va.ptrs, self.vc.ptrs, pads.buf.ptrs, pads.ticket_ptr,
                                         pads.ticket_issued & 0xFFFFFFFF, me, self.n, pads.barrier_epoch,
                                         pads.timeout_ns, pads.status_ptr, self.dtype, self.ctas,
-                                        self.device, st)
+                                        self.device, st, **self._op_kw)
             pads.advance_tickets(ctas)
             self.launches += 1
         elif self.algo == "nvls":
@@ -245,12 +299,15 @@ class AllreduceMiniapp:
             dst = tensor_from_ptr(vc, self.nbytes, self.device, _TORCH_DTYPE[self.dtype])
             dst.copy_(src)
             if P > 1:
-                dist.all_reduce(dst)
+                dist.all_reduce(dst, **({"op": _nccl_op(self.op)} if self.op != "sum" else {}))
         elif self.algo == "ring-unfused":
             cur, other = va, self.vb.local_ptr
             r_other = self.vb.ptrs[self.right]
             r_cur = self.va.ptrs[self.right]
-            C.accumulate(cur, vc, self.n, self.dtype, st)
+            if self.op == "sum":
+                C.accumulate(cur, vc, self.n, self.dtype, st)
+            else:                                       # the other ops overwrite VC: step 0 is VC = VA
+                C.memcpy_async(vc, cur, self.nbytes, st)
             for _ in range(1, P):
                 self.step_epoch += 1
                 ep = self.step_epoch
@@ -262,7 +319,7 @@ class AllreduceMiniapp:
                 C.wait(pads.word(me, C.PAD_DONE + self.left), ep, pads.timeout_ns, pads.status_ptr, st)
                 cur, other = other, cur
                 r_cur, r_other = r_other, r_cur
-                C.accumulate(cur, vc, self.n, self.dtype, st)
+                C.accumulate(cur, vc, self.n, self.dtype, st, **self._op_kw)
                 self.launches += 4
             self.launches += 1
         elif self.algo == "ring-nccl":
@@ -272,7 +329,13 @@ class AllreduceMiniapp:
             cur = tensor_from_ptr(va, self.nbytes, self.device, td)
             other = self.vb.tensor(td)
             acc = tensor_from_ptr(vc, self.nbytes, self.device, td)
-            acc.add_(cur)
+            combine = {"sum": lambda: acc.add_(cur), "prod": lambda: torch.mul(acc, cur, out=acc),
+                       "min": lambda: torch.minimum(acc, cur, out=acc),
+                       "max": lambda: torch.maximum(acc, cur, out=acc)}
+            if self.op == "sum":
+                acc.add_(cur)
+            else:
+                acc.copy_(cur)
             torch.cuda.synchronize(self.device)        # the reference's .wait()
             for _ in range(1, P):
                 ops = [dist.P2POp(dist.isend, cur, self.right), dist.P2POp(dist.irecv, other, self.left)]
@@ -280,13 +343,13 @@ class AllreduceMiniapp:
                     w.wait()
                 torch.cuda.synchronize(self.device)    # blocking MPI_Send/Recv semantics
                 cur, other = other, cur
-                acc.add_(cur)
+                combine[self.op]()
                 torch.cuda.synchronize(self.device)
 
     def mismatches(self) -> int:
         _, vc = self._ptrs()
         count = torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.device))
-        self.C.count_mismatch(vc, self.n, expected_value(self.world), self.dtype, count.data_ptr(),
+        self.C.count_mismatch(vc, self.n, expected_value(self.world, self.op), self.dtype, count.data_ptr(),
                               self._stream())
         torch.cuda.synchronize(self.device)
         return int(count.item())
@@ -314,7 +377,7 @@ class AllreduceMiniapp:
         bad = self.mismatches()
         total_bad = int(self.comm.sum(bad))
         print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong elements", flush=True)
-        return AllreduceResult(self.algo, self.dtype, self.world, self.n, best, total_bad, self.esz)
+        return AllreduceResult(self.algo, self.dtype, self.world, self.n, best, total_bad, self.esz, self.op)
 
     def close(self) -> None:
         torch.cuda.synchronize(self.device)
@@ -336,13 +399,15 @@ class VirtualAllreduce:
     MAX_WORLD = 8
 
     def __init__(self, world: int, n: int, dtype: str = "float", algo: str = "ring", slots: int = 0,
-                 pull: bool = False, ctas: int = 0, chunk_elems: int = 0, device: int = 0, timeout_s: float = 10.0):
+                 pull: bool = False, ctas: int = 0, chunk_elems: int = 0, device: int = 0, timeout_s: float = 10.0,
+                 op: str = "sum"):
         from ..parallel.local import LocalGroup
 
         if not 1 <= world <= self.MAX_WORLD:
             raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
         if algo not in VIRTUAL_ALGOS:
             raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        op = reduce_op(op)
         C = native()
         esz = C.elem_size(dtype)
         n = element_count(esz, world, n_elems=n)
@@ -360,14 +425,14 @@ class VirtualAllreduce:
         sl = self.group.symmetric(slot_bytes, zero=False) if algo in ("ring", "ring-rsag") else none
         self.ranks: List[AllreduceMiniapp] = [
             AllreduceMiniapp(self.group.comms[r], device, dtype=dtype, algo=algo, chunk_elems=chunk_elems,
-                             ctas=self.ctas, timeout_s=timeout_s, slots=slots, pull=pull, n_elems=n,
+                             ctas=self.ctas, timeout_s=timeout_s, slots=slots, pull=pull, n_elems=n, op=op,
                              _shared={"pads": pads[r], "va": va[r], "vb": vb[r], "vc": vc[r], "slots": sl[r]})
             for r in range(world)]
         self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, vas: List[torch.Tensor]) -> None:
-        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the rings accumulate into it;
-        ring-rsag overwrites it)."""
+        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the sum rings accumulate into
+        it; ring-rsag and every op other than the sum overwrite it)."""
         td = _TORCH_DTYPE[self.dtype]
         torch.cuda.synchronize(self.device)
         for app, v in zip(self.ranks, vas):
@@ -398,7 +463,7 @@ class VirtualAllreduce:
             app.close()
 
 
-def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int):
+def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int, op: str = "sum"):
     """Which one-launch collective the ``-a`` path (↔ MPI_Allreduce, allreduce-mpi-sycl.cpp:61-67) uses.
 
     Decided BEFORE anything is allocated and agreed across ranks (min over ranks of the local probe), so ranks can
@@ -406,8 +471,11 @@ def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int):
       * int:   two-shot — ``multimem.ld_reduce`` has no vector form for .s32 (one 4-byte request per thread), peer loads are 128-bit for every type;
       * bfloat16 / half: two-shot — its fp32 accumulation rounds once, where the rings round P-1 times (the NVLS
         kernel reduces fp32 and 32-bit integers only);
-      * float: NVLS (in-switch reduction) when every rank reports multicast support, else two-shot."""
+      * float: NVLS (in-switch reduction) when every rank reports multicast support, else two-shot;
+      * any op but the sum: two-shot (the NVLS kernel reduces sums only)."""
     C = native()
+    if reduce_op(op) != "sum":
+        return "twoshot", f"op={reduce_op(op)}: NVLS reduces sums only"
     if dtype in FLOAT16_TYPES:
         return "twoshot", "16-bit floats: two-shot sums in fp32 and rounds once"
     if dtype != "float":
@@ -435,21 +503,25 @@ def main(argv: Optional[List[str]] = None) -> int:
                          "default world-1 slots")
     ap.add_argument("--pull", action="store_true",
                     help="fused ring, receiver-driven: blocks are loaded from the left neighbour (peer loads)")
+    ap.add_argument("--op", default="sum", choices=OPS + tuple(_OP_ALIASES),
+                    help="reduction (default sum; nvls is sum-only, -a uses two-shot for the others)")
     args = ap.parse_args(argv)
+    op = reduce_op(args.op)
     comm = Comm()
     device = comm.device   # chosen before the process group was bound to it (Comm.pick_device)
     algo = args.algo
     app = None
     if args.a:
-        algo, why = choose_collective(comm, device, args.type, args.p)
+        algo, why = choose_collective(comm, device, args.type, args.p, op)
         if comm.rank == 0:
             print(f"# -a: {algo} ({why})", flush=True)
-    app = AllreduceMiniapp(comm, device, args.p, args.type, algo, slots=args.slots, pull=args.pull)
+    app = AllreduceMiniapp(comm, device, args.p, args.type, algo, slots=args.slots, pull=args.pull, op=op)
     res = app.run(args.iters, args.warmup)
     if comm.rank == 0:
         row = res.row()
         print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | {algo} {args.type} "
-              f"P={comm.world} N={res.elements} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank",
+              f"P={comm.world} N={res.elements}{'' if op == 'sum' else ' op=' + op} | "
+              f"{row['GBps_sent_per_rank']:.1f} GB/s sent per rank",
               flush=True)
         if args.json:
             with open(args.json, "a") as f:
