@@ -161,25 +161,20 @@ __device__ __forceinline__ void st_put(uint4* p, const uint4& v) {
 // rows it keeps in flight (`kChunk`), the stencil on it, and the two helpers of the step check.  Every field type computes one step per element as: widen the three
 // inputs exactly to the compute type (fp32, or fp64 for double), alpha*u + s*(up + dn) one rounded operation at a time,
 // never contracted, then round once to T (round-to-nearest-even, subnormals kept).  alpha and s are fp32 values.
-struct F32Vec {  // 4 lanes: the fp32 kernels' float4 code
-  using Raw = float4;
-  static constexpr int kChunk = kHaloChunk;
-  __device__ static __forceinline__ Raw stencil(const Raw& up, const Raw& ce, const Raw& dn, float alpha, float s) {
-    return stencil4(up, ce, dn, alpha, s);
-  }
-  __device__ static __forceinline__ Raw from_bits(const uint4& w) {
-    return make_float4(__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w));
-  }
-  __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
-    return (got.x != want.x) + (got.y != want.y) + (got.z != want.z) + (got.w != want.w);
-  }
-};
-
 __device__ __forceinline__ double stencil1(double up, double ce, double dn, float alpha, float s) {
   return __dadd_rn(__dmul_rn(static_cast<double>(alpha), ce), __dmul_rn(static_cast<double>(s), __dadd_rn(up, dn)));
 }
 
-// Element <-> compute type, and a 32-bit word <-> a pair of 16-bit elements (element 2i in the low half).
+// The rule of both halo checks: an element is wrong iff its bit pattern differs from the reference's, unless both are
+// NaN (of any sign or payload: the GPU's and the host's canonical NaNs differ).  So a wrong sign of zero or a flushed
+// subnormal is counted, and a NaN where a NaN is due is not.  `mag` clears the sign bit, `inf` is the infinity pattern.
+template <class B>
+__device__ __forceinline__ int bits_differ(B a, B b, B mag, B inf) {
+  return a != b && !((a & mag) > inf && (b & mag) > inf);
+}
+
+// Element <-> compute type, `differs` (the rule above), and a 32-bit word <-> a pair of 16-bit elements (element 2i
+// in the low half).
 template <class T>
 struct Elem;
 template <>
@@ -187,18 +182,31 @@ struct Elem<float> {
   using Compute = float;
   __device__ static __forceinline__ float widen(float x) { return x; }
   __device__ static __forceinline__ float narrow(float x) { return x; }
+  __device__ static __forceinline__ int differs(float a, float b) {
+    return bits_differ<uint32_t>(__float_as_uint(a), __float_as_uint(b), 0x7FFFFFFFu, 0x7F800000u);
+  }
 };
 template <>
 struct Elem<double> {
   using Compute = double;
   __device__ static __forceinline__ double widen(double x) { return x; }
   __device__ static __forceinline__ double narrow(double x) { return x; }
+  __device__ static __forceinline__ int differs(double a, double b) {
+    return bits_differ<uint64_t>(__double_as_longlong(a), __double_as_longlong(b), 0x7FFFFFFFFFFFFFFFull,
+                                 0x7FF0000000000000ull);
+  }
 };
 template <>
 struct Elem<__nv_bfloat16> {
   using Compute = float;
   __device__ static __forceinline__ float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
   __device__ static __forceinline__ __nv_bfloat16 narrow(float x) { return __float2bfloat16_rn(x); }
+  __device__ static __forceinline__ int differs(__nv_bfloat16 a, __nv_bfloat16 b) {
+    return bits_differ<uint16_t>(__bfloat16_as_ushort(a), __bfloat16_as_ushort(b), 0x7FFFu, 0x7F80u);
+  }
+  __device__ static __forceinline__ __nv_bfloat16 from_half_word(uint32_t w) {  // the low 16 bits of w
+    return __ushort_as_bfloat16(static_cast<unsigned short>(w));
+  }
   __device__ static __forceinline__ float2 widen2(uint32_t w) {  // bf16 is the high half of an fp32: one op per lane
     return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
   }
@@ -214,6 +222,12 @@ struct Elem<__half> {
   using Compute = float;
   __device__ static __forceinline__ float widen(__half x) { return __half2float(x); }
   __device__ static __forceinline__ __half narrow(float x) { return __float2half_rn(x); }
+  __device__ static __forceinline__ int differs(__half a, __half b) {
+    return bits_differ<uint16_t>(__half_as_ushort(a), __half_as_ushort(b), 0x7FFFu, 0x7C00u);
+  }
+  __device__ static __forceinline__ __half from_half_word(uint32_t w) {
+    return __ushort_as_half(static_cast<unsigned short>(w));
+  }
   __device__ static __forceinline__ float2 widen2(uint32_t w) {
     __half2 h;
     memcpy(&h, &w, 4);
@@ -224,6 +238,22 @@ struct Elem<__half> {
     uint32_t w;
     memcpy(&w, &h, 4);
     return w;
+  }
+};
+
+struct F32Vec {  // 4 lanes: the fp32 kernels' float4 code
+  using Raw = float4;
+  static constexpr int kChunk = kHaloChunk;
+  __device__ static __forceinline__ Raw stencil(const Raw& up, const Raw& ce, const Raw& dn, float alpha, float s) {
+    return stencil4(up, ce, dn, alpha, s);
+  }
+  __device__ static __forceinline__ Raw from_bits(const uint4& w) {
+    return make_float4(__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w));
+  }
+  __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
+    using E = Elem<float>;
+    return E::differs(got.x, want.x) + E::differs(got.y, want.y) + E::differs(got.z, want.z) +
+           E::differs(got.w, want.w);
   }
 };
 
@@ -241,7 +271,8 @@ struct F64Vec {  // 2 lanes, each a pair of 32-bit words
   }
   __device__ static __forceinline__ Raw from_bits(const uint4& w) { return w; }
   __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
-    return (lane(got.x, got.y) != lane(want.x, want.y)) + (lane(got.z, got.w) != lane(want.z, want.w));
+    return Elem<double>::differs(lane(got.x, got.y), lane(want.x, want.y)) +
+           Elem<double>::differs(lane(got.z, got.w), lane(want.z, want.w));
   }
 };
 
@@ -261,8 +292,9 @@ struct Pair16Vec {
   }
   __device__ static __forceinline__ Raw from_bits(const uint4& w) { return w; }
   __device__ static __forceinline__ int lanes_differ(uint32_t a, uint32_t b) {
-    const float2 x = Elem<T>::widen2(a), y = Elem<T>::widen2(b);
-    return (x.x != y.x) + (x.y != y.y);
+    using E = Elem<T>;
+    return E::differs(E::from_half_word(a), E::from_half_word(b)) +
+           E::differs(E::from_half_word(a >> 16), E::from_half_word(b >> 16));
   }
   __device__ static __forceinline__ int mismatches(const Raw& got, const Raw& want) {
     return lanes_differ(got.x, want.x) + lanes_differ(got.y, want.y) + lanes_differ(got.z, want.z) +
@@ -421,8 +453,8 @@ __global__ void halo_init_typed_kernel(T* __restrict__ u, T* __restrict__ halo_l
 
 // Independent check from the closed-form initial field: every thread owns one column of the GLOBAL
 // field (all world * rows rows), advances it `steps` times with the periodic stencil in the kernel's
-// operation order and compares this rank's rows exactly.  The column is kept in the compute type, rounded to T after
-// every step as the field is.
+// operation order and compares this rank's rows bit for bit (Elem<T>::differs).  The column is kept in the compute
+// type, rounded to T after every step as the field is, so narrowing it back to T is exact.
 constexpr int kHaloMaxGlobalRows = 128;
 template <class T>
 __device__ __forceinline__ void halo_verify_init_body(const T* __restrict__ u, int rows, size_t row_elems, int rank,
@@ -446,7 +478,7 @@ __device__ __forceinline__ void halo_verify_init_body(const T* __restrict__ u, i
       }
     }
     for (int r = 0; r < rows; ++r)
-      bad += (Elem<T>::widen(__ldcg(u + static_cast<size_t>(r) * row_elems + j)) != v[rank * rows + r]);
+      bad += Elem<T>::differs(__ldcg(u + static_cast<size_t>(r) * row_elems + j), Elem<T>::narrow(v[rank * rows + r]));
   }
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatch_count, bad);

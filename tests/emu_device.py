@@ -23,6 +23,7 @@ from hpc_patterns_b200.models import peer2pear as peer2pear_mod
 from hpc_patterns_b200.models.halo import initial_field, reference_steps
 from hpc_patterns_b200.parallel import local as local_mod
 from hpc_patterns_b200.parallel import symmetric as symmetric_mod
+from tests.field_compare import count_far, count_wrong
 
 FLAG_WORDS = 8          # kHaloFlagWords (csrc/kernels/api.h): one 32-byte sector per CTA
 
@@ -145,7 +146,7 @@ class EmuNative:
         self._arr(vc, n, dtype)[:] += self._arr(va, n, dtype)
 
     def count_mismatch(self, v, n, expected, dtype, count, stream):
-        ctypes.c_int64.from_address(count).value += int((self._arr(v, n, dtype) != self._NP[dtype](expected)).sum())
+        ctypes.c_int64.from_address(count).value += count_far(self._arr(v, n, dtype), expected)
 
     def ring_allreduce(self, va, vc, slots_local, slots_right, arrived_local, arrived_right, world, n, chunk_elems,
                        epoch_base, timeout_ns, status, dtype, ctas, device, stream, slots_policy=0, ack_local=0,
@@ -239,7 +240,7 @@ class EmuNative:
     def halo_verify_from_init(self, u, rows, row_elems, rank, world, steps, alpha, s, mismatch, stream):
         want = reference_steps(initial_field(world, rows, row_elems), steps, alpha, s)[rank * rows:(rank + 1) * rows]
         got = _f32(u, rows * row_elems).view(rows, row_elems)
-        ctypes.c_int64.from_address(mismatch).value += int((got != want).sum())
+        ctypes.c_int64.from_address(mismatch).value += count_wrong(got, want)
 
     def halo_verify_step(self, u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch, stream):
         old = _f32(u_old, rows * row_elems).view(rows, row_elems)
@@ -247,7 +248,7 @@ class EmuNative:
         a, b = torch.tensor(alpha, dtype=torch.float32), torch.tensor(s, dtype=torch.float32)
         want = a * ext[1:-1] + b * (ext[:-2] + ext[2:])
         got = _f32(u_new, rows * row_elems).view(rows, row_elems)
-        ctypes.c_int64.from_address(mismatch).value += int((got != want).sum())
+        ctypes.c_int64.from_address(mismatch).value += count_wrong(got, want)
 
 
 class _Stream:

@@ -12,6 +12,7 @@ import torch
 
 from hpc_patterns_b200.models.halo import compute_dtype, initial_field, reference_steps
 from tests.emu_device import EmuNative, _u32
+from tests.field_compare import count_wrong
 
 TORCH = {"float": torch.float32, "double": torch.float64, "bfloat16": torch.bfloat16, "half": torch.float16}
 
@@ -103,7 +104,7 @@ class HaloDtypeEmu(EmuNative):
         dt = TORCH[kw["dtype"]]
         want = reference_steps(initial_field(world, rows, row_elems, dt), steps, alpha, s)[rank * rows:(rank + 1) * rows]
         got = typed_view(u, rows * row_elems, dt).view(rows, row_elems)
-        ctypes.c_int64.from_address(mismatch).value += int((got != want).sum())
+        ctypes.c_int64.from_address(mismatch).value += count_wrong(got, want)
 
     def halo_verify_step(self, u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch, stream, **kw):
         self.calls.append(("halo_verify_step", kw.get("dtype")))
@@ -113,5 +114,5 @@ class HaloDtypeEmu(EmuNative):
         old = typed_view(u_old, rows * row_elems, dt).view(rows, row_elems)
         want = step_rows(typed_view(up_row, row_elems, dt), old, typed_view(dn_row, row_elems, dt), alpha, s)
         got = typed_view(u_new, rows * row_elems, dt).view(rows, row_elems)
-        ctypes.c_int64.from_address(mismatch).value += int((got != want).sum())
+        ctypes.c_int64.from_address(mismatch).value += count_wrong(got, want)
 

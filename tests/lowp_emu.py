@@ -19,6 +19,7 @@ import torch
 
 import tests.emu_device as emu_device
 from tests.emu_device import EmuNative, SharedEmuNative, _u32
+from tests.field_compare import count_far
 from tests.rsag_emu import RsAgEmu
 
 TORCH16 = {"bfloat16": torch.bfloat16, "half": torch.float16}
@@ -44,7 +45,7 @@ class Float16Emu(RsAgEmu):
     def count_mismatch(self, v, n, expected, dtype, count, stream):
         if dtype not in TORCH16:
             return super().count_mismatch(v, n, expected, dtype, count, stream)
-        ctypes.c_int64.from_address(count).value += int((self._arr(v, n, dtype) != float(expected)).sum())
+        ctypes.c_int64.from_address(count).value += count_far(self._arr(v, n, dtype).double().numpy(), expected)
 
     def ring_allreduce(self, va, vc, slots_local, slots_right, arrived_local, arrived_right, world, n, chunk_elems,
                        epoch_base, timeout_ns, status, dtype, ctas, device, stream, slots_policy=0, ack_local=0,
