@@ -73,8 +73,8 @@ struct DevCommand {
       t.b = b;
       t.c = c;
       t.s = 3.0f;
-      t.n = n & ~static_cast<size_t>(3);
-      launch_triad_put(t, CopyEngine::kLdSt, CopyTuning{}, SyncOps{}, nullptr, 0, device, s);
+      t.n = n & ~static_cast<size_t>(3);  // the triad covers whole 16-byte vectors; fewer than 4 elements is no work
+      if (t.n != 0) launch_triad_put(t, CopyEngine::kLdSt, CopyTuning{}, SyncOps{}, nullptr, 0, device, s);
     } else {
       HPCP_CUDA(cudaMemcpyAsync(dst, src, bytes(), cudaMemcpyDefault, s));
     }

@@ -178,6 +178,16 @@ void launch_busy_wait(float* out, size_t n_items, size_t tripcount, cudaStream_t
 int launch_fused_bench(const FusedCommand* cmds, int n_cmds, CopyEngine engine,
                        const CopyTuning& tune, int device, cudaStream_t stream) {
   HPCP_REQUIRE(n_cmds >= 1 && n_cmds <= kFusedMaxCommands, "fused bench: 1..8 commands per group");
+  // Copies and triads move 16-byte vectors (cp.async.bulk, LDG/STG.128); refuse before any CUDA call.
+  for (int k = 0; k < n_cmds; ++k) {
+    if (cmds[k].kind == FusedKind::kCopy)
+      HPCP_REQUIRE(((reinterpret_cast<uintptr_t>(cmds[k].dst) | reinterpret_cast<uintptr_t>(cmds[k].src)) & 15) == 0,
+                   "fused bench: copy pointers must be 16-byte aligned");
+    if (cmds[k].kind == FusedKind::kTriad)
+      HPCP_REQUIRE(((reinterpret_cast<uintptr_t>(cmds[k].a) | reinterpret_cast<uintptr_t>(cmds[k].b) |
+                     reinterpret_cast<uintptr_t>(cmds[k].c)) & 15) == 0,
+                   "fused bench: triad pointers must be 16-byte aligned");
+  }
   const int sms = device_sm_count(device);
   const int threads = 512;
 
@@ -224,10 +234,6 @@ int launch_fused_bench(const FusedCommand* cmds, int n_cmds, CopyEngine engine,
     s.b = cmds[k].b;
     s.c = cmds[k].c;
     s.s = cmds[k].s;
-    if (cmds[k].kind == FusedKind::kCopy)
-      HPCP_REQUIRE((reinterpret_cast<uintptr_t>(s.dst) & 15) == 0 &&
-                       (reinterpret_cast<uintptr_t>(s.src) & 15) == 0,
-                   "fused bench: copy pointers must be 16-byte aligned");
   }
 
   const uint32_t stage_bytes = static_cast<uint32_t>((tune.stage_kb > 0 ? tune.stage_kb : 16) * 1024);

@@ -26,6 +26,7 @@
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
+#include "payload.h"
 
 namespace hpcp {
 
@@ -273,19 +274,14 @@ __global__ void __launch_bounds__(kTmaThreads)
 }
 
 // ---------------------------------------------------- inputs and checking ----
-__device__ __forceinline__ float triad_b(size_t i, int rank) {
-  return static_cast<float>((i + 17u * static_cast<unsigned>(rank)) & 1023u);
-}
-__device__ __forceinline__ float triad_c(size_t i, int rank) {
-  return static_cast<float>((i * 3u + static_cast<unsigned>(rank)) & 7u);
-}
-
+// b and c of rank r at element i (payload.h): integers in [0, 1023] and [0, 7] drawn from one hash of (i, r).
 __global__ void fill_triad_kernel(float* __restrict__ b, float* __restrict__ c, size_t n,
                                   int rank) {
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
-    b[i] = triad_b(i, rank);
-    c[i] = triad_c(i, rank);
+    const uint32_t w = triad_word(i, rank);
+    b[i] = static_cast<float>(triad_b_bits(w));
+    c[i] = static_cast<float>(triad_c_bits(w));
   }
 }
 
@@ -294,7 +290,8 @@ __global__ void verify_triad_kernel(const float* __restrict__ a, size_t n, int s
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   unsigned long long bad = 0;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float want = fmaf(s, triad_c(i, src_rank), triad_b(i, src_rank));
+    const uint32_t w = triad_word(i, src_rank);
+    const float want = fmaf(s, static_cast<float>(triad_c_bits(w)), static_cast<float>(triad_b_bits(w)));
     bad += (__ldcg(a + i) != want);
   }
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
@@ -306,20 +303,25 @@ __global__ void verify_triad_kernel(const float* __restrict__ a, size_t n, int s
 int launch_triad_put(const TriadPutArgs& args, CopyEngine engine, const CopyTuning& tune,
                      const SyncOps& sync, const uint32_t* arrive_flag, uint32_t arrive_epoch,
                      int device, cudaStream_t stream) {
+  HPCP_REQUIRE(args.n > 0, "triad_put: n must be positive (an empty triad launches nothing)");
   HPCP_REQUIRE(args.n % 4 == 0, "triad_put: n must be a multiple of 4 elements");
+  // Every engine moves 16-byte vectors (LDG/STG.128 or cp.async.bulk); a_peer only matters when there is a put.
+  HPCP_REQUIRE(((reinterpret_cast<uintptr_t>(args.a_local) | reinterpret_cast<uintptr_t>(args.a_peer) |
+                 reinterpret_cast<uintptr_t>(args.b) | reinterpret_cast<uintptr_t>(args.c)) & 15) == 0,
+               "triad_put: pointers must be 16-byte aligned");
   const size_t n_put = args.n_put == 0 ? args.n : args.n_put;
   HPCP_REQUIRE(n_put <= args.n && args.n % n_put == 0, "triad_put: n must be a multiple of n_put");
   const int ratio = static_cast<int>(args.n / n_put);
   HPCP_REQUIRE(sync.signal_flag == nullptr || sync.ticket != nullptr,
                "triad_put: a signal needs a ticket counter");
-  const int sms = device_sm_count(device);
+  // Every refusal comes before the first CUDA call (device_sm_count), so a bad call never reaches the device.
   const size_t nvec = args.n / 4;
   const bool put = args.a_peer != nullptr;
   int ctas = 0;
   if (engine == CopyEngine::kLdSt && ratio > 1) {
     HPCP_REQUIRE((n_put / 4) % kHaloTileVec == 0, "triad_put: halo (n_put) must be a multiple of 16 KiB");
     const size_t tiles = (n_put / 4 / kHaloTileVec) * static_cast<size_t>(ratio);
-    const int cap = tune.ctas > 0 ? tune.ctas : sms * 2;
+    const int cap = tune.ctas > 0 ? tune.ctas : device_sm_count(device) * 2;
     ctas = static_cast<int>(std::min<size_t>(tiles, static_cast<size_t>(cap)));
     uint4* al = reinterpret_cast<uint4*>(args.a_local);
     uint4* ap = reinterpret_cast<uint4*>(args.a_peer);
@@ -336,7 +338,7 @@ int launch_triad_put(const TriadPutArgs& args, CopyEngine engine, const CopyTuni
     const int unroll = tune.unroll > 0 ? tune.unroll : 2;
     const size_t per_cta = static_cast<size_t>(threads) * unroll * (tune.vec_bytes == 32 ? 2 : 1);
     const size_t want = std::max<size_t>(1, (nvec + per_cta - 1) / per_cta);
-    const int cap = tune.ctas > 0 ? tune.ctas : sms * 2;
+    const int cap = tune.ctas > 0 ? tune.ctas : device_sm_count(device) * 2;
     ctas = static_cast<int>(std::min<size_t>(want, static_cast<size_t>(cap)));
     const bool wide = tune.vec_bytes == 32 && args.n % 8 == 0 &&
                       ((reinterpret_cast<uintptr_t>(args.a_local) | reinterpret_cast<uintptr_t>(args.a_peer) |
@@ -380,7 +382,7 @@ int launch_triad_put(const TriadPutArgs& args, CopyEngine engine, const CopyTuni
                  "triad_put: halo (n_put) must be a multiple of the TMA tile size");
     const size_t tiles = std::max<size_t>(1, (n_bytes + tile_bytes - 1) / tile_bytes);
     const int per_sm = std::max(1, static_cast<int>((227 * 1024) / smem));
-    const int cap = tune.ctas > 0 ? tune.ctas : sms * per_sm;
+    const int cap = tune.ctas > 0 ? tune.ctas : device_sm_count(device) * per_sm;
     ctas = static_cast<int>(std::min<size_t>(tiles, static_cast<size_t>(cap)));
     if (tune.l2_hint != 0) {  // experimental variant with L2 cache-policy operands
       if (put) {

@@ -20,22 +20,11 @@
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
+#include "payload.h"
 
 namespace hpcp {
 
 namespace {
-
-__host__ __device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16;
-  x *= 0x7feb352du;
-  x ^= x >> 15;
-  x *= 0x846ca68bu;
-  x ^= x >> 16;
-  return x;
-}
-__host__ __device__ __forceinline__ uint32_t pattern_word(size_t i, uint32_t seed) {
-  return mix32(static_cast<uint32_t>(i) * 2654435761u ^ seed);
-}
 
 // Prologue shared by the data movers: one thread waits for the epoch, the CTA
 // learns the outcome through smem.

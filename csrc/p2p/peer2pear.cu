@@ -37,6 +37,7 @@
 #include "../common/rank_runtime.h"
 #include "../common/signal_layout.h"
 #include "../kernels/api.h"
+#include "../kernels/payload.h"
 #include "topology_core.hpp"
 
 namespace {
@@ -344,17 +345,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
 // Same pairing, phases, iteration/min logic, bandwidth formulas, payload and exact verification, with
 // host buffers and memcpy standing in for the NVLink transports: the program logic can be exercised on a
 // machine without a GPU.
-uint32_t host_mix32(uint32_t x) {
-  x ^= x >> 16;
-  x *= 0x7feb352du;
-  x ^= x >> 15;
-  x *= 0x846ca68bu;
-  x ^= x >> 16;
-  return x;
-}
-uint32_t host_pattern_word(size_t i, uint32_t seed) {
-  return host_mix32(static_cast<uint32_t>(i) * 2654435761u ^ seed);
-}
+uint32_t host_pattern_word(size_t i, uint32_t seed) { return pattern_word(i, seed); }
 
 int run_on_host(const Config& cfg) {
   const int P = cfg.ranks > 0 ? cfg.ranks : 2;

@@ -26,9 +26,15 @@ def triad_reference(b: torch.Tensor, c: torch.Tensor, s: float) -> torch.Tensor:
     return b.float() + float(s) * c.float()
 
 
+TRIAD_SEED = 0x7A1AD000   # kTriadSeed, csrc/kernels/payload.h
+
+
 def triad_inputs_reference(n: int, rank: int):
-    """CPU reference of fill_triad_inputs: b[i]=(i+17r)&1023, c[i]=(3i+r)&7."""
-    i = torch.arange(n, dtype=torch.int64)
-    b = ((i + 17 * rank) & 1023).float()
-    c = ((i * 3 + rank) & 7).float()
+    """CPU reference of fill_triad_inputs: w = pattern word i of seed TRIAD_SEED + rank, b[i] = w & 1023,
+    c[i] = (w >> 10) & 7.  No period below 2^32 elements, so a misplaced tile changes almost every value."""
+    from .p2p import pattern_reference
+
+    w = pattern_reference(n, (TRIAD_SEED + rank) & 0xFFFFFFFF)
+    b = (w & 1023).float()
+    c = ((w >> 10) & 7).float()
     return b, c

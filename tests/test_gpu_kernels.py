@@ -110,32 +110,6 @@ def test_fill_and_verify_pattern(native, dev):
     assert int(counters[0]) == 1
 
 
-@pytest.mark.parametrize("engine,tune", [("ldst", {}), ("ldst", {"unroll": 4}), ("ldst", {"unroll": 1}),
-                                         ("ldst", {"vec_bytes": 32}), ("ldst", {"vec_bytes": 32, "blocked": 1}),
-                                         ("ldst", {"blocked": 1, "ctas": 37}),
-                                         ("tma", {}), ("tma", {"stages": 3, "stage_kb": 8})])
-@pytest.mark.parametrize("n", [4096, (1 << 22) + 8, 12345 * 4])
-def test_triad_put_matches_fp32_reference(native, dev, engine, tune, n):
-    from hpc_patterns_b200.ops.fused import triad_reference
-
-    b = torch.randn(n, device=dev)
-    c = torch.randn(n, device=dev)
-    a_local = torch.zeros(n, device=dev)
-    a_peer = torch.zeros(n, device=dev)  # loop-back "peer"
-    native.triad_put(a_local.data_ptr(), a_peer.data_ptr(), b.data_ptr(), c.data_ptr(), 2.5, n, engine, tune, {},
-                     0, 0, 0, _stream())
-    torch.cuda.synchronize()
-    ref = torch.addcmul(b, c, torch.tensor(2.5, device=dev))  # fused multiply-add order differs by <= 1 ulp
-    assert torch.allclose(a_local, triad_reference(b, c, 2.5), rtol=1e-6, atol=1e-6)
-    assert torch.equal(a_local, a_peer)
-    assert torch.allclose(a_local, ref, rtol=1e-6, atol=1e-6)
-    # plain triad (no put)
-    a2 = torch.zeros(n, device=dev)
-    native.triad_put(a2.data_ptr(), 0, b.data_ptr(), c.data_ptr(), 2.5, n, engine, tune, {}, 0, 0, 0, _stream())
-    torch.cuda.synchronize()
-    assert torch.equal(a2, a_local)
-
-
 def test_fill_triad_inputs_and_verify(native, dev):
     from hpc_patterns_b200.ops.fused import triad_inputs_reference
 
@@ -155,25 +129,6 @@ def test_fill_triad_inputs_and_verify(native, dev):
     native.verify_triad(a.data_ptr(), n, 3, 3.0, cnt.data_ptr(), _stream())
     torch.cuda.synchronize()
     assert int(cnt) == 1
-
-
-@pytest.mark.parametrize("engine", ["ldst", "tma"])
-@pytest.mark.parametrize("ratio", [2, 3, 4])
-def test_triad_put_halo_mode(native, dev, engine, ratio):
-    """Triad over ratio x the halo; only the halo reaches the (loop-back) peer buffer."""
-    n_put = (3 * 16384) // 4 * 8          # 24 tiles of 16 KiB
-    n = n_put * ratio
-    b = torch.randn(n, device=dev)
-    c = torch.randn(n, device=dev)
-    a = torch.zeros(n, device=dev)
-    peer = torch.full((n_put + 1024,), -7.0, device=dev)
-    native.triad_put(a.data_ptr(), peer.data_ptr(), b.data_ptr(), c.data_ptr(), 2.0, n, engine, {}, {}, 0, 0, 0,
-                     _stream(), n_put)
-    torch.cuda.synchronize()
-    ref = torch.addcmul(b, c, torch.tensor(2.0, device=dev))
-    assert torch.allclose(a, ref, rtol=1e-6, atol=1e-6)
-    assert torch.equal(peer[:n_put], a[:n_put])
-    assert bool((peer[n_put:] == -7.0).all())      # nothing but the halo was put
 
 
 @pytest.mark.parametrize("ratio", [1, 3])
@@ -200,27 +155,6 @@ def test_busy_wait_semantics(native, dev):
     torch.cuda.synchronize()
     assert float(out[0]) == 0.0          # y=0 stays 0 through the FMA chain
     assert bool(torch.isinf(out[1:]).all())  # everything else overflows to +inf
-
-
-def test_fused_bench_commands(native, dev):
-    n = (2 << 20) + 4
-    src = torch.randn(n, device=dev)
-    dst = torch.zeros(n, device=dev)
-    b = torch.randn(n, device=dev)
-    c = torch.randn(n, device=dev)
-    a = torch.zeros(n, device=dev)
-    out = torch.full((64,), -1.0, device=dev)
-    for engine in ("tma", "ldst"):
-        dst.zero_(); a.zero_(); out.fill_(-1)
-        cmds = [{"kind": "busy", "n": 64, "tripcount": 50, "a": out.data_ptr()},
-                {"kind": "copy", "n": n, "dst": dst.data_ptr(), "src": src.data_ptr()},
-                {"kind": "triad", "n": n, "a": a.data_ptr(), "b": b.data_ptr(), "c": c.data_ptr(), "s": 3.0}]
-        ctas = native.fused_bench(cmds, engine, {}, 0, _stream())
-        torch.cuda.synchronize()
-        assert ctas >= 3
-        assert torch.equal(dst, src)
-        assert torch.allclose(a, b + 3.0 * c, rtol=1e-6, atol=1e-6)
-        assert float(out[0]) == 0.0 and bool(torch.isinf(out[1:]).all())
 
 
 def test_fused_bench_pinned_host_copy(native, dev):
@@ -440,35 +374,3 @@ def test_gemm_put_cta_pairs_exact(native, dev, m, n, k):
     gemm_put(a, b, c_bf, 0, out_dtype=torch.bfloat16, cluster=2, ctas=6)   # several tiles per pair
     torch.cuda.synchronize()
     assert torch.equal(c_bf, ref.to(torch.bfloat16))
-
-
-@pytest.mark.parametrize("ratio", [1, 3])
-def test_triad_put_tma_l2_hint(native, dev, ratio):
-    """L2 evict_first cache-policy operands on the TMA engine's streamed copies (round-1 flagship): same values."""
-    n_put = (64 * 16384) // 4
-    n = n_put * ratio
-    b = torch.randn(n, device=dev)
-    c = torch.randn(n, device=dev)
-    a = torch.zeros(n, device=dev)
-    peer = torch.full((n_put + 64,), -7.0, device=dev)
-    native.triad_put(a.data_ptr(), peer.data_ptr(), b.data_ptr(), c.data_ptr(), 2.0, n, "tma",
-                     {"l2_hint": 1}, {}, 0, 0, 0, _stream(), n_put)
-    torch.cuda.synchronize()
-    assert torch.allclose(a, torch.addcmul(b, c, torch.tensor(2.0, device=dev)), rtol=1e-6, atol=1e-6)
-    assert torch.equal(peer[:n_put], a[:n_put]) and bool((peer[n_put:] == -7.0).all())
-
-
-@pytest.mark.parametrize("halo_ctas", [8, 48, 147])
-def test_triad_put_halo_split_scheduling(native, dev, halo_ctas):
-    """Dedicated halo CTAs instead of interleaved halo/interior tiles (TMA engine, round-1 flagship): same values."""
-    n_put = (64 * 16384) // 4
-    n = n_put * 3
-    b = torch.randn(n, device=dev)
-    c = torch.randn(n, device=dev)
-    a = torch.zeros(n, device=dev)
-    peer = torch.full((n_put + 64,), -7.0, device=dev)
-    native.triad_put(a.data_ptr(), peer.data_ptr(), b.data_ptr(), c.data_ptr(), 2.0, n, "tma",
-                     {"halo_ctas": halo_ctas}, {}, 0, 0, 0, _stream(), n_put)
-    torch.cuda.synchronize()
-    assert torch.allclose(a, torch.addcmul(b, c, torch.tensor(2.0, device=dev)), rtol=1e-6, atol=1e-6)
-    assert torch.equal(peer[:n_put], a[:n_put]) and bool((peer[n_put:] == -7.0).all())

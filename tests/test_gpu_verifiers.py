@@ -289,6 +289,16 @@ def test_verify_triad_counts_exactly(native, src_rank):
     assert run(want + 0.5) == n
     other = triad_inputs_reference(n, src_rank + 1)[0]      # another rank's data
     assert run(other) == int((other != want).sum())
+    # Displacement: a block moved by its own size (a tile at its neighbour's offset) and a stale stage of the default
+    # TMA ring (6 stages of 16 KiB: tile j holds tile j - 6).  The count must match the host AND cover the moved
+    # elements: a payload that repeats every 4 KiB would give 0 on both sides.
+    for name, (shift, lo, size) in {"4 KiB block": (1024, 8192, 1024), "16 KiB block": (4096, 16384, 4096),
+                                    "64 KiB block": (16384, 65536, 16384),
+                                    "stale stage": (6 * 4096, 18 * 4096, 4096)}.items():
+        got = want.clone()
+        got[lo:lo + size] = want[lo - shift:lo - shift + size]
+        host = int((got != want).sum())
+        assert run(got) == host >= 0.99 * size, (name, host)
 
 
 @pytest.mark.parametrize("n_words", [1, 17, 31, 4097, 3 * 135168 + 3])
