@@ -22,6 +22,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <string>
+#include <type_traits>
 
 #include "../kernels/api.h"
 
@@ -113,6 +114,41 @@ inline const char* elem_type_name(ElemType t) {
   }
   return "?";
 }
+
+// Run f(T{}) with the C++ type of `t`.
+template <typename F>
+void dispatch_elem(ElemType t, F&& f) {
+  switch (t) {
+    case ElemType::kFloat: f(float{}); break;
+    case ElemType::kInt: f(int{}); break;
+    case ElemType::kUInt: f(static_cast<unsigned int>(0)); break;
+    case ElemType::kDouble: f(double{}); break;
+    case ElemType::kLong: f(static_cast<long long>(0)); break;
+    case ElemType::kULong: f(static_cast<unsigned long long>(0)); break;
+    case ElemType::kShort: f(static_cast<short>(0)); break;
+    case ElemType::kUShort: f(static_cast<unsigned short>(0)); break;
+    case ElemType::kUChar: f(static_cast<unsigned char>(0)); break;
+    case ElemType::kBFloat16: f(__nv_bfloat16{}); break;
+    case ElemType::kHalf: f(__half{}); break;
+  }
+}
+
+// C++ element type -> the addition class its sum kernels are instantiated for: signed and unsigned integers of one
+// width share the add (and the wrapping product).
+template <typename T> struct AddClass { using type = T; };
+template <> struct AddClass<unsigned int> { using type = int; };
+template <> struct AddClass<unsigned long long> { using type = long long; };
+template <> struct AddClass<unsigned short> { using type = short; };
+
+// Run f(C{}) with the addition class of `t` (eight kernel instantiations instead of eleven).
+template <typename F>
+void dispatch_add_class(ElemType t, F&& f) {
+  dispatch_elem(t, [&](auto tag) { f(typename AddClass<decltype(tag)>::type{}); });
+}
+
+// The 16-bit floating types: two-shot accumulates them in fp32 and rounds once.
+template <typename T>
+constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
 
 // Reduction by name: sum, prod (or product), min, max; false if unknown.
 inline bool reduce_op_from_name(const std::string& name, ReduceOp* out) {

@@ -1,4 +1,7 @@
-// Allreduce miniapp kernels (float and int).
+// Allreduce miniapp: the launchers of every algorithm, the sum's instantiations of the kernel templates of
+// ring_allreduce.cuh (prod, min and max are instantiated in ring_allreduce_ops.cu), the NVLS kernel and the small
+// init / accumulate / verify kernels.  A launcher validates, fills the device argument block, takes the kernel of
+// (type, op) from allreduce_kernels() and launches it: the sum goes the same way as every other op.
 //
 // Reference pattern (aurora.mpich.miniapps/src/allreduce/mpi-sycl/allreduce-mpi-sycl.cpp:173-182):
 //     Accumulate(VA,VC).wait();
@@ -73,35 +76,6 @@ __global__ void count_mismatch_kernel(const T* __restrict__ v, size_t n, double 
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(count, bad);
 }
 
-// ------------------------------------------------------------- sum kernels ----
-// The kernel bodies live in ring_allreduce.cuh, templated on the combine policy; these are their sum instantiations.
-template <typename T, bool kAck = false>
-__global__ void __launch_bounds__(512) ring_allreduce_kernel(const __grid_constant__ RingDev a) {
-  ring_push_body<SumOp<T>, kAck, false>(a);
-}
-
-template <typename T, bool kTwoSlots>
-__global__ void __launch_bounds__(512) ring_pull_kernel(const __grid_constant__ RingPullDev a) {
-  ring_pull_body<SumOp<T>, kTwoSlots, false>(a);
-}
-
-template <typename T>
-__global__ void __launch_bounds__(512) ring_rsag_kernel(const __grid_constant__ RingRsAgDev a) {
-  ring_rsag_body<SumOp<T>>(a);
-}
-
-// The tail loop adds rank 0 first, unlike the main blocks (owner first).
-template <typename T, int W, int U>
-__global__ void __launch_bounds__(512) two_shot_kernel(const __grid_constant__ TwoShotDev a) {
-  two_shot_body<SumOp<T>, W, U, false>(a);
-}
-
-// The 16-bit floating types: fp32 sums, owner first everywhere, rounded once.
-template <typename T, int W, int U>
-__global__ void __launch_bounds__(512) two_shot_f32_kernel(const __grid_constant__ TwoShotDev a) {
-  two_shot_f32_body<Sum8<T>, W, U>(a);
-}
-
 // -------------------------------------------------------------------- NVLS ----
 struct NvlsDev {
   const unsigned char* va_mc;
@@ -159,6 +133,35 @@ int env_choice(const char* name, std::initializer_list<int> allowed, int fallbac
   return fallback;
 }
 
+// The kernels of (type, op): the sum's are instantiated here, the other ops' in ring_allreduce_ops.cu.
+AllreduceKernels allreduce_kernels(ElemType type, ReduceOp op) {
+  if (op != ReduceOp::kSum) return op_allreduce_kernels(type, op);
+  AllreduceKernels k{};
+  dispatch_add_class(type, [&](auto tag) { k = allreduce_kernels_of<SumOp<decltype(tag)>, false, false>(); });
+  return k;
+}
+
+// The fields RingDev and RingPullDev share.
+template <class Dev>
+Dev ring_dev(const RingArgs& args, size_t esz, size_t ce) {
+  const size_t lanes = 16 / esz;
+  Dev d{};
+  d.va = static_cast<const uint4*>(args.va);
+  d.vc = static_cast<uint4*>(args.vc);
+  d.arrived_local = args.arrived_local;
+  d.arrived_right = args.arrived_right;
+  d.ack_local = args.ack_local;
+  d.ack_left = args.ack_left;
+  d.world = args.world;
+  d.nvec = args.n / lanes;
+  d.chunk_vec = ce / lanes;
+  d.n_chunks = ring_num_chunks(args.n, ce, esz);
+  d.epoch_base = args.epoch_base;
+  d.timeout_ns = args.timeout_ns;
+  d.status = args.status;
+  return d;
+}
+
 }  // namespace
 
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
@@ -176,14 +179,14 @@ void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaSt
   const size_t lanes = 16 / elem_size(type);
   const size_t nvec = n / lanes, tail = n % lanes;
   const int ctas = grid_for(std::max<size_t>(nvec, 1), 512, 132 * 4);
+  // The sum keeps accumulate_kernel, whose scalar tail is typed: it is the timed step of ring-unfused, and running it
+  // as combine_kernel<SumOp> would change that arm's instructions.
   if (op != ReduceOp::kSum) {
     const uint4* va_v = static_cast<const uint4*>(va);
     uint4* vc_v = static_cast<uint4*>(vc);
     const unsigned char* va_tail = static_cast<const unsigned char*>(va) + nvec * 16;
     unsigned char* vc_tail = static_cast<unsigned char*>(vc) + nvec * 16;
-    size_t nvec_arg = nvec, tail_bytes = tail * elem_size(type);
-    void* params[] = {&va_v, &vc_v, &nvec_arg, &va_tail, &vc_tail, &tail_bytes};
-    HPCP_CUDA(cudaLaunchKernel(select_combine_op(type, op), ctas, 512, params, 0, stream));
+    launch_512(op_combine_kernel(type, op), ctas, stream, va_v, vc_v, nvec, va_tail, vc_tail, tail * elem_size(type));
     return;
   }
   dispatch_elem(type, [&](auto tag) {
@@ -217,93 +220,30 @@ void launch_ring_allreduce(const RingArgs& args, ElemType type, int ctas, int de
   HPCP_REQUIRE(args.n % lanes == 0, "ring: the block must be a multiple of 16 bytes");
   const size_t ce = args.chunk_elems == 0 ? kRingDefaultChunkBytes / esz : args.chunk_elems;
   HPCP_REQUIRE(ce % lanes == 0, "ring: a chunk must be a multiple of 16 bytes");
-  RingDev d{};
-  d.va = static_cast<const uint4*>(args.va);
-  d.vc = static_cast<uint4*>(args.vc);
-  d.slots_local = static_cast<const uint4*>(args.slots_local);
-  d.slots_right = static_cast<uint4*>(args.slots_right);
-  d.arrived_local = args.arrived_local;
-  d.arrived_right = args.arrived_right;
-  d.world = args.world;
-  d.nvec = args.n / lanes;
-  d.chunk_vec = ce / lanes;
-  d.n_chunks = ring_num_chunks(args.n, ce, esz);
-  d.epoch_base = args.epoch_base;
-  d.timeout_ns = args.timeout_ns;
-  d.status = args.status;
   const bool ack = args.n_slots == 2 && args.world > 3 && !args.pull;  // with P <= 3 no slot is ever written twice
   HPCP_REQUIRE(args.n_slots == 0 || args.n_slots == 2 || args.n_slots == args.world - 1,
                "ring: n_slots must be 0 (= world-1, no flow control) or 2 (double buffer + acks)");
   HPCP_REQUIRE(!ack || (args.ack_local != nullptr && args.ack_left != nullptr), "ring: n_slots=2 needs the ack words");
-  d.ack_local = args.ack_local;
-  d.ack_left = args.ack_left;
   HPCP_REQUIRE(!args.pull || args.world == 1 ||
                    (args.va_left != nullptr && (args.world == 2 || args.slots_left != nullptr)),
                "ring: the pull variant needs the left neighbour's VA and slots (peer-mapped)");
   HPCP_REQUIRE(!args.pull || args.n_slots != 2 || args.world <= 4 ||
                    (args.ack_local != nullptr && args.ack_left != nullptr),
                "ring: pull with n_slots=2 needs the ack words");
-  const bool two_slots_k = args.n_slots == 2;
-  const bool op = args.op != ReduceOp::kSum;
-  const void* kernel = op ? select_ring_op(type, args.op, args.pull, two_slots_k) : nullptr;
-  if (!op)
-    dispatch_add_class(type, [&](auto tag) {
-      using C = decltype(tag);
-      if (args.pull)
-        kernel = two_slots_k ? reinterpret_cast<const void*>(ring_pull_kernel<C, true>)
-                             : reinterpret_cast<const void*>(ring_pull_kernel<C, false>);
-      else
-        kernel = two_slots_k ? reinterpret_cast<const void*>(ring_allreduce_kernel<C, true>)
-                             : reinterpret_cast<const void*>(ring_allreduce_kernel<C, false>);
-    });
-  const int grid = ring_grid(kernel, d.n_chunks, ctas, device);
   const bool two_slots = args.n_slots == 2;  // slot index t % 2 even when no ack is ever needed (P <= 3)
+  const void* kernel = allreduce_kernels(type, args.op).ring[args.pull][two_slots];
   if (args.pull) {
-    RingPullDev p{};
-    p.va = d.va;
-    p.vc = d.vc;
-    p.va_left = static_cast<const uint4*>(args.va_left);
-    p.slots_left = static_cast<const uint4*>(args.slots_left);
-    p.slots_local = static_cast<uint4*>(args.slots_local);
-    p.arrived_local = d.arrived_local;
-    p.arrived_right = d.arrived_right;
-    p.ack_local = args.ack_local;
-    p.ack_left = args.ack_left;
-    p.world = d.world;
-    p.nvec = d.nvec;
-    p.chunk_vec = d.chunk_vec;
-    p.n_chunks = d.n_chunks;
-    p.epoch_base = d.epoch_base;
-    p.timeout_ns = d.timeout_ns;
-    p.status = d.status;
-    if (op) {
-      void* params[] = {&p};
-      HPCP_CUDA(cudaLaunchKernel(kernel, grid, 512, params, 0, stream));
-      return;
-    }
-    dispatch_add_class(type, [&](auto tag) {
-      using C = decltype(tag);
-      if (two_slots)
-        ring_pull_kernel<C, true><<<grid, 512, 0, stream>>>(p);
-      else
-        ring_pull_kernel<C, false><<<grid, 512, 0, stream>>>(p);
-    });
-    HPCP_CUDA(cudaGetLastError());
-    return;
+    RingPullDev d = ring_dev<RingPullDev>(args, esz, ce);
+    d.va_left = static_cast<const uint4*>(args.va_left);
+    d.slots_left = static_cast<const uint4*>(args.slots_left);
+    d.slots_local = static_cast<uint4*>(args.slots_local);
+    launch_512(kernel, ring_grid(kernel, d.n_chunks, ctas, device), stream, d);
+  } else {
+    RingDev d = ring_dev<RingDev>(args, esz, ce);
+    d.slots_local = static_cast<const uint4*>(args.slots_local);
+    d.slots_right = static_cast<uint4*>(args.slots_right);
+    launch_512(kernel, ring_grid(kernel, d.n_chunks, ctas, device), stream, d);
   }
-  if (op) {
-    void* params[] = {&d};
-    HPCP_CUDA(cudaLaunchKernel(kernel, grid, 512, params, 0, stream));
-    return;
-  }
-  dispatch_add_class(type, [&](auto tag) {
-    using C = decltype(tag);
-    if (two_slots)
-      ring_allreduce_kernel<C, true><<<grid, 512, 0, stream>>>(d);
-    else
-      ring_allreduce_kernel<C, false><<<grid, 512, 0, stream>>>(d);
-  });
-  HPCP_CUDA(cudaGetLastError());
 }
 
 void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int device, cudaStream_t stream) {
@@ -337,18 +277,8 @@ void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int dev
   d.timeout_ns = args.timeout_ns;
   d.status = args.status;
   // The all-gather phase only copies: every op shares the sum's kernel there.
-  if (args.op != ReduceOp::kSum && args.phases != kRsAgAllGather) {
-    const void* kernel = select_rsag_op(type, args.op);
-    void* params[] = {&d};
-    HPCP_CUDA(cudaLaunchKernel(kernel, ring_grid(kernel, d.n_chunks, ctas, device), 512, params, 0, stream));
-    return;
-  }
-  dispatch_add_class(type, [&](auto tag) {
-    using C = decltype(tag);
-    const int grid = ring_grid(reinterpret_cast<const void*>(ring_rsag_kernel<C>), d.n_chunks, ctas, device);
-    ring_rsag_kernel<C><<<grid, 512, 0, stream>>>(d);
-  });
-  HPCP_CUDA(cudaGetLastError());
+  const void* kernel = allreduce_kernels(type, args.phases == kRsAgAllGather ? ReduceOp::kSum : args.op).rsag;
+  launch_512(kernel, ring_grid(kernel, d.n_chunks, ctas, device), stream, d);
 }
 
 int launch_allreduce_two_shot(const TwoShotArgs& args, ElemType type, int ctas, int device,
@@ -373,32 +303,7 @@ int launch_allreduce_two_shot(const TwoShotArgs& args, ElemType type, int ctas, 
   const int sms = device_sm_count(device);
   const int grid = grid_for(std::max<size_t>(d.slice_vec, 1), 512, ctas > 0 ? ctas : sms * 2);
   d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
-  if (args.op != ReduceOp::kSum) {
-    const int w = args.world <= 2 ? 2 : args.world <= 4 ? 4 : args.world <= 8 ? 8 : 16;  // <W, U> as below
-    void* params[] = {&d};
-    HPCP_CUDA(cudaLaunchKernel(select_two_shot_op(type, args.op, w), grid, 512, params, 0, stream));
-    return grid;
-  }
-#define HPCP_TWO_SHOT(W, U)                                              \
-  do {                                                                     \
-    dispatch_add_class(type, [&](auto tag) {                               \
-      using C = decltype(tag);                                             \
-      if constexpr (kSum16InF32<C>)                                        \
-        two_shot_f32_kernel<C, W, U><<<grid, 512, 0, stream>>>(d);         \
-      else                                                                 \
-        two_shot_kernel<C, W, U><<<grid, 512, 0, stream>>>(d);             \
-    });                                                                    \
-  } while (0)
-  if (args.world <= 2)
-    HPCP_TWO_SHOT(2, 4);
-  else if (args.world <= 4)
-    HPCP_TWO_SHOT(4, 4);
-  else if (args.world <= 8)
-    HPCP_TWO_SHOT(8, 2);
-  else
-    HPCP_TWO_SHOT(16, 1);
-#undef HPCP_TWO_SHOT
-  HPCP_CUDA(cudaGetLastError());
+  launch_512(allreduce_kernels(type, args.op).two_shot[two_shot_shape(args.world)], grid, stream, d);
   return grid;
 }
 
@@ -425,25 +330,16 @@ int launch_allreduce_nvls(const NvlsArgs& args, ElemType type, int ctas, int dev
   // HPCP_NVLS_UNROLL=4|8 (vectors in flight per thread; default 4), HPCP_NVLS_CTAS_PER_SM=k or --ctas / ctas>0 (grid).
   static const int unroll = env_choice("HPCP_NVLS_UNROLL", {4, 8}, 4);
   static const int per_sm = env_choice("HPCP_NVLS_CTAS_PER_SM", {0, 1, 2, 3, 4}, 0);
-  constexpr int threads = 512;
   const int sms = device_sm_count(device);
   // Default grid: 32 CTAs.  The in-switch reduction saturates at modest request parallelism and more requesters only
   // queue in the switch.  HPCP_NVLS_CTAS_PER_SM / --ctas override.
-  const int grid = grid_for(std::max<size_t>(d.slice_vec, 1), threads, ctas > 0 ? ctas : per_sm > 0 ? sms * per_sm : 32);
+  const int grid = grid_for(std::max<size_t>(d.slice_vec, 1), 512, ctas > 0 ? ctas : per_sm > 0 ? sms * per_sm : 32);
   d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
-#define HPCP_NVLS(U)                                                  \
-  do {                                                                \
-    if (type == ElemType::kFloat)                                     \
-      nvls_kernel<float, U, threads><<<grid, threads, 0, stream>>>(d); \
-    else                                                              \
-      nvls_kernel<int, U, threads><<<grid, threads, 0, stream>>>(d);   \
-  } while (0)
-  if (unroll == 8)
-    HPCP_NVLS(8);
-  else
-    HPCP_NVLS(4);
-#undef HPCP_NVLS
-  HPCP_CUDA(cudaGetLastError());
+  const bool f32 = type == ElemType::kFloat;
+  const void* kernel =
+      unroll == 8 ? (f32 ? kernel_ptr(nvls_kernel<float, 8, 512>) : kernel_ptr(nvls_kernel<int, 8, 512>))
+                  : (f32 ? kernel_ptr(nvls_kernel<float, 4, 512>) : kernel_ptr(nvls_kernel<int, 4, 512>));
+  launch_512(kernel, grid, stream, d);
   return grid;
 }
 

@@ -1,8 +1,10 @@
-// Pieces shared by the allreduce kernels of ring_allreduce.cu (sum) and ring_allreduce_ops.cu (prod, min, max): the
-// 16-byte lane policies, the element-type dispatch, the device argument blocks, and the kernel bodies as __forceinline__
-// templates on a COMBINE POLICY -- a type with `static uint4 combine(const uint4& acc, const uint4& x)` that reduces
-// every lane of one 16-byte vector.  The sum kernels instantiate the bodies with SumOp<T> (their instructions do not
-// depend on the op machinery); the op kernels overwrite VC at hop 0 instead of accumulating into it (kOverwrite).
+// The allreduce kernels of ring_allreduce.cu (sum) and ring_allreduce_ops.cu (prod, min, max): the 16-byte lane
+// policies, the device argument blocks, the kernel bodies, one __global__ template per kernel family and the table of
+// kernel pointers the launchers pick from.  Everything is a template on a COMBINE POLICY -- a type with
+// `static uint4 combine(const uint4& acc, const uint4& x)` that reduces every lane of one 16-byte vector.  The sum is
+// the policy SumOp<C>; it differs from the others in two template arguments only: its rings accumulate into VC where
+// the others overwrite it at hop 0 (kOverwrite), and its two-shot tail combines rank 0 first (kOwnerFirstTail).
+// The argument blocks' layouts are part of the fingerprinted instruction streams (docs/sass/VALIDATED.sha256).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -10,8 +12,10 @@
 
 #include <algorithm>
 #include <type_traits>
+#include <utility>
 
 #include "../common/cuda_check.h"
+#include "../common/dtype_traits.h"
 #include "../common/signal.cuh"
 #include "api.h"
 #include "ring_order.h"
@@ -94,10 +98,6 @@ struct SumOp {
   static __device__ __forceinline__ uint4 combine(const uint4& acc, const uint4& x) { return Vec4<T>::add(acc, x); }
 };
 
-// 16-bit floating types: two-shot accumulates them in fp32 and rounds once (two_shot_f32_kernel).
-template <typename T>
-constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
-
 // The eight lanes of a 16-byte vector of T (bf16 or fp16) as fp32 partials: set / combine widen exactly, round()
 // rounds every lane once to nearest even in T (F2FP.*.F32.PACK_AB).  F is the fp32 operation (IEEE, no FTZ).
 template <typename T>
@@ -148,35 +148,6 @@ struct Wide8 {
 template <typename T>
 using Sum8 = Wide8<T, AddF32>;
 
-// C++ element type -> the addition class its kernels are instantiated for.
-template <typename T> struct AddClass { using type = T; };
-template <> struct AddClass<unsigned int> { using type = int; };
-template <> struct AddClass<unsigned long long> { using type = long long; };
-template <> struct AddClass<unsigned short> { using type = short; };
-
-// Run f(T{}) with the C++ type of `t`.
-template <typename F>
-void dispatch_elem(ElemType t, F&& f) {
-  switch (t) {
-    case ElemType::kFloat: f(float{}); break;
-    case ElemType::kInt: f(int{}); break;
-    case ElemType::kUInt: f(static_cast<unsigned int>(0)); break;
-    case ElemType::kDouble: f(double{}); break;
-    case ElemType::kLong: f(static_cast<long long>(0)); break;
-    case ElemType::kULong: f(static_cast<unsigned long long>(0)); break;
-    case ElemType::kShort: f(static_cast<short>(0)); break;
-    case ElemType::kUShort: f(static_cast<unsigned short>(0)); break;
-    case ElemType::kUChar: f(static_cast<unsigned char>(0)); break;
-    case ElemType::kBFloat16: f(__nv_bfloat16{}); break;
-    case ElemType::kHalf: f(__half{}); break;
-  }
-}
-// Run f(C{}) with the addition class of `t` (eight kernel instantiations instead of eleven).
-template <typename F>
-void dispatch_add_class(ElemType t, F&& f) {
-  dispatch_elem(t, [&](auto tag) { f(typename AddClass<decltype(tag)>::type{}); });
-}
-
 // ------------------------------------------------------------------ K-ring ----
 struct RingDev {
   const uint4* va;
@@ -192,14 +163,14 @@ struct RingDev {
   uint32_t epoch_base;
   uint64_t timeout_ns;
   uint32_t* status;
-  // kAck only (appended so that the layout the default instantiation reads is unchanged):
+  // kAck only:
   uint32_t* ack_local;  // n_chunks words written by the right neighbour: "hop t of chunk c consumed"
   uint32_t* ack_left;   // peer-mapped: the left neighbour's ack words
 };
 
 // kAck = false: P-1 receive slots, hop t lands in slot t-1.  kAck = true: two slots, hop t lands in slot
 // (t-1) % 2 and the sender waits for the receiver's ack of hop t-1 before it overwrites the slot at hop t+1.
-// kOverwrite: hop 0 stores VA into VC without reading VC (the op kernels); otherwise VC accumulates every hop.
+// kOverwrite: hop 0 stores VA into VC without reading VC (every op but the sum); otherwise VC accumulates every hop.
 template <class Op, bool kAck, bool kOverwrite>
 __device__ __forceinline__ void ring_push_body(const RingDev& a) {
   __shared__ int ok_s;
@@ -252,6 +223,11 @@ __device__ __forceinline__ void ring_push_body(const RingDev& a) {
         publish_epoch_light(a.ack_left + c, a.epoch_base + t);
     }
   }
+}
+
+template <class Op, bool kAck, bool kOverwrite>
+__global__ void __launch_bounds__(512) ring_push_kernel(const __grid_constant__ RingDev a) {
+  ring_push_body<Op, kAck, kOverwrite>(a);
 }
 
 // ------------------------------------------------------------ K-ring, pull variant ----
@@ -334,6 +310,11 @@ __device__ __forceinline__ void ring_pull_body(const RingPullDev& a) {
   }
 }
 
+template <class Op, bool kTwoSlots, bool kOverwrite>
+__global__ void __launch_bounds__(512) ring_pull_kernel(const __grid_constant__ RingPullDev a) {
+  ring_pull_body<Op, kTwoSlots, kOverwrite>(a);
+}
+
 // ------------------------------------------------- K-ring, reduce-scatter + all-gather ----
 // Bandwidth-optimal ring: segment s (nvec / P vectors) of the block is reduced hop by hop on its way to rank s, then
 // the finished segments travel once more round the ring.  Per (hop, chunk) a CTA waits on arrival word c, reads the
@@ -414,6 +395,11 @@ __device__ __forceinline__ void ring_rsag_body(const RingRsAgDev& a) {
   }
 }
 
+template <class Op>
+__global__ void __launch_bounds__(512) ring_rsag_kernel(const __grid_constant__ RingRsAgDev a) {
+  ring_rsag_body<Op>(a);
+}
+
 // ---------------------------------------------------------------- two-shot ----
 struct TwoShotDev {
   const uint4* va[kApiMaxRanks];
@@ -454,6 +440,8 @@ __device__ __forceinline__ void grid_then_node_barrier(uint32_t* ticket, uint32_
 // W = compile-time bound on the world size (register arrays), U = vectors per thread per trip:
 // up to U*W independent NVLink loads in flight per thread.  The main blocks combine owner first,
 // ((VA[s] o VA[s+1]) o ...); the tail loop does too with kOwnerFirstTail, else it goes rank 0 first.
+// kOwnerFirstTail is false for the sum only.  Its tail adding rank 0 first, unlike its main blocks, is part of the
+// sum's results (a floating sum's last bits depend on the order) and of its fingerprinted instructions.
 template <class Op, int W, int U, bool kOwnerFirstTail>
 __device__ __forceinline__ void two_shot_body(const TwoShotDev& a) {
   const size_t base = static_cast<size_t>(a.rank) * a.slice_vec;
@@ -498,6 +486,11 @@ __device__ __forceinline__ void two_shot_body(const TwoShotDev& a) {
   }
   grid_then_node_barrier(a.ticket, a.ticket_target, a.pads, a.rank, a.world, a.barrier_epoch,
                          a.timeout_ns, a.status);
+}
+
+template <class Op, int W, int U, bool kOwnerFirstTail>
+__global__ void __launch_bounds__(512) two_shot_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_body<Op, W, U, kOwnerFirstTail>(a);
 }
 
 // Two-shot for the 16-bit floating types: same loads, stores and barrier as two_shot_body, but every lane is widened
@@ -548,6 +541,20 @@ __device__ __forceinline__ void two_shot_f32_body(const TwoShotDev& a) {
                          a.timeout_ns, a.status);
 }
 
+template <class Acc, int W, int U>
+__global__ void __launch_bounds__(512) two_shot_f32_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_f32_body<Acc, W, U>(a);
+}
+
+// The combine policies two-shot runs through two_shot_f32_kernel, and the accumulator (a Wide8) each one uses: the sum
+// of the 16-bit floating types here, their product in ring_allreduce_ops.cu.
+template <class Op>
+struct TwoShotInF32 : std::false_type {};
+template <typename T>
+struct TwoShotInF32<SumOp<T>> : std::integral_constant<bool, kSum16InF32<T>> {
+  using acc = Sum8<T>;
+};
+
 // ------------------------------------------------------------------- grids ----
 inline int grid_for(size_t items, int threads, int cap) {
   const size_t want = (items + threads - 1) / threads;
@@ -590,16 +597,68 @@ constexpr size_t kRingDefaultChunkBytes = 128 * 1024;  // payload per arrival wo
 
 }  // namespace
 
-// The prod / min / max kernels (ring_allreduce_ops.cu) for the launchers of ring_allreduce.cu, which set up the same
-// argument blocks as for the sum and launch these with cudaLaunchKernel.  `op` is never kSum.  Kernel parameters:
-//   select_ring_op       RingDev (push) or RingPullDev (pull)
-//   select_rsag_op       RingRsAgDev
-//   select_two_shot_op   TwoShotDev; w = 2, 4, 8 or 16 is W (U = 4, 4, 2, 1 as for the sum)
-//   select_combine_op    (const uint4* va, uint4* vc, size_t nvec, const unsigned char* va_tail,
-//                         unsigned char* vc_tail, size_t tail_bytes): VC = op(VC, VA)
-const void* select_ring_op(ElemType type, ReduceOp op, bool pull, bool two_slots);
-const void* select_rsag_op(ElemType type, ReduceOp op);
-const void* select_two_shot_op(ElemType type, ReduceOp op, int w);
-const void* select_combine_op(ElemType type, ReduceOp op);
+// --------------------------------------------------------- kernel selection ----
+// Two-shot's <W, U> by world size: the first row with world <= W runs (the last one takes the rest).
+struct TwoShotShape {
+  int w, u;
+};
+constexpr TwoShotShape kTwoShotShapes[] = {{2, 4}, {4, 4}, {8, 2}, {16, 1}};
+constexpr int kTwoShotShapeCount = sizeof(kTwoShotShapes) / sizeof(kTwoShotShapes[0]);
+inline int two_shot_shape(int world) {
+  int i = 0;
+  while (i + 1 < kTwoShotShapeCount && world > kTwoShotShapes[i].w) ++i;
+  return i;
+}
+
+// The kernels of one (element type, op), every one launched with 512 threads and its family's argument block.
+struct AllreduceKernels {
+  const void* ring[2][2];                    // [pull][two slots]: RingDev (push) or RingPullDev (pull)
+  const void* rsag;                          // RingRsAgDev
+  const void* two_shot[kTwoShotShapeCount];  // [two_shot_shape(world)]: TwoShotDev
+};
+
+namespace {
+
+template <class K>
+const void* kernel_ptr(K* kernel) {
+  return reinterpret_cast<const void*>(kernel);
+}
+
+template <class Op, bool kOwnerFirstTail, int I>
+const void* two_shot_kernel_of() {
+  constexpr int W = kTwoShotShapes[I].w, U = kTwoShotShapes[I].u;
+  if constexpr (TwoShotInF32<Op>::value)
+    return kernel_ptr(two_shot_f32_kernel<typename TwoShotInF32<Op>::acc, W, U>);
+  else
+    return kernel_ptr(two_shot_kernel<Op, W, U, kOwnerFirstTail>);
+}
+
+template <class Op, bool kOverwrite, bool kOwnerFirstTail, int... I>
+AllreduceKernels allreduce_kernels_of(std::integer_sequence<int, I...>) {
+  return {{{kernel_ptr(ring_push_kernel<Op, false, kOverwrite>), kernel_ptr(ring_push_kernel<Op, true, kOverwrite>)},
+           {kernel_ptr(ring_pull_kernel<Op, false, kOverwrite>), kernel_ptr(ring_pull_kernel<Op, true, kOverwrite>)}},
+          kernel_ptr(ring_rsag_kernel<Op>),
+          {two_shot_kernel_of<Op, kOwnerFirstTail, I>()...}};
+}
+// Every kernel of the combine policy Op.
+template <class Op, bool kOverwrite, bool kOwnerFirstTail>
+AllreduceKernels allreduce_kernels_of() {
+  return allreduce_kernels_of<Op, kOverwrite, kOwnerFirstTail>(std::make_integer_sequence<int, kTwoShotShapeCount>{});
+}
+
+// One launch of 512 threads per CTA; `args` are the kernel's parameters, with exactly their types.
+template <class... Args>
+void launch_512(const void* kernel, int grid, cudaStream_t stream, Args... args) {
+  void* params[] = {&args...};
+  HPCP_CUDA(cudaLaunchKernel(kernel, dim3(grid), dim3(512), params, 0, stream));
+}
+
+}  // namespace
+
+// The prod / min / max kernels (ring_allreduce_ops.cu) for the launchers of ring_allreduce.cu; `op` is not kSum.
+AllreduceKernels op_allreduce_kernels(ElemType type, ReduceOp op);
+// VC = op(VC, VA), parameters (const uint4* va, uint4* vc, size_t nvec, const unsigned char* va_tail,
+// unsigned char* vc_tail, size_t tail_bytes).
+const void* op_combine_kernel(ElemType type, ReduceOp op);
 
 }  // namespace hpcp

@@ -1,7 +1,7 @@
 // Allreduce kernels for the reductions other than the sum: prod, min and max (↔ MPI_PROD / MPI_MIN / MPI_MAX).
 //
-// The bodies are the sum kernels' (ring_allreduce.cuh): the same loads, stores, arrival / ack words and barriers, in
-// the same combine order, with a different combine policy.  Two differences on purpose:
+// They are the kernel templates of ring_allreduce.cuh, the ones the sum runs, instantiated with another combine policy:
+// the same loads, stores, arrival / ack words and barriers, in the same combine order.  Two differences on purpose:
 //   * the rings OVERWRITE VC (hop 0 stores VA[r] without reading VC), as MPI_Allreduce does; the sum accumulates;
 //   * two-shot combines owner first, ((VA[s] o VA[s+1]) o ...), in its tail loop too, so every element has one order.
 // Semantics per type (docs/allreduce.md):
@@ -199,36 +199,10 @@ struct Prod8 : Wide8<T, MulF32Raw> {
                       canonical_nan16x2<inf>(r.w));
   }
 };
-template <class Op> struct TwoShotInF32 : std::false_type {};
 template <> struct TwoShotInF32<Prod<__nv_bfloat16>> : std::true_type { using acc = Prod8<__nv_bfloat16>; };
 template <> struct TwoShotInF32<Prod<__half>> : std::true_type { using acc = Prod8<__half>; };
 
 // ---------------------------------------------------------------- kernels ----
-template <class Op, bool kAck>
-__global__ void __launch_bounds__(512) ring_push_op_kernel(const __grid_constant__ RingDev a) {
-  ring_push_body<Op, kAck, true>(a);
-}
-
-template <class Op, bool kTwoSlots>
-__global__ void __launch_bounds__(512) ring_pull_op_kernel(const __grid_constant__ RingPullDev a) {
-  ring_pull_body<Op, kTwoSlots, true>(a);
-}
-
-template <class Op>
-__global__ void __launch_bounds__(512) ring_rsag_op_kernel(const __grid_constant__ RingRsAgDev a) {
-  ring_rsag_body<Op>(a);
-}
-
-template <class Op, int W, int U>
-__global__ void __launch_bounds__(512) two_shot_op_kernel(const __grid_constant__ TwoShotDev a) {
-  two_shot_body<Op, W, U, true>(a);
-}
-
-template <class Acc, int W, int U>
-__global__ void __launch_bounds__(512) two_shot_f32_op_kernel(const __grid_constant__ TwoShotDev a) {
-  two_shot_f32_body<Acc, W, U>(a);
-}
-
 // VC = op(VC, VA) over whole vectors; block 0's thread 0 combines the last partial vector in registers and writes back
 // only its tail_bytes.
 template <class Op>
@@ -263,54 +237,17 @@ void dispatch_op(ElemType type, ReduceOp op, F&& f) {
   });
 }
 
-template <int W, int U>
-const void* two_shot_op_for(ElemType type, ReduceOp op) {
-  const void* k = nullptr;
-  dispatch_op(type, op, [&](auto tag) {
-    using Op = decltype(tag);
-    if constexpr (TwoShotInF32<Op>::value)
-      k = reinterpret_cast<const void*>(two_shot_f32_op_kernel<typename TwoShotInF32<Op>::acc, W, U>);
-    else
-      k = reinterpret_cast<const void*>(two_shot_op_kernel<Op, W, U>);
-  });
-  return k;
-}
-
 }  // namespace
 
-const void* select_ring_op(ElemType type, ReduceOp op, bool pull, bool two_slots) {
-  const void* k = nullptr;
-  dispatch_op(type, op, [&](auto tag) {
-    using Op = decltype(tag);
-    if (pull)
-      k = two_slots ? reinterpret_cast<const void*>(ring_pull_op_kernel<Op, true>)
-                    : reinterpret_cast<const void*>(ring_pull_op_kernel<Op, false>);
-    else
-      k = two_slots ? reinterpret_cast<const void*>(ring_push_op_kernel<Op, true>)
-                    : reinterpret_cast<const void*>(ring_push_op_kernel<Op, false>);
-  });
+AllreduceKernels op_allreduce_kernels(ElemType type, ReduceOp op) {
+  AllreduceKernels k{};
+  dispatch_op(type, op, [&](auto tag) { k = allreduce_kernels_of<decltype(tag), true, true>(); });
   return k;
 }
 
-const void* select_rsag_op(ElemType type, ReduceOp op) {
+const void* op_combine_kernel(ElemType type, ReduceOp op) {
   const void* k = nullptr;
-  dispatch_op(type, op, [&](auto tag) { k = reinterpret_cast<const void*>(ring_rsag_op_kernel<decltype(tag)>); });
-  return k;
-}
-
-// <W, U> as the sum's two-shot: 2/4, 4/4, 8/2, 16/1.
-const void* select_two_shot_op(ElemType type, ReduceOp op, int w) {
-  switch (w) {
-    case 2: return two_shot_op_for<2, 4>(type, op);
-    case 4: return two_shot_op_for<4, 4>(type, op);
-    case 8: return two_shot_op_for<8, 2>(type, op);
-    default: return two_shot_op_for<16, 1>(type, op);
-  }
-}
-
-const void* select_combine_op(ElemType type, ReduceOp op) {
-  const void* k = nullptr;
-  dispatch_op(type, op, [&](auto tag) { k = reinterpret_cast<const void*>(combine_kernel<decltype(tag)>); });
+  dispatch_op(type, op, [&](auto tag) { k = kernel_ptr(combine_kernel<decltype(tag)>); });
   return k;
 }
 

@@ -147,8 +147,6 @@ __nv_bfloat16 host_add(__nv_bfloat16 a, __nv_bfloat16 b) {
 }
 __half host_add(__half a, __half b) { return __float2half_rn(__half2float(a) + __half2float(b)); }
 template <typename T>
-constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
-template <typename T>
 T host_from_float(float x) {
   return static_cast<T>(x);
 }
@@ -223,20 +221,9 @@ std::string op_json(ReduceOp op) {
 }
 
 double first_element_as_double(const void* p, ElemType t) {
-  switch (t) {
-    case ElemType::kBFloat16: return host_to_double(*static_cast<const __nv_bfloat16*>(p));
-    case ElemType::kHalf: return host_to_double(*static_cast<const __half*>(p));
-    case ElemType::kFloat: return *static_cast<const float*>(p);
-    case ElemType::kInt: return *static_cast<const int*>(p);
-    case ElemType::kUInt: return *static_cast<const unsigned int*>(p);
-    case ElemType::kDouble: return *static_cast<const double*>(p);
-    case ElemType::kLong: return static_cast<double>(*static_cast<const long long*>(p));
-    case ElemType::kULong: return static_cast<double>(*static_cast<const unsigned long long*>(p));
-    case ElemType::kShort: return *static_cast<const short*>(p);
-    case ElemType::kUShort: return *static_cast<const unsigned short*>(p);
-    case ElemType::kUChar: return *static_cast<const unsigned char*>(p);
-  }
-  return 0;
+  double x = 0;
+  dispatch_elem(t, [&](auto tag) { x = host_to_double(*static_cast<const decltype(tag)*>(p)); });
+  return x;
 }
 
 template <typename T>
@@ -250,20 +237,9 @@ unsigned long long count_mismatch_typed(const void* p, size_t n, double expected
   return bad;
 }
 unsigned long long count_mismatch_on_host(const void* p, size_t n, double expected, ElemType t) {
-  switch (t) {
-    case ElemType::kBFloat16: return count_mismatch_typed<__nv_bfloat16>(p, n, expected);
-    case ElemType::kHalf: return count_mismatch_typed<__half>(p, n, expected);
-    case ElemType::kFloat: return count_mismatch_typed<float>(p, n, expected);
-    case ElemType::kInt: return count_mismatch_typed<int>(p, n, expected);
-    case ElemType::kUInt: return count_mismatch_typed<unsigned int>(p, n, expected);
-    case ElemType::kDouble: return count_mismatch_typed<double>(p, n, expected);
-    case ElemType::kLong: return count_mismatch_typed<long long>(p, n, expected);
-    case ElemType::kULong: return count_mismatch_typed<unsigned long long>(p, n, expected);
-    case ElemType::kShort: return count_mismatch_typed<short>(p, n, expected);
-    case ElemType::kUShort: return count_mismatch_typed<unsigned short>(p, n, expected);
-    case ElemType::kUChar: return count_mismatch_typed<unsigned char>(p, n, expected);
-  }
-  return n;
+  unsigned long long bad = n;
+  dispatch_elem(t, [&](auto tag) { bad = count_mismatch_typed<decltype(tag)>(p, n, expected); });
+  return bad;
 }
 
 uint32_t* pad_of(const Shared& sh, int r) { return static_cast<uint32_t*>(sh.pads.ptr[r]); }
@@ -617,20 +593,9 @@ int run_on_host_typed(const Config& cfg) {
 }
 
 int run_on_host(const Config& cfg) {
-  switch (cfg.type) {
-    case ElemType::kFloat: return run_on_host_typed<float>(cfg);
-    case ElemType::kInt: return run_on_host_typed<int>(cfg);
-    case ElemType::kUInt: return run_on_host_typed<unsigned int>(cfg);
-    case ElemType::kDouble: return run_on_host_typed<double>(cfg);
-    case ElemType::kLong: return run_on_host_typed<long long>(cfg);
-    case ElemType::kULong: return run_on_host_typed<unsigned long long>(cfg);
-    case ElemType::kShort: return run_on_host_typed<short>(cfg);
-    case ElemType::kUShort: return run_on_host_typed<unsigned short>(cfg);
-    case ElemType::kUChar: return run_on_host_typed<unsigned char>(cfg);
-    case ElemType::kBFloat16: return run_on_host_typed<__nv_bfloat16>(cfg);
-    case ElemType::kHalf: return run_on_host_typed<__half>(cfg);
-  }
-  return 1;
+  int rc = 1;
+  dispatch_elem(cfg.type, [&](auto tag) { rc = run_on_host_typed<decltype(tag)>(cfg); });
+  return rc;
 }
 }  // namespace
 

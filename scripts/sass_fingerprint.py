@@ -28,10 +28,8 @@ MANIFEST = os.path.join(ROOT, "docs", "sass", "VALIDATED.sha256")
 # at most the rank counts below on one device)
 UNVALIDATED = (
     # more than 8 ranks: needs > 8 GPUs (ranks sharing one GPU's hardware queue serialise their spinning kernels)
-    r"two_shot_kernel<[\w ]+, 16, 1>",
-    r"two_shot_f32_kernel<[\w ]+, 16, 1>",   # the 16-bit floating types' two-shot, same rank bound
-    r"two_shot_op_kernel<[\w<> ]+, 16, 1>",       # prod / min / max two-shot, same rank bound
-    r"two_shot_f32_op_kernel<[\w<> ]+, 16, 1>",   # the 16-bit prod two-shot (fp32 products), same rank bound
+    r"two_shot_kernel<[\w<> ]+, 16, 1, \w+>",   # every op and type
+    r"two_shot_f32_kernel<[\w<>, ]+, 16, 1>",   # the 16-bit floating types' fp32 sums and products, same rank bound
 )
 
 
