@@ -50,16 +50,14 @@
 
 #include <algorithm>
 #include <cstring>
+#include <map>
 #include <mutex>
-#include <string>
-#include <type_traits>
-
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
+#include <utility>
 
 #include "../common/cuda_check.h"
 #include "../common/signal.cuh"
 #include "halo_columns.h"
+#include "halo_field.h"
 
 namespace hpcp {
 
@@ -173,34 +171,25 @@ __device__ __forceinline__ int bits_differ(B a, B b, B mag, B inf) {
   return a != b && !((a & mag) > inf && (b & mag) > inf);
 }
 
-// Element <-> compute type, `differs` (the rule above), and a 32-bit word <-> a pair of 16-bit elements (element 2i
-// in the low half).
+// Element <-> compute type (FieldElem, halo_field.h), `differs` (the rule above), and a 32-bit word <-> a pair of
+// 16-bit elements (element 2i in the low half).
 template <class T>
 struct Elem;
 template <>
-struct Elem<float> {
-  using Compute = float;
-  __device__ static __forceinline__ float widen(float x) { return x; }
-  __device__ static __forceinline__ float narrow(float x) { return x; }
+struct Elem<float> : FieldElem<float> {
   __device__ static __forceinline__ int differs(float a, float b) {
     return bits_differ<uint32_t>(__float_as_uint(a), __float_as_uint(b), 0x7FFFFFFFu, 0x7F800000u);
   }
 };
 template <>
-struct Elem<double> {
-  using Compute = double;
-  __device__ static __forceinline__ double widen(double x) { return x; }
-  __device__ static __forceinline__ double narrow(double x) { return x; }
+struct Elem<double> : FieldElem<double> {
   __device__ static __forceinline__ int differs(double a, double b) {
     return bits_differ<uint64_t>(__double_as_longlong(a), __double_as_longlong(b), 0x7FFFFFFFFFFFFFFFull,
                                  0x7FF0000000000000ull);
   }
 };
 template <>
-struct Elem<__nv_bfloat16> {
-  using Compute = float;
-  __device__ static __forceinline__ float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
-  __device__ static __forceinline__ __nv_bfloat16 narrow(float x) { return __float2bfloat16_rn(x); }
+struct Elem<__nv_bfloat16> : FieldElem<__nv_bfloat16> {
   __device__ static __forceinline__ int differs(__nv_bfloat16 a, __nv_bfloat16 b) {
     return bits_differ<uint16_t>(__bfloat16_as_ushort(a), __bfloat16_as_ushort(b), 0x7FFFu, 0x7F80u);
   }
@@ -218,10 +207,7 @@ struct Elem<__nv_bfloat16> {
   }
 };
 template <>
-struct Elem<__half> {
-  using Compute = float;
-  __device__ static __forceinline__ float widen(__half x) { return __half2float(x); }
-  __device__ static __forceinline__ __half narrow(float x) { return __float2half_rn(x); }
+struct Elem<__half> : FieldElem<__half> {
   __device__ static __forceinline__ int differs(__half a, __half b) {
     return bits_differ<uint16_t>(__half_as_ushort(a), __half_as_ushort(b), 0x7FFFu, 0x7C00u);
   }
@@ -364,9 +350,10 @@ __device__ __forceinline__ void halo_column(const HaloParams& p, int in, uint64_
   store(R - 1, V::stencil(cur, last, dn, alpha, s));
 }
 
-// The kernel body of every field type.  kMode: 0 none, 1 pull, 2 push.
-template <class V, int kMode>
-__device__ __forceinline__ void halo_body(const HaloParams& p) {
+// The stencil kernel of every field type: T = float, double, __nv_bfloat16, __half.  kMode: 0 none, 1 pull, 2 push.
+template <class T, int kMode>
+__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_kernel(const HaloParams p) {
+  using V = typename VecOf<T>::type;
   __shared__ int abort_w;
   const uint32_t ntiles = static_cast<uint32_t>(halo_cta_tiles(p.cols, blockIdx.x));  // < 2^32 float4 per row
   if (ntiles == 0) return;  // same geometry on every rank: nobody waits for this CTA index
@@ -409,29 +396,11 @@ __device__ __forceinline__ void halo_body(const HaloParams& p) {
   }
 }
 
-// The fp32 kernels (their SASS is fingerprinted in docs/sass/VALIDATED.sha256) ...
-template <int kMode>
-__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_kernel(const HaloParams p) {
-  halo_body<F32Vec, kMode>(p);
-}
-// ... and the other field types: T = double, __nv_bfloat16, __half.
-template <class T, int kMode>
-__global__ void __launch_bounds__(kHaloThreads, kHaloCtasPerSm) halo_stencil_typed_kernel(const HaloParams p) {
-  halo_body<typename VecOf<T>::type, kMode>(p);
-}
-
 // ------------------------------------------------------------- field values ----
-// u0(global row, column): a hash folded to [-32, 32) with 10 fractional bits, reproducible on the host
-// (models/halo.py::initial_field).  A field of type T starts at u0 rounded to T (exact for float and double).
-__device__ __forceinline__ float halo_u0(uint32_t grow, uint64_t j) {
-  const uint32_t jl = static_cast<uint32_t>(j);
-  const uint32_t h = (grow * 2654435761u) ^ (jl * 40503u + (jl >> 11));
-  return static_cast<float>(static_cast<int>(h & 0xFFFFu) - 32768) * (1.0f / 1024.0f);
-}
-
+// The closed-form initial field u0 (halo_u0, halo_field.h), rounded to the field type.
 template <class T>
-__device__ __forceinline__ void halo_init_body(T* __restrict__ u, T* __restrict__ halo_lo, T* __restrict__ halo_hi,
-                                               int rows, size_t row_elems, int rank, int world) {
+__global__ void halo_init_kernel(T* __restrict__ u, T* __restrict__ halo_lo, T* __restrict__ halo_hi, int rows,
+                                 size_t row_elems, int rank, int world) {
   const uint32_t grows = static_cast<uint32_t>(rows) * world;
   const uint32_t first = static_cast<uint32_t>(rank) * rows;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -441,25 +410,14 @@ __device__ __forceinline__ void halo_init_body(T* __restrict__ u, T* __restrict_
     if (halo_hi != nullptr) halo_hi[j] = Elem<T>::narrow(halo_u0((first + rows) % grows, j));
   }
 }
-__global__ void halo_init_kernel(float* __restrict__ u, float* __restrict__ halo_lo, float* __restrict__ halo_hi,
-                                 int rows, size_t row_elems, int rank, int world) {
-  halo_init_body(u, halo_lo, halo_hi, rows, row_elems, rank, world);
-}
-template <class T>
-__global__ void halo_init_typed_kernel(T* __restrict__ u, T* __restrict__ halo_lo, T* __restrict__ halo_hi, int rows,
-                                       size_t row_elems, int rank, int world) {
-  halo_init_body(u, halo_lo, halo_hi, rows, row_elems, rank, world);
-}
 
 // Independent check from the closed-form initial field: every thread owns one column of the GLOBAL
 // field (all world * rows rows), advances it `steps` times with the periodic stencil in the kernel's
 // operation order and compares this rank's rows bit for bit (Elem<T>::differs).  The column is kept in the compute
 // type, rounded to T after every step as the field is, so narrowing it back to T is exact.
-constexpr int kHaloMaxGlobalRows = 128;
 template <class T>
-__device__ __forceinline__ void halo_verify_init_body(const T* __restrict__ u, int rows, size_t row_elems, int rank,
-                                                      int world, uint32_t steps, float alpha, float s,
-                                                      unsigned long long* mismatch_count) {
+__global__ void halo_verify_init_kernel(const T* __restrict__ u, int rows, size_t row_elems, int rank, int world,
+                                        uint32_t steps, float alpha, float s, unsigned long long* mismatch_count) {
   using C = typename Elem<T>::Compute;
   const int G = rows * world;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -483,24 +441,13 @@ __device__ __forceinline__ void halo_verify_init_body(const T* __restrict__ u, i
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatch_count, bad);
 }
-__global__ void halo_verify_init_kernel(const float* __restrict__ u, int rows, size_t row_elems, int rank, int world,
-                                        uint32_t steps, float alpha, float s, unsigned long long* mismatch_count) {
-  halo_verify_init_body(u, rows, row_elems, rank, world, steps, alpha, s, mismatch_count);
-}
-template <class T>
-__global__ void halo_verify_init_typed_kernel(const T* __restrict__ u, int rows, size_t row_elems, int rank, int world,
-                                              uint32_t steps, float alpha, float s,
-                                              unsigned long long* mismatch_count) {
-  halo_verify_init_body(u, rows, row_elems, rank, world, steps, alpha, s, mismatch_count);
-}
 
 // Check of ONE step through an independent data path: plain (coherent) vector loads of the step's input,
 // including the neighbours' boundary rows wherever they live (peer-mapped field or local halo buffer).
 template <class T>
-__device__ __forceinline__ void halo_verify_step_body(const T* __restrict__ u_new, const T* __restrict__ u_old,
-                                                      const T* __restrict__ up_row, const T* __restrict__ dn_row,
-                                                      int rows, size_t row_elems, float alpha, float s,
-                                                      unsigned long long* mismatch_count) {
+__global__ void halo_verify_step_kernel(const T* __restrict__ u_new, const T* __restrict__ u_old,
+                                        const T* __restrict__ up_row, const T* __restrict__ dn_row, int rows,
+                                        size_t row_elems, float alpha, float s, unsigned long long* mismatch_count) {
   using V = typename VecOf<T>::type;
   using Raw = typename V::Raw;
   const size_t nvec = row_elems / (16 / sizeof(T));
@@ -522,81 +469,50 @@ __device__ __forceinline__ void halo_verify_step_body(const T* __restrict__ u_ne
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatch_count, bad);
 }
-__global__ void halo_verify_step_kernel(const float* __restrict__ u_new, const float* __restrict__ u_old,
-                                        const float* __restrict__ up_row, const float* __restrict__ dn_row, int rows,
-                                        size_t row_elems, float alpha, float s, unsigned long long* mismatch_count) {
-  halo_verify_step_body(u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch_count);
-}
-template <class T>
-__global__ void halo_verify_step_typed_kernel(const T* __restrict__ u_new, const T* __restrict__ u_old,
-                                              const T* __restrict__ up_row, const T* __restrict__ dn_row, int rows,
-                                              size_t row_elems, float alpha, float s,
-                                              unsigned long long* mismatch_count) {
-  halo_verify_step_body(u_new, u_old, up_row, dn_row, rows, row_elems, alpha, s, mismatch_count);
-}
 
-struct HaloGeometry {
-  uint32_t tile_bytes;
-  int ctas;
-};
+using StencilKernel = void (*)(HaloParams);
 
-template <class T>
-struct Tag {
-  using type = T;
-};
-// Calls f(Tag<T>{}) with the C++ type of a field type; any other type is an error.
-template <class F>
-void with_field_type(ElemType t, const char* what, F&& f) {
-  switch (t) {
-    case ElemType::kFloat: f(Tag<float>{}); return;
-    case ElemType::kDouble: f(Tag<double>{}); return;
-    case ElemType::kBFloat16: f(Tag<__nv_bfloat16>{}); return;
-    case ElemType::kHalf: f(Tag<__half>{}); return;
-    default: break;
-  }
-  HPCP_FAIL(std::string(what) + ": the field type must be float, double, bfloat16 or half");
+// The stencil kernel of a field type and mode: the one place that maps (ElemType, HaloMode) to an instantiation.
+StencilKernel stencil_kernel(ElemType type, HaloMode mode) {
+  StencilKernel k = nullptr;
+  with_field_type(type, "halo_stencil", [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    switch (mode) {
+      case HaloMode::kNone: k = halo_stencil_kernel<T, 0>; break;
+      case HaloMode::kPull: k = halo_stencil_kernel<T, 1>; break;
+      case HaloMode::kPush: k = halo_stencil_kernel<T, 2>; break;
+    }
+  });
+  return k;
 }
 
-template <class T, int kMode>
-constexpr auto stencil_kernel() {
-  if constexpr (std::is_same_v<T, float>)
-    return halo_stencil_kernel<kMode>;
-  else
-    return halo_stencil_typed_kernel<T, kMode>;
-}
-
-template <class T, int kMode>
-int occupancy_of() {
-  // One occupancy query per (type, mode, device), not per launch (per-step launches come here K times).
+// Resident CTAs per SM of a stencil kernel on the current device.  One occupancy query per (kernel, device), that is
+// per (type, mode, device), not per launch (per-step launches come here K times).
+int occupancy_of(StencilKernel kernel) {
   static std::mutex mu;
-  static int per_sm[64] = {0};
+  static std::map<std::pair<StencilKernel, int>, int> per_sm;
   int device = 0;
   HPCP_CUDA(cudaGetDevice(&device));
   std::lock_guard<std::mutex> lk(mu);
-  if (device < 0 || device >= 64 || per_sm[device] == 0) {
-    int n = 0;
-    HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, stencil_kernel<T, kMode>(), kHaloThreads, 0));
-    if (device < 0 || device >= 64) return n;
-    per_sm[device] = n;
-  }
-  return per_sm[device];
+  int& n = per_sm[{kernel, device}];
+  if (n == 0) HPCP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kHaloThreads, 0));
+  return n;
 }
+
+struct HaloGeometry {
+  StencilKernel kernel;
+  uint32_t tile_bytes;
+  int ctas;
+};
 
 HaloGeometry halo_geometry(size_t row_bytes, const HaloTuning& tune, HaloMode mode, int device, ElemType type) {
   HaloGeometry g;
   HPCP_REQUIRE(tune.tile_kb >= 0 && tune.tile_kb <= 1024, "halo_stencil: tile_kb in 1 .. 1024 (0 -> 16)");
   g.tile_bytes = static_cast<uint32_t>((tune.tile_kb > 0 ? tune.tile_kb : kHaloDefaultTileKb) * 1024);
   const int sms = device_sm_count(device);
-  int per_sm = 1;
+  g.kernel = stencil_kernel(type, mode);
   // Co-residency: a persistent multi-step launch spins on neighbour words, so every CTA must be resident.
-  with_field_type(type, "halo_stencil", [&](auto tag) {
-    using T = typename decltype(tag)::type;
-    switch (mode) {
-      case HaloMode::kNone: per_sm = occupancy_of<T, 0>(); break;
-      case HaloMode::kPull: per_sm = occupancy_of<T, 1>(); break;
-      case HaloMode::kPush: per_sm = occupancy_of<T, 2>(); break;
-    }
-  });
+  const int per_sm = occupancy_of(g.kernel);
   HPCP_REQUIRE(per_sm >= 1, "halo_stencil: kernel does not fit on an SM");
   const size_t tiles = (row_bytes + g.tile_bytes - 1) / g.tile_bytes;
   const int resident = std::min(sms * std::min(per_sm, kHaloCtasPerSm), kHaloMaxCtas);  // one step word per CTA
@@ -672,15 +588,7 @@ int launch_halo_stencil(const HaloStencilArgs& a, HaloMode mode, const HaloTunin
     p.signal_hi = a.flags_right + set_words;              // and the left neighbour of my right neighbour
     p.pace = a.flags_local + set_words + 1;               // word 1 of CTA 0's sector of the wait_lo side (unused)
   }
-  auto launch = [&](auto kernel) { kernel<<<ctas, kHaloThreads, 0, stream>>>(p); };
-  with_field_type(a.type, "halo_stencil", [&](auto tag) {
-    using T = typename decltype(tag)::type;
-    switch (mode) {
-      case HaloMode::kNone: launch(stencil_kernel<T, 0>()); break;
-      case HaloMode::kPull: launch(stencil_kernel<T, 1>()); break;
-      case HaloMode::kPush: launch(stencil_kernel<T, 2>()); break;
-    }
-  });
+  g.kernel<<<ctas, kHaloThreads, 0, stream>>>(p);
   HPCP_CUDA(cudaGetLastError());
   return ctas;
 }
@@ -691,11 +599,8 @@ void launch_halo_init(void* u, void* halo_lo, void* halo_hi, int rows, size_t ro
   const int ctas = std::max(static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 8)), 1);
   with_field_type(type, "halo_init", [&](auto tag) {
     using T = typename decltype(tag)::type;
-    T *pu = static_cast<T*>(u), *lo = static_cast<T*>(halo_lo), *hi = static_cast<T*>(halo_hi);
-    if constexpr (std::is_same_v<T, float>)
-      halo_init_kernel<<<ctas, threads, 0, stream>>>(pu, lo, hi, rows, row_elems, rank, world);
-    else
-      halo_init_typed_kernel<T><<<ctas, threads, 0, stream>>>(pu, lo, hi, rows, row_elems, rank, world);
+    halo_init_kernel<T><<<ctas, threads, 0, stream>>>(static_cast<T*>(u), static_cast<T*>(halo_lo),
+                                                      static_cast<T*>(halo_hi), rows, row_elems, rank, world);
   });
   HPCP_CUDA(cudaGetLastError());
 }
@@ -708,13 +613,8 @@ void launch_halo_verify_from_init(const void* u, int rows, size_t row_elems, int
   const int ctas = std::max(static_cast<int>(std::min<size_t>((row_elems + threads - 1) / threads, 132 * 16)), 1);
   with_field_type(type, "halo_verify_from_init", [&](auto tag) {
     using T = typename decltype(tag)::type;
-    const T* pu = static_cast<const T*>(u);
-    if constexpr (std::is_same_v<T, float>)
-      halo_verify_init_kernel<<<ctas, threads, 0, stream>>>(pu, rows, row_elems, rank, world, steps, alpha, s,
-                                                            mismatch_count);
-    else
-      halo_verify_init_typed_kernel<T><<<ctas, threads, 0, stream>>>(pu, rows, row_elems, rank, world, steps, alpha,
-                                                                     s, mismatch_count);
+    halo_verify_init_kernel<T><<<ctas, threads, 0, stream>>>(static_cast<const T*>(u), rows, row_elems, rank, world,
+                                                             steps, alpha, s, mismatch_count);
   });
   HPCP_CUDA(cudaGetLastError());
 }
@@ -728,12 +628,8 @@ void launch_halo_verify_step(const void* u_new, const void* u_old, const void* u
   with_field_type(type, "halo_verify_step", [&](auto tag) {
     using T = typename decltype(tag)::type;
     auto c = [](const void* q) { return static_cast<const T*>(q); };
-    if constexpr (std::is_same_v<T, float>)
-      halo_verify_step_kernel<<<ctas, threads, 0, stream>>>(c(u_new), c(u_old), c(up_row), c(dn_row), rows,
-                                                            row_elems, alpha, s, mismatch_count);
-    else
-      halo_verify_step_typed_kernel<T><<<ctas, threads, 0, stream>>>(c(u_new), c(u_old), c(up_row), c(dn_row), rows,
-                                                                     row_elems, alpha, s, mismatch_count);
+    halo_verify_step_kernel<T><<<ctas, threads, 0, stream>>>(c(u_new), c(u_old), c(up_row), c(dn_row), rows,
+                                                             row_elems, alpha, s, mismatch_count);
   });
   HPCP_CUDA(cudaGetLastError());
 }

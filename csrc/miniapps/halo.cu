@@ -40,6 +40,7 @@
 #include "../common/rank_runtime.h"
 #include "../common/signal_layout.h"
 #include "../kernels/api.h"
+#include "../kernels/halo_field.h"
 #include "devices.hpp"
 
 namespace {
@@ -234,43 +235,42 @@ __attribute__((noinline)) double host_stencil1(double prev, double cur, double n
   return mid + side;
 }
 
-float host_u0(uint32_t grow, uint64_t j) {  // halo_u0 of kernels/halo_stencil.cu
-  const uint32_t jl = static_cast<uint32_t>(j);
-  const uint32_t h = (grow * 2654435761u) ^ (jl * 40503u + (jl >> 11));
-  return static_cast<float>(static_cast<int>(h & 0xFFFFu) - 32768) * (1.0f / 1024.0f);
-}
-
-// Element type <-> compute type on the host, the same roundings as the kernels (cuda_bf16.h / cuda_fp16.h conversions
-// are host functions too).
-template <class T>
-struct HostElem {  // float, double
-  static T widen(T x) { return x; }
-  static T narrow(T x) { return x; }
-};
-template <>
-struct HostElem<__nv_bfloat16> {
-  static float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
-  static __nv_bfloat16 narrow(float x) { return __float2bfloat16_rn(x); }
-};
-template <>
-struct HostElem<__half> {
-  static float widen(__half x) { return __half2float(x); }
-  static __half narrow(float x) { return __float2half_rn(x); }
-};
 template <class T>
 T host_stencil(T prev, T cur, T next, float alpha, float s) {
-  using E = HostElem<T>;
+  using E = FieldElem<T>;
   return E::narrow(host_stencil1(E::widen(prev), E::widen(cur), E::widen(next), alpha, s));
 }
 template <class T>
 T host_init(uint32_t grow, uint64_t j) {
-  return HostElem<T>::narrow(host_u0(grow, j));
+  return FieldElem<T>::narrow(halo_u0(grow, j));
 }
 // The halo checks' rule (Elem<T>::differs in kernels/halo_stencil.cu): the same bit pattern, or both NaN.
 template <class T>
 bool host_same(T a, T b) {
   return std::memcmp(&a, &b, sizeof(T)) == 0 ||
-         (std::isnan(HostElem<T>::widen(a)) && std::isnan(HostElem<T>::widen(b)));
+         (std::isnan(FieldElem<T>::widen(a)) && std::isnan(FieldElem<T>::widen(b)));
+}
+
+// The report line and the JSON row of a run of P ranks: `what` names the variant, `ctas` the grid (0 on the host).
+void report(const Config& cfg, int P, const std::string& what, int ctas, double best_ms, unsigned long long total_bad) {
+  const double ms_per_step = best_ms / cfg.steps;
+  const double bus = static_cast<double>(P) * 2.0 * static_cast<double>(cfg.bytes) / (ms_per_step * 1e6);
+  const char* type = elem_type_name(cfg.type);
+  std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << best_ms << " ms for " << cfg.steps
+            << " steps = " << ms_per_step << " ms/step | halo " << what << " P=" << P << " rows=" << cfg.rows
+            << " bytes=" << cfg.bytes << " ctas=" << ctas << " type=" << type << " | " << bus
+            << " GB/s P2P bus (aggregate), " << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
+  if (!cfg.json_path.empty()) {
+    if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
+      std::fprintf(f,
+                   "{\"pattern\":\"halo\",\"variant\":\"%s\",\"ranks\":%d,\"rows\":%d,\"bytes\":%zu,\"steps\":%d,"
+                   "\"ms_per_step\":%.6f,\"bus_GBps\":%.3f,\"per_gpu_per_dir_GBps\":%.3f,\"ctas\":%d,"
+                   "\"mismatches\":%llu,\"type\":\"%s\"}\n",
+                   what.c_str(), P, cfg.rows, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, ctas, total_bad,
+                   type);
+      std::fclose(f);
+    }
+  }
 }
 
 template <class T>
@@ -361,24 +361,8 @@ int run_on_host(const Config& cfg) {
     for (int r = 0; r < P; ++r) std::fwrite(u[final_parity][r].data(), sizeof(T), u[final_parity][r].size(), f);
     std::fclose(f);
   }
-  const double ms_per_step = best_ms / cfg.steps;
-  const double bus = static_cast<double>(P) * 2.0 * static_cast<double>(cfg.bytes) / (ms_per_step * 1e6);
-  const std::string what = std::string(!cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode) + "/host-threads";
-  const char* type = elem_type_name(cfg.type);
-  std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << best_ms << " ms for " << cfg.steps
-            << " steps = " << ms_per_step << " ms/step | halo " << what << " P=" << P << " rows=" << R
-            << " bytes=" << cfg.bytes << " ctas=0 type=" << type << " | " << bus << " GB/s P2P bus (aggregate), "
-            << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
-  if (!cfg.json_path.empty()) {
-    if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
-      std::fprintf(f,
-                   "{\"pattern\":\"halo\",\"variant\":\"%s\",\"ranks\":%d,\"rows\":%d,\"bytes\":%zu,\"steps\":%d,"
-                   "\"ms_per_step\":%.6f,\"bus_GBps\":%.3f,\"per_gpu_per_dir_GBps\":%.3f,\"ctas\":0,"
-                   "\"mismatches\":%llu,\"type\":\"%s\"}\n",
-                   what.c_str(), P, R, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, total_bad, type);
-      std::fclose(f);
-    }
-  }
+  report(cfg, P, std::string(!cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode) + "/host-threads", 0, best_ms,
+         total_bad);
   return total_bad == 0 ? 0 : 1;
 }
 
@@ -437,20 +421,16 @@ int main(int argc, char** argv) {
     HPCP_REQUIRE(cfg.stock.empty() || cfg.stock == "memcpy", "--stock accepts memcpy");
     HPCP_REQUIRE(cfg.rows >= 1 && cfg.bytes >= 16 && cfg.bytes % 16 == 0, "--rows >= 1, --bytes a multiple of 16");
     HPCP_REQUIRE(cfg.dump_path.empty() || cfg.cpu, "--dump belongs to --cpu");
-    if (cfg.type != ElemType::kFloat && cfg.type != ElemType::kDouble && cfg.type != ElemType::kBFloat16 &&
-        cfg.type != ElemType::kHalf) {
+    int host_rc = 1;  // with --cpu the whole run happens inside the type dispatch
+    const bool field_type = with_field_type(cfg.type, [&](auto tag) {
+      if (cfg.cpu) host_rc = run_on_host<typename decltype(tag)::type>(cfg);
+    });
+    if (!field_type) {
       std::cerr << "Error: --type must be float, double, bfloat16 or half\n";
       print_help();
       return 1;
     }
-    if (cfg.cpu) {
-      switch (cfg.type) {
-        case ElemType::kDouble: return run_on_host<double>(cfg);
-        case ElemType::kBFloat16: return run_on_host<__nv_bfloat16>(cfg);
-        case ElemType::kHalf: return run_on_host<__half>(cfg);
-        default: return run_on_host<float>(cfg);
-      }
-    }
+    if (cfg.cpu) return host_rc;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
       (void)cudaGetLastError();
@@ -459,7 +439,7 @@ int main(int argc, char** argv) {
     }
     const int P = cfg.ranks > 0 ? cfg.ranks : ndev;
     HPCP_REQUIRE(P >= 1 && P <= kMaxRanks, "ranks out of range");
-    HPCP_REQUIRE(P * cfg.rows <= 128, "ranks x rows must not exceed 128 (verification kernel)");
+    HPCP_REQUIRE(P * cfg.rows <= kHaloMaxGlobalRows, "ranks x rows must not exceed 128 (verification kernel)");
     std::vector<int> devices;
     for (int r = 0; r < P; ++r) devices.push_back(primary_device(r, P, ndev));
     const int ranks_per_dev = (P + ndev - 1) / ndev;
@@ -486,26 +466,8 @@ int main(int argc, char** argv) {
 
     run_ranks(P, [&](RankCtx& ctx) { rank_main(ctx, sh); });
 
-    const double ms_per_step = sh.best_ms / cfg.steps;
-    const double bus = static_cast<double>(P) * 2.0 * static_cast<double>(cfg.bytes) / (ms_per_step * 1e6);
-    const std::string what =
-        !cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode + (cfg.per_step ? "/per-step" : "/persistent");
-    const char* type = elem_type_name(cfg.type);
-    std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << sh.best_ms << " ms for " << cfg.steps
-              << " steps = " << ms_per_step << " ms/step | halo " << what << " P=" << P << " rows=" << cfg.rows
-              << " bytes=" << cfg.bytes << " ctas=" << sh.ctas << " type=" << type << " | " << bus
-              << " GB/s P2P bus (aggregate), " << bus / P / 2.0 << " GB/s per GPU per direction" << std::endl;
-    if (!cfg.json_path.empty()) {
-      if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
-        std::fprintf(f,
-                     "{\"pattern\":\"halo\",\"variant\":\"%s\",\"ranks\":%d,\"rows\":%d,\"bytes\":%zu,\"steps\":%d,"
-                     "\"ms_per_step\":%.6f,\"bus_GBps\":%.3f,\"per_gpu_per_dir_GBps\":%.3f,\"ctas\":%d,"
-                     "\"mismatches\":%llu,\"type\":\"%s\"}\n",
-                     what.c_str(), P, cfg.rows, cfg.bytes, cfg.steps, ms_per_step, bus, bus / P / 2.0, sh.ctas,
-                     sh.total_bad, type);
-        std::fclose(f);
-      }
-    }
+    report(cfg, P, !cfg.stock.empty() ? "stock-" + cfg.stock : cfg.mode + (cfg.per_step ? "/per-step" : "/persistent"),
+           sh.ctas, sh.best_ms, sh.total_bad);
     mem.free(sh.field);
     mem.free(sh.halo);
     mem.free(sh.flags);

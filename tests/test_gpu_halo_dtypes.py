@@ -1,8 +1,9 @@
-"""GPU tests of K-halo's double, bfloat16 and half fields (halo_stencil_typed_kernel and the typed init / verify
-kernels in csrc/kernels/halo_stencil.cu), bit for bit against models/halo.py::reference_steps: virtual rings of 1-8
-ranks in pull and push mode with per-step and persistent launches, rows that are not a multiple of the column tile,
-24 MiB rows at the default geometry, the stock memcpy / NCCL arms, step_from_host, the stencil_step op (subnormal
-results of the 16-bit types are kept), and the native and torchrun command lines."""
+"""GPU tests of K-halo's double, bfloat16 and half fields (the double, __nv_bfloat16 and __half instantiations of
+halo_stencil_kernel, halo_init_kernel, halo_verify_init_kernel and halo_verify_step_kernel in
+csrc/kernels/halo_stencil.cu), bit for bit against models/halo.py::reference_steps: virtual rings of 1-8 ranks in pull
+and push mode with per-step and persistent launches, rows that are not a multiple of the column tile, 24 MiB rows at
+the default geometry, the stock memcpy / NCCL arms, step_from_host, the stencil_step op (subnormal results of the
+16-bit types are kept), and the native and torchrun command lines."""
 import os
 import subprocess
 import sys

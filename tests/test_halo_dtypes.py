@@ -9,7 +9,7 @@
    error.
 4. The Python layer (HaloStencil / VirtualRing / step_from_host / stock steps / stencil_step checks) on the emulated
    device of tests/halo_dtype_emu.py; fp32 calls into the native module keep their old shape.
-5. No typed K-halo stencil kernel touches local memory.
+5. No double, bfloat16 or half instantiation of the K-halo stencil kernel touches local memory.
 """
 import os
 import re
@@ -272,11 +272,12 @@ def test_unsupported_dtype_is_refused(emu):
 
 
 # ------------------------------------------------------------------------------------------- SASS ----
-def test_typed_stencil_kernels_use_no_local_memory(native):
+def test_non_float_stencil_kernels_use_no_local_memory(native):
     obj = os.path.join(ROOT, "build", "kernels", "halo_stencil.o")
     sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
     fns = re.split(r"\n\s+Function : ", sass)[1:]
-    typed = [f for f in fns if "halo_stencil_typed_kernel" in f.split("\n", 1)[0]]
+    # the nine non-float instantiations; the fp32 pull kernel keeps a documented once-per-tile local slot
+    typed = [f for f in fns if re.search(r"halo_stencil_kernelI(?!f)", f.split("\n", 1)[0])]
     assert len(typed) == 9
     for f in typed:
         assert not re.search(r"\b(STL|LDL)", f), f.split("\n", 1)[0]
