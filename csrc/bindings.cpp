@@ -55,7 +55,7 @@ ElemType elem_from(const std::string& s) {
 ReduceOp op_from(const std::string& s) {
   ReduceOp op;
   if (reduce_op_from_name(s, &op)) return op;
-  throw std::invalid_argument("op must be one of sum prod product min max, not '" + s + "'");
+  throw std::invalid_argument("op must be one of sum prod product min max band bor bxor land lor lxor, not '" + s + "'");
 }
 
 CopyTuning tuning_from(const py::dict& d) {
@@ -626,7 +626,8 @@ PYBIND11_MODULE(_C, m) {
                           op_from(op));
       },
       py::arg("va"), py::arg("vc"), py::arg("n"), py::arg("dtype"), py::arg("stream"), py::arg("op") = "sum",
-      "VC += VA (op=sum), else VC = op(VC, VA); op = sum | prod | product | min | max.");
+      "VC += VA (op=sum), else VC = op(VC, VA); op = sum | prod | product | min | max, and on integer types "
+      "band | bor | bxor | land | lor | lxor.");
   m.def("count_mismatch", [](uintptr_t v, size_t n, double expected, const std::string& dtype,
                              uintptr_t count, uintptr_t stream) {
     launch_count_mismatch(as_ptr<const void>(v), n, expected, elem_from(dtype),
@@ -734,7 +735,8 @@ PYBIND11_MODULE(_C, m) {
       py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0,
       py::arg("phases") = "allreduce", py::arg("op") = "sum",
       "Reduce-scatter + all-gather ring in one launch per rank (kernels/ring_order.h: rsag_*); "
-      "phases = allreduce | reduce_scatter | all_gather; op = sum | prod | product | min | max.");
+      "phases = allreduce | reduce_scatter | all_gather; op = sum | prod | product | min | max, and on integer "
+      "types band | bor | bxor | land | lor | lxor.");
   m.def(
       "allreduce_two_shot",
       [](const std::vector<uintptr_t>& va, const std::vector<uintptr_t>& vc,

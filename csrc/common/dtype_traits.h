@@ -150,12 +150,18 @@ void dispatch_add_class(ElemType t, F&& f) {
 template <typename T>
 constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
 
-// Reduction by name: sum, prod (or product), min, max; false if unknown.
+// Reduction by name: sum, prod (or product), min, max, band, bor, bxor, land, lor, lxor; false if unknown.
 inline bool reduce_op_from_name(const std::string& name, ReduceOp* out) {
   if (name == "sum") *out = ReduceOp::kSum;
   else if (name == "prod" || name == "product") *out = ReduceOp::kProd;
   else if (name == "min") *out = ReduceOp::kMin;
   else if (name == "max") *out = ReduceOp::kMax;
+  else if (name == "band") *out = ReduceOp::kBAnd;
+  else if (name == "bor") *out = ReduceOp::kBOr;
+  else if (name == "bxor") *out = ReduceOp::kBXor;
+  else if (name == "land") *out = ReduceOp::kLAnd;
+  else if (name == "lor") *out = ReduceOp::kLOr;
+  else if (name == "lxor") *out = ReduceOp::kLXor;
   else return false;
   return true;
 }
@@ -165,8 +171,28 @@ inline const char* reduce_op_name(ReduceOp op) {
     case ReduceOp::kProd: return "prod";
     case ReduceOp::kMin: return "min";
     case ReduceOp::kMax: return "max";
+    case ReduceOp::kBAnd: return "band";
+    case ReduceOp::kBOr: return "bor";
+    case ReduceOp::kBXor: return "bxor";
+    case ReduceOp::kLAnd: return "land";
+    case ReduceOp::kLOr: return "lor";
+    case ReduceOp::kLXor: return "lxor";
   }
   return "?";
+}
+
+// The bitwise and logical ops reduce the integer types only, as in MPI.
+inline bool reduce_op_integer_only(ReduceOp op) {
+  return op == ReduceOp::kBAnd || op == ReduceOp::kBOr || op == ReduceOp::kBXor || op == ReduceOp::kLAnd ||
+         op == ReduceOp::kLOr || op == ReduceOp::kLXor;
+}
+inline bool elem_type_is_integer(ElemType t) {
+  return t != ElemType::kFloat && t != ElemType::kDouble && t != ElemType::kBFloat16 && t != ElemType::kHalf;
+}
+// The refusal of an integer-only op on a floating type, the same words in every layer.
+inline std::string reduce_op_type_error(ReduceOp op, ElemType t) {
+  return std::string("op must be sum, prod, min or max for ") + elem_type_name(t) + ": " + reduce_op_name(op) +
+         " reduces integer types only";
 }
 
 }  // namespace hpcp

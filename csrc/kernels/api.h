@@ -302,9 +302,10 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
                        cudaStream_t stream);
 
 // ------------------------------------------------------ allreduce miniapp ----
-// The reduction of an allreduce (↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX).  kSum accumulates into VC as the
-// reference does; the other ops overwrite VC (docs/allreduce.md has their semantics per type).  NVLS is sum-only.
-enum class ReduceOp : int { kSum = 0, kProd = 1, kMin = 2, kMax = 3 };
+// The reduction of an allreduce (↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX, and on the integer types MPI_BAND / MPI_BOR
+// / MPI_BXOR / MPI_LAND / MPI_LOR / MPI_LXOR).  kSum accumulates into VC as the reference does; the other ops overwrite
+// VC (docs/allreduce.md has their semantics per type).  NVLS is sum-only.
+enum class ReduceOp : int { kSum = 0, kProd = 1, kMin = 2, kMax = 3, kBAnd = 4, kBOr, kBXor, kLAnd, kLOr, kLXor };
 
 // VA = a, VB = b, VC = c (↔ Initialize, allreduce-mpi-sycl.cpp:33-41). Any pointer may be null.
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,

@@ -1,4 +1,6 @@
-// Allreduce kernels for the reductions other than the sum: prod, min and max (↔ MPI_PROD / MPI_MIN / MPI_MAX).
+// Allreduce kernels for the reductions other than the sum: prod, min and max (↔ MPI_PROD / MPI_MIN / MPI_MAX), and on
+// the integer types band, bor, bxor, land, lor and lxor (↔ MPI_BAND / MPI_BOR / MPI_BXOR / MPI_LAND / MPI_LOR /
+// MPI_LXOR).
 //
 // They are the kernel templates of ring_allreduce.cuh, the ones the sum runs, instantiated with another combine policy:
 // the same loads, stores, arrival / ack words and barriers, in the same combine order.  Two differences on purpose:
@@ -8,7 +10,9 @@
 //   min / max   integers compare signed or unsigned by type; floats follow IEEE 754-2019 minimum / maximum (any NaN
 //               gives NaN, -0 < +0), 16-bit floats in their own format (the result is one of the inputs);
 //   prod        integers wrap modulo 2^w (signed and unsigned share the bits, as for the sum); floats round every
-//               product to nearest even without FTZ; two-shot multiplies the 16-bit types in fp32 and rounds once.
+//               product to nearest even without FTZ; two-shot multiplies the 16-bit types in fp32 and rounds once;
+//   band / bor / bxor   &, |, ^ of the element bits, whatever the width and signedness (one kernel set for all);
+//   land / lor / lxor   an element is true iff it is nonzero over its whole width; the result is 0 or 1 of the type.
 // A NaN result is the type's canonical quiet NaN (all bits set but the sign), the same bits on every rank.
 #include "ring_allreduce.cuh"
 
@@ -202,6 +206,78 @@ struct Prod8 : Wide8<T, MulF32Raw> {
 template <> struct TwoShotInF32<Prod<__nv_bfloat16>> : std::true_type { using acc = Prod8<__nv_bfloat16>; };
 template <> struct TwoShotInF32<Prod<__half>> : std::true_type { using acc = Prod8<__half>; };
 
+// ------------------------------------------------- bitwise and logical ----
+// Integer types only (dispatch_op refuses the floating ones).  All six are exact, commutative and associative: every
+// combine order gives the same bits.
+
+// band / bor / bxor act on the bits alone: one instantiation serves every integer type.
+struct AndW {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return a & b; }
+};
+struct OrW {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return a | b; }
+};
+struct XorW {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return a ^ b; }
+};
+struct BAnd : Words<AndW> {};
+struct BOr : Words<OrW> {};
+struct BXor : Words<XorW> {};
+
+// The lanes of width class C (AddClass): t(x) is 1 in every lane of x that is nonzero over the whole element width (a
+// long holding 1 << 40 is true) and 0 in the others.  Two lanes are both true iff their unsigned minimum (umin) is
+// nonzero and either is iff their OR is, so land and lor test one value per lane; lxor (x) is lor but not land (for
+// bytes on the top bit of each lane before it is normalised).  Each form keeps the push and pull rings within the
+// registers of Max of the same width (testing every input on its own costs the narrow lanes two more).
+template <typename C> struct Lanes;
+template <> struct Lanes<int> {
+  static __device__ __forceinline__ uint32_t t(uint32_t x) { return x != 0u; }
+  static __device__ __forceinline__ uint32_t umin(uint32_t a, uint32_t b) { return min(a, b); }
+  static __device__ __forceinline__ uint32_t x(uint32_t a, uint32_t b) { return t(a | b) ^ t(umin(a, b)); }
+};
+template <> struct Lanes<long long> {  // the full 64-bit lane, never its 32-bit halves
+  using W = unsigned long long;
+  static __device__ __forceinline__ W t(W x) { return x != 0ull; }
+  static __device__ __forceinline__ W umin(W a, W b) { return min(a, b); }
+  static __device__ __forceinline__ W x(W a, W b) { return t(a | b) ^ t(umin(a, b)); }
+};
+template <> struct Lanes<short> {
+  static __device__ __forceinline__ uint32_t t(uint32_t x) { return __vcmpne2(x, 0u) & 0x00010001u; }
+  static __device__ __forceinline__ uint32_t umin(uint32_t a, uint32_t b) { return __vminu2(a, b); }
+  static __device__ __forceinline__ uint32_t x(uint32_t a, uint32_t b) { return t(a | b) ^ t(umin(a, b)); }
+};
+template <> struct Lanes<unsigned char> {
+  static __device__ __forceinline__ uint32_t t(uint32_t x) { return __vcmpne4(x, 0u) & 0x01010101u; }
+  static __device__ __forceinline__ uint32_t umin(uint32_t a, uint32_t b) { return __vminu4(a, b); }
+  // (v & 0x7f) + 0x7f carries into the top bit of a byte iff its low bits are nonzero, and | v adds the top bit itself
+  static __device__ __forceinline__ uint32_t top(uint32_t v) { return ((v & 0x7f7f7f7fu) + 0x7f7f7f7fu) | v; }
+  static __device__ __forceinline__ uint32_t x(uint32_t a, uint32_t b) {
+    return ((top(a | b) ^ top(umin(a, b))) >> 7) & 0x01010101u;
+  }
+};
+
+struct LAndF {
+  template <class L, typename W> static __device__ __forceinline__ W g(W a, W b) { return L::t(L::umin(a, b)); }
+};
+struct LOrF {
+  template <class L, typename W> static __device__ __forceinline__ W g(W a, W b) { return L::t(a | b); }
+};
+struct LXorF {
+  template <class L, typename W> static __device__ __forceinline__ W g(W a, W b) { return L::x(a, b); }
+};
+template <typename C, class F>
+struct LogicW {
+  static __device__ __forceinline__ uint32_t f(uint32_t a, uint32_t b) { return F::template g<Lanes<C>>(a, b); }
+  static __device__ __forceinline__ unsigned long long f64(unsigned long long a, unsigned long long b) {
+    return F::template g<Lanes<C>>(a, b);
+  }
+};
+template <typename C, class L> struct LanesOf : Words<L> {};
+template <class L> struct LanesOf<long long, L> : DWords<L> {};
+template <typename C> struct LAnd : LanesOf<C, LogicW<C, LAndF>> {};
+template <typename C> struct LOr : LanesOf<C, LogicW<C, LOrF>> {};
+template <typename C> struct LXor : LanesOf<C, LogicW<C, LXorF>> {};
+
 // ---------------------------------------------------------------- kernels ----
 // VC = op(VC, VA) over whole vectors; block 0's thread 0 combines the last partial vector in registers and writes back
 // only its tail_bytes.
@@ -223,7 +299,22 @@ __global__ void __launch_bounds__(512) combine_kernel(const uint4* __restrict__ 
   }
 }
 
-// Run f(Op{}) with the combine policy of (type, op).
+// The bitwise and logical policies of width class C.
+template <typename C, typename F>
+void dispatch_bit_op(ReduceOp op, F& f) {
+  switch (op) {
+    case ReduceOp::kBAnd: f(BAnd{}); break;
+    case ReduceOp::kBOr: f(BOr{}); break;
+    case ReduceOp::kBXor: f(BXor{}); break;
+    case ReduceOp::kLAnd: f(LAnd<C>{}); break;
+    case ReduceOp::kLOr: f(LOr<C>{}); break;
+    case ReduceOp::kLXor: f(LXor<C>{}); break;
+    default: HPCP_FAIL("allreduce ops: not a bitwise or logical op"); break;
+  }
+}
+
+// Run f(Op{}) with the combine policy of (type, op).  The bitwise and logical ops are refused for the floating types
+// here, before any kernel is chosen, as MPI refuses them.
 template <typename F>
 void dispatch_op(ElemType type, ReduceOp op, F&& f) {
   dispatch_elem(type, [&](auto tag) {
@@ -233,6 +324,12 @@ void dispatch_op(ElemType type, ReduceOp op, F&& f) {
       case ReduceOp::kMin: f(Min<T>{}); break;
       case ReduceOp::kProd: f(Prod<typename AddClass<T>::type>{}); break;
       case ReduceOp::kSum: HPCP_FAIL("allreduce ops: the sum has its own kernels"); break;
+      default:
+        if constexpr (std::is_integral<T>::value)
+          dispatch_bit_op<typename AddClass<T>::type>(op, f);
+        else
+          HPCP_FAIL(reduce_op_type_error(op, type));
+        break;
     }
   });
 }

@@ -27,6 +27,11 @@
 // overwrite VC and run on every algorithm except nvls (sum-only; -a picks two-shot for them).  Each op has its own
 // constant-data check, exact in every type up to P = 16: max (rank r holds r) -> P-1, min (P-r) -> 1, prod (2 on the
 // odd ranks below 8, else 1) -> 2^min(P/2, 4).
+// On the integer types only (↔ MPI_BAND ... MPI_LXOR; a floating --type is a usage error): band, bor, bxor, land, lor
+// and lxor, same rules.  Their checks (docs/allreduce.md) are exact in uchar and tell the bitwise from the logical op at
+// every P >= 2: band (255 - 2^(r mod 4)) -> 256 - 2^min(P,4), bor (2^(r mod 4)) -> 2^min(P,4) - 1, bxor (128 on rank 0,
+// r elsewhere) -> 128 ^ 1 ^ ... ^ (P-1), land (r+1) -> 1, lor (2(r mod 2)) -> 1, lxor (3 on rank 0, else 0) -> 1; at
+// P = 1 VC is VA.
 #include <cuda_profiler_api.h>
 #include <getopt.h>
 
@@ -104,6 +109,7 @@ void print_help() {
                "                            bandwidth-optimal reduce-scatter + all-gather ring\n"
                " --coll auto|nvls|twoshot   collective used with -a\n"
                " --op sum|prod|min|max      reduction (default sum; nvls is sum-only, -a uses two-shot for the others)\n"
+               "    |band|bor|bxor|land|lor|lxor   bitwise and logical reductions: integer types only\n"
                " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
                " --ctas N --chunk N    kernel tuning (CTAs per rank, elements per ring chunk)\n"
                " --pull                fused ring, receiver-driven: every block is LOADED from the left neighbour's\n"
@@ -167,12 +173,22 @@ T host_canonical_nan() {
 // op(a, b) with the kernels' semantics (docs/allreduce.md): integers compare by their own signedness and multiply
 // modulo 2^w; floats follow IEEE maximum / minimum (NaN wins, -0 < +0) and round every product once; the 16-bit floats
 // compare exactly and round every product to their format (from its exact fp64 value); NaN results are canonical.
+// The bitwise ops act on the bits; the logical ones take an element as true iff it is nonzero and give 0 or 1.
 template <typename T>
 T host_combine(ReduceOp op, T a, T b) {
   if (op == ReduceOp::kSum) return host_add(a, b);
   if constexpr (std::is_integral<T>::value) {
-    if (op == ReduceOp::kProd)
-      return static_cast<T>(static_cast<unsigned long long>(a) * static_cast<unsigned long long>(b));
+    switch (op) {
+      case ReduceOp::kProd:
+        return static_cast<T>(static_cast<unsigned long long>(a) * static_cast<unsigned long long>(b));
+      case ReduceOp::kBAnd: return static_cast<T>(a & b);
+      case ReduceOp::kBOr: return static_cast<T>(a | b);
+      case ReduceOp::kBXor: return static_cast<T>(a ^ b);
+      case ReduceOp::kLAnd: return static_cast<T>(a != 0 && b != 0);
+      case ReduceOp::kLOr: return static_cast<T>(a != 0 || b != 0);
+      case ReduceOp::kLXor: return static_cast<T>((a != 0) != (b != 0));
+      default: break;
+    }
     return op == ReduceOp::kMax ? std::max(a, b) : std::min(a, b);
   } else {
     const double x = host_to_double(a), y = host_to_double(b);
@@ -194,27 +210,52 @@ T host_combine(ReduceOp op, T a, T b) {
 
 // Constant-data check of every op: what rank r holds and what every element of the result must equal (exact up to
 // P = 16 in every type).
+// The integer-only ops' values fit in uchar, and each bitwise op's result differs from its logical twin's at P >= 2.
 double op_input(ReduceOp op, int r, int P) {
   switch (op) {
     case ReduceOp::kSum: return r;
     case ReduceOp::kMax: return r;
     case ReduceOp::kMin: return P - r;
     case ReduceOp::kProd: return r % 2 == 1 && r < 8 ? 2 : 1;
+    case ReduceOp::kBAnd: return 255 - (1 << (r % 4));
+    case ReduceOp::kBOr: return 1 << (r % 4);
+    case ReduceOp::kBXor: return r == 0 ? 128 : r;
+    case ReduceOp::kLAnd: return r + 1;
+    case ReduceOp::kLOr: return 2 * (r % 2);
+    case ReduceOp::kLXor: return r == 0 ? 3 : 0;
   }
   return 0;
 }
 double op_expected(ReduceOp op, int P) {
+  int x = 128;
   switch (op) {
     case ReduceOp::kSum: return 0.5 * P * (P - 1);
     case ReduceOp::kMax: return P - 1;
     case ReduceOp::kMin: return 1;
     case ReduceOp::kProd: return std::ldexp(1.0, std::min(P / 2, 4));
+    case ReduceOp::kBAnd: return 256 - (1 << std::min(P, 4));
+    case ReduceOp::kBOr: return (1 << std::min(P, 4)) - 1;
+    case ReduceOp::kBXor:
+      for (int r = 1; r < P; ++r) x ^= r;
+      return x;
+    case ReduceOp::kLAnd: return 1;
+    case ReduceOp::kLOr: return P >= 2 ? 1 : 0;
+    case ReduceOp::kLXor: return P >= 2 ? 1 : 3;  // one rank: VC is VA, unnormalised
   }
   return 0;
 }
 // VC before the run: 0 for the sum, which accumulates into it; for the other ops a value that would change the result
 // if a kernel read VC instead of overwriting it.
-double op_vc_init(ReduceOp op, int P) { return op == ReduceOp::kMax ? P : 0; }
+double op_vc_init(ReduceOp op, int P) {
+  switch (op) {
+    case ReduceOp::kMax: return P;
+    case ReduceOp::kBOr: return 16;
+    case ReduceOp::kBXor: return 64;
+    case ReduceOp::kLOr: return 3;
+    case ReduceOp::kLXor: return 5;
+    default: return 0;
+  }
+}
 // The JSON rows carry "op" only when it is not the sum (sum rows keep their shape).
 std::string op_json(ReduceOp op) {
   return op == ReduceOp::kSum ? std::string() : std::string(",\"op\":\"") + reduce_op_name(op) + "\"";
@@ -659,7 +700,8 @@ int main(int argc, char** argv) {
         case 12: cfg.map_alias = true; break;
         case 13: cfg.profile_relaunch = true; break;
         case 14:
-          if (!reduce_op_from_name(optarg, &cfg.op)) HPCP_FAIL(std::string("unknown --op ") + optarg + " (sum|prod|min|max)");
+          if (!reduce_op_from_name(optarg, &cfg.op))
+            HPCP_FAIL(std::string("unknown --op ") + optarg + " (sum|prod|min|max|band|bor|bxor|land|lor|lxor)");
           break;
         case 10: cfg.slots = std::atoi(optarg); break;
         case 11: cfg.pull = true; break;
@@ -674,6 +716,8 @@ int main(int argc, char** argv) {
                  "--slots 2 and --pull are variants of --algo ring, not of ring-rsag");
     HPCP_REQUIRE(cfg.op == ReduceOp::kSum || !cfg.use_collective || cfg.coll != "nvls",
                  std::string("--coll nvls is sum-only: --op ") + reduce_op_name(cfg.op) + " needs --coll twoshot or auto");
+    HPCP_REQUIRE(!reduce_op_integer_only(cfg.op) || elem_type_is_integer(cfg.type),
+                 reduce_op_type_error(cfg.op, cfg.type) + " (pass --type or run a typed binary such as allreduce.int)");
 
     if (cfg.cpu) return run_on_host(cfg);
     const int ndev = visible_device_count();

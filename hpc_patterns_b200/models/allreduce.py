@@ -19,6 +19,10 @@ element of VC equals P(P-1)/2.  Algorithms:
 Reductions (``op``, ↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX): ``sum`` (default) accumulates into VC; ``prod``, ``min``
 and ``max`` overwrite it, on every algorithm but nvls (sum-only).  Each op has its own constant-data check: max (rank r
 holds r) -> P-1, min (P-r) -> 1, prod (2 on the odd ranks below 8, else 1) -> 2^min(P/2, 4).
+On the integer types only (↔ MPI_BAND / MPI_BOR / MPI_BXOR / MPI_LAND / MPI_LOR / MPI_LXOR): ``band``, ``bor``,
+``bxor`` act on the element bits; ``land``, ``lor``, ``lxor`` take an element as true iff it is nonzero and give 0 or 1
+(at one rank VC is VA).  A floating type is refused, as MPI does, and so is ``nccl``, which has no such reductions.
+Their checks are listed in ``op_input`` and ``expected_value``.
 
 The native single-process CLI twin is ``bin/allreduce`` (csrc/miniapps/allreduce.cu).
 """
@@ -44,9 +48,11 @@ _TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32,
                 "long": torch.int64, "ulong": torch.int64, "short": torch.int16, "ushort": torch.int16,
                 "uchar": torch.uint8, "bfloat16": torch.bfloat16, "half": torch.float16}
 FLOAT16_TYPES = ("bfloat16", "half")
-OPS = ("sum", "prod", "min", "max")
+INTEGER_OPS = ("band", "bor", "bxor", "land", "lor", "lxor")   # integer types only, as in MPI
+OPS = ("sum", "prod", "min", "max") + INTEGER_OPS
 _OP_ALIASES = {"product": "prod"}
 UNSIGNED_TYPES = ("uint", "ulong", "ushort")   # torch stand-ins are signed: NCCL min/max would compare them signed
+FLOAT_TYPES = ("float", "double") + FLOAT16_TYPES
 
 
 def reduce_op(op: str) -> str:
@@ -57,6 +63,12 @@ def reduce_op(op: str) -> str:
     return op
 
 
+def check_op_type(op: str, dtype: str) -> None:
+    """ValueError if ``op`` does not reduce ``dtype``: the bitwise and logical ops take integer types only."""
+    if reduce_op(op) in INTEGER_OPS and dtype in FLOAT_TYPES:
+        raise ValueError(f"op must be sum, prod, min or max for {dtype}: {reduce_op(op)} reduces integer types only")
+
+
 def expected_value(world: int, op: str = "sum") -> float:
     """Every element of VC after the constant-data run of ``op`` (see ``op_input``)."""
     if op == "max":
@@ -65,16 +77,50 @@ def expected_value(world: int, op: str = "sum") -> float:
         return 1.0
     if op == "prod":
         return 2.0 ** min(world // 2, 4)
+    if op == "band":
+        return 256.0 - 2 ** min(world, 4)
+    if op == "bor":
+        return 2.0 ** min(world, 4) - 1
+    if op == "bxor":
+        x = 128
+        for r in range(1, world):
+            x ^= r
+        return float(x)
+    if op == "land":
+        return 1.0
+    if op == "lor":
+        return 1.0 if world >= 2 else 0.0
+    if op == "lxor":
+        return 1.0 if world >= 2 else 3.0     # one rank: VC is VA, unnormalised
     return world * (world - 1) / 2.0
 
 
 def op_input(op: str, rank: int, world: int) -> float:
-    """What ``rank`` holds in the constant-data run of ``op`` (exact in every type up to 16 ranks)."""
+    """What ``rank`` holds in the constant-data run of ``op`` (exact in every type up to 16 ranks).  The integer-only
+    ops' values fit in uchar, and each bitwise op's result differs from its logical twin's from 2 ranks on."""
     if op == "min":
         return float(world - rank)
     if op == "prod":
         return 2.0 if rank % 2 == 1 and rank < 8 else 1.0
+    if op == "band":
+        return 255.0 - 2 ** (rank % 4)
+    if op == "bor":
+        return 2.0 ** (rank % 4)
+    if op == "bxor":
+        return 128.0 if rank == 0 else float(rank)
+    if op == "land":
+        return rank + 1.0
+    if op == "lor":
+        return 2.0 * (rank % 2)
+    if op == "lxor":
+        return 3.0 if rank == 0 else 0.0
     return float(rank)
+
+
+def vc_init(op: str, world: int) -> float:
+    """VC before the constant-data run: 0 for the sum, which accumulates into it; for the other ops a value that would
+    change the result if a kernel read VC instead of overwriting it."""
+    return {"max": float(world), "bor": 16.0, "bxor": 64.0, "lor": 3.0, "lxor": 5.0}.get(op, 0.0)
 
 
 def _nccl_op(op: str):
@@ -161,15 +207,19 @@ class AllreduceMiniapp:
         every block is loaded from the left neighbour's memory instead of being stored into the right neighbour's.
         ``n_elems``: exact element count per rank instead of 2^log2_elems.  ``_shared``: buffers made by an
         in-process group (``VirtualAllreduce``): ``pads``, ``va``, ``vc`` and, where the algorithm uses them, ``vb`` and
-        ``slots``.  ``op``: sum (default), prod / product, min or max; nvls is sum-only, and the NCCL algorithms refuse
-        min / max on unsigned types (their torch stand-ins are signed)."""
+        ``slots``.  ``op``: sum (default), prod / product, min or max; on integer types also band, bor, bxor, land, lor
+        or lxor.  nvls is sum-only, nccl has no bitwise or logical reductions, and the NCCL algorithms refuse min / max
+        on unsigned types (their torch stand-ins are signed)."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
         if dtype not in _TORCH_DTYPE:
             raise ValueError(f"dtype must be one of {sorted(_TORCH_DTYPE)}")
         op = reduce_op(op)
+        check_op_type(op, dtype)
         if op != "sum" and algo == "nvls":
             raise ValueError(f"nvls reduces sums only: op={op} needs twoshot or a ring")
+        if op in INTEGER_OPS and algo == "nccl":
+            raise ValueError(f"nccl has no bitwise or logical reductions: op={op} needs twoshot or a ring")
         if op in ("min", "max") and algo in ("nccl", "ring-nccl") and dtype in UNSIGNED_TYPES:
             raise ValueError(f"{algo} compares {dtype} as a signed torch type: op={op} is refused")
         self.op = op
@@ -244,8 +294,7 @@ class AllreduceMiniapp:
         vb = self.vb.local_ptr if self.vb is not None else 0
         x = op_input(self.op, self.rank, self.world)
         # VC: 0 for the sum, which accumulates into it; the other ops must overwrite it whatever it holds
-        self.C.init3(va, vb, vc, self.n, x, x, float(self.world) if self.op == "max" else 0.0, self.dtype,
-                     self._stream())
+        self.C.init3(va, vb, vc, self.n, x, x, vc_init(self.op, self.world), self.dtype, self._stream())
 
     def run_once(self) -> None:
         """Enqueue one allreduce on the current stream (no host sync except for ring-nccl).
@@ -331,7 +380,13 @@ class AllreduceMiniapp:
             acc = tensor_from_ptr(vc, self.nbytes, self.device, td)
             combine = {"sum": lambda: acc.add_(cur), "prod": lambda: torch.mul(acc, cur, out=acc),
                        "min": lambda: torch.minimum(acc, cur, out=acc),
-                       "max": lambda: torch.maximum(acc, cur, out=acc)}
+                       "max": lambda: torch.maximum(acc, cur, out=acc),
+                       "band": lambda: torch.bitwise_and(acc, cur, out=acc),
+                       "bor": lambda: torch.bitwise_or(acc, cur, out=acc),
+                       "bxor": lambda: torch.bitwise_xor(acc, cur, out=acc),
+                       "land": lambda: acc.copy_(torch.logical_and(acc, cur).to(td)),
+                       "lor": lambda: acc.copy_(torch.logical_or(acc, cur).to(td)),
+                       "lxor": lambda: acc.copy_(torch.logical_xor(acc, cur).to(td))}
             if self.op == "sum":
                 acc.add_(cur)
             else:
@@ -408,6 +463,7 @@ class VirtualAllreduce:
         if algo not in VIRTUAL_ALGOS:
             raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
         op = reduce_op(op)
+        check_op_type(op, dtype)
         C = native()
         esz = C.elem_size(dtype)
         n = element_count(esz, world, n_elems=n)
@@ -504,9 +560,11 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--pull", action="store_true",
                     help="fused ring, receiver-driven: blocks are loaded from the left neighbour (peer loads)")
     ap.add_argument("--op", default="sum", choices=OPS + tuple(_OP_ALIASES),
-                    help="reduction (default sum; nvls is sum-only, -a uses two-shot for the others)")
+                    help="reduction (default sum; nvls is sum-only, -a uses two-shot for the others; "
+                         "band bor bxor land lor lxor take integer types only)")
     args = ap.parse_args(argv)
     op = reduce_op(args.op)
+    check_op_type(op, args.type)
     comm = Comm()
     device = comm.device   # chosen before the process group was bound to it (Comm.pick_device)
     algo = args.algo
