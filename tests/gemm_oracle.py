@@ -15,6 +15,8 @@ should round, still matches them.  The data here uses every mantissa bit the acc
                           ``bf16_shard_bound`` the bound used above four ranks, where the P! orders are too many.
 * ``activation_bound``    per-element bounds of the fused epilogue activations against the fp64 activation of the
                           exact C, from the documented error of the approximations the kernel uses.
+* ``mlp_exact_operands``  the operands of a relu MLP block whose two chained GEMMs are both exact in fp32 in any order
+                          (``mlp_down_bits`` counts the bits of the second one).
 * ``general_bound``       a deliberately loose bound for random operands: it admits a truncating fp32 accumulator.
 """
 from __future__ import annotations
@@ -193,6 +195,33 @@ def activation_bound(c: torch.Tensor, activation: str) -> Tuple[torch.Tensor, to
         bound = torch.where(x < SILU_OVERFLOW, want.abs() * (1 + rel), bound)
         return want, bound
     raise ValueError(activation)
+
+
+def mlp_down_bits(hidden: int, ffn: int, p_up: int, p_down: int) -> int:
+    """Bits that the largest partial sum of the second GEMM of a relu MLP block needs on ``mlp_exact_operands`` data.
+
+    Row i of x has exponent e_i and every row of w_up exponent 0, all with ``p_up`` bits: every product of row i of
+    the first GEMM is a multiple of g_i = 2^(e_i - 2(p_up-1)) and |C| < 4 hidden 2^e_i.  bf16 keeps such a multiple
+    exactly below 2^8 g_i and rounds it to a multiple of 2 g_i or more above, never beyond the power of two above, so
+    every hidden value h is a multiple of g_i with |h| / g_i <= 2^(2 + log2 hidden + 2(p_up-1)).  Row n of w_down has
+    one exponent d_n over the whole ffn axis and ``p_down`` bits: |w| / 2^(d_n - (p_down-1)) < 2^p_down.  So every
+    term h w of output (i, n), on every rank, is a multiple of G = g_i 2^(d_n - (p_down-1)) below 2^(that sum) G, and a
+    partial sum of up to ffn terms, in any order and grouping (each rank's K-slice, then the P shard additions), stays
+    a multiple of G below 2^bits G: exact in fp32 when bits <= 24."""
+    return (math.ceil(math.log2(ffn)) + 2 + math.ceil(math.log2(hidden)) + 2 * (p_up - 1) + p_down)
+
+
+def mlp_exact_operands(tokens: int, hidden: int, ffn: int, seed: int, *, p_up: int = 2, p_down: int = 3,
+                       device="cpu") -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """bf16 x ``[tokens, hidden]``, w_up ``[ffn, hidden]``, w_down ``[hidden, ffn]`` of a relu MLP block whose two
+    GEMMs are exact in fp32 in any order (``mlp_down_bits`` <= 24): the block output equals the fp64 product of the
+    hidden values bit for bit.  Rank r holds rows r of x, row block r of w_up and column block r of w_down.  Exponents
+    stay within +-2 per row, so every product and sum is a normal fp32 value."""
+    if mlp_down_bits(hidden, ffn, p_up, p_down) > FP32_BITS:
+        raise ValueError(f"hidden = {hidden}, ffn = {ffn}, p = {p_up}, {p_down}: the second GEMM needs more than 24 bits")
+    x, w_up = exact_operands(tokens, ffn, hidden, seed, p=p_up, a_exp=(-2, 2), b_exp=(0, 0), device=device)
+    w_down = exact_operands(hidden, 1, ffn, seed + 1, p=p_down, a_exp=(-2, 2), device=device)[0]
+    return x, w_up, w_down
 
 
 def general_bound(a: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -173,6 +173,41 @@ def test_parallel_mlp_chains_the_layers(fakes):
     mlp.close()
 
 
+def test_layers_take_buffers_from_the_caller(fakes):
+    """``_shared``: the buffers of virtual ranks made by a LocalGroup are used as given, nothing else is allocated;
+    ParallelMLP hands its ``ctas`` and ``_shared`` parts to both layers."""
+    rec, ops = fakes
+    comm = FakeComm(1, 2)
+    pads = [tp.SignalPads(comm, 0) for _ in range(4)]
+    shard = FakeSymmetricBuffer(comm, 256 * 512 * 4, 0)
+    a = FakeSymmetricBuffer(comm, 512 * 256 * 2, 0)
+    before = FakeSymmetricBuffer.base
+    row = tp.RowParallelLinear(comm, 0, m=512, n=512, k_local=64, _shared={"pads": pads[0], "shard": shard})
+    col = tp.ColumnParallelLinear(comm, 0, m=512, n_local=256, k=256, _shared={"pads": pads[1], "a": a})
+    assert FakeSymmetricBuffer.base == before
+    assert row.pads is pads[0] and row.shard is shard and row.y.data_ptr() == shard.tensor().data_ptr()
+    assert col.pads is pads[1] and col.a is a and col.a_full.data_ptr() == a.tensor().data_ptr()
+    row.forward(torch.zeros(512, 64, dtype=torch.bfloat16))
+    assert ops[-1][1][2] == shard.ptrs and pads[0].ticket_issued == 148
+    col.forward(torch.zeros(256, 256, dtype=torch.bfloat16))
+    assert ops[-1][1][1] == [a.ptrs[q] + q * 256 * 256 * 2 for q in range(2)] and pads[1].ticket_issued == 146
+    with pytest.raises(ValueError):                              # a shard of the wrong size
+        tp.RowParallelLinear(comm, 0, m=512, n=256, k_local=64, _shared={"pads": pads[0], "shard": shard})
+    with pytest.raises(ValueError):
+        tp.RowParallelLinear(comm, 0, m=512, n=512, k_local=64, reduce="all", _shared={"pads": pads[0], "shard": shard})
+    up_a = FakeSymmetricBuffer(comm, 512 * 256 * 2, 0)
+    down_shard = FakeSymmetricBuffer(comm, 256 * 256 * 4, 0)
+    before = FakeSymmetricBuffer.base
+    mlp = tp.ParallelMLP(comm, 0, tokens=512, hidden=256, ffn=512, activation="relu", ctas=6,
+                         _shared={"up": {"pads": pads[2], "a": up_a}, "down": {"pads": pads[3], "shard": down_shard}})
+    assert FakeSymmetricBuffer.base == before
+    assert mlp.up.pads is pads[2] and mlp.up.a is up_a and mlp.down.pads is pads[3] and mlp.down.shard is down_shard
+    mlp.forward(torch.zeros(256, 256, dtype=torch.bfloat16))
+    assert [(name, k["ctas"]) for name, _, k in ops[-2:]] == [("allgather_gemm", 6), ("gemm_reduce_scatter", 6)]
+    plain = tp.ParallelMLP(comm, 0, tokens=512, hidden=256, ffn=512)           # without: own buffers, every SM
+    assert FakeSymmetricBuffer.base > before and plain.up.ctas == plain.down.ctas == 0
+
+
 def test_tp_program_end_to_end_dry(fakes, monkeypatch, capsys):
     """`python -m hpc_patterns_b200 tp --check --mlp ...` with every GPU-facing piece replaced: the whole program
     (argument handling, the three layers, the MLP block, the JSON line) runs; the numbers mean nothing."""
@@ -223,5 +258,6 @@ def test_tp_program_end_to_end_dry(fakes, monkeypatch, capsys):
     for key in ("row_parallel", "column_parallel", "mlp"):
         assert {"fused_ms", "stock_ms", "speedup"} <= set(out[key])
     assert "row_parallel_exact" in out and "column_parallel_exact" in out and "mlp_max_abs_diff" in out
+    assert isinstance(out["mlp_within_bound"], bool) and isinstance(out["mlp_hidden_exact"], bool)   # judged
     assert rc in (0, 1)                                          # the recorders compute nothing, so 'exact' is false
     assert [name for name, _, _ in ops].count("allgather_gemm") >= 3
