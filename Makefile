@@ -44,6 +44,7 @@ cli: $(CLIS) aliases
 aliases: $(CLIS)
 	@for n in allreduce.float allreduce.int allreduce.double allreduce.long allreduce.short allreduce.uint allreduce.uchar \
 	          allreduce.bfloat16 allreduce.half \
+	          allreduce.float_int allreduce.double_int allreduce.long_int allreduce.2int allreduce.short_int \
 	          allreduce-mpi-sycl.float allreduce-mpi-sycl.int \
 	          allreduce-usm-mpi-omp-offload.float allreduce-map-mpi-omp-offload.float; do ln -sf allreduce bin/$$n; done
 	@for n in halo.float halo.double halo.bfloat16 halo.half; do ln -sf halo bin/$$n; done

@@ -49,13 +49,15 @@ ElemType elem_from(const std::string& s) {
   ElemType t;
   if (elem_type_from_name(s, &t)) return t;
   throw std::invalid_argument(
-      "dtype must be one of float int uint double long ulong short ushort uchar bfloat16 half");
+      "dtype must be one of float int uint double long ulong short ushort uchar bfloat16 half, or a value-index pair "
+      "float_int double_int long_int 2int short_int");
 }
 
 ReduceOp op_from(const std::string& s) {
   ReduceOp op;
   if (reduce_op_from_name(s, &op)) return op;
-  throw std::invalid_argument("op must be one of sum prod product min max band bor bxor land lor lxor, not '" + s + "'");
+  throw std::invalid_argument("op must be one of sum prod product min max band bor bxor land lor lxor maxloc minloc, not '" +
+                              s + "'");
 }
 
 CopyTuning tuning_from(const py::dict& d) {
@@ -627,12 +629,27 @@ PYBIND11_MODULE(_C, m) {
       },
       py::arg("va"), py::arg("vc"), py::arg("n"), py::arg("dtype"), py::arg("stream"), py::arg("op") = "sum",
       "VC += VA (op=sum), else VC = op(VC, VA); op = sum | prod | product | min | max, and on integer types "
-      "band | bor | bxor | land | lor | lxor.");
+      "band | bor | bxor | land | lor | lxor; on the pair types maxloc | minloc only.");
   m.def("count_mismatch", [](uintptr_t v, size_t n, double expected, const std::string& dtype,
                              uintptr_t count, uintptr_t stream) {
     launch_count_mismatch(as_ptr<const void>(v), n, expected, elem_from(dtype),
                           as_ptr<unsigned long long>(count), as_stream(stream));
   });
+  m.def(
+      "init_pair",
+      [](uintptr_t v, size_t n, double value, int index, const std::string& dtype, uintptr_t stream) {
+        launch_init_pair(as_ptr<void>(v), n, value, index, elem_from(dtype), as_stream(stream));
+      },
+      py::arg("v"), py::arg("n"), py::arg("value"), py::arg("index"), py::arg("dtype"), py::arg("stream"),
+      "Pair types: every element of v = (value, index), padding bytes zero.");
+  m.def(
+      "count_pair_mismatch",
+      [](uintptr_t v, size_t n, double value, int index, const std::string& dtype, uintptr_t count, uintptr_t stream) {
+        launch_count_pair_mismatch(as_ptr<const void>(v), n, value, index, elem_from(dtype),
+                                   as_ptr<unsigned long long>(count), as_stream(stream));
+      },
+      py::arg("v"), py::arg("n"), py::arg("value"), py::arg("index"), py::arg("dtype"), py::arg("count"),
+      py::arg("stream"), "Pair types: adds to *count the elements of v whose bytes differ from (value, index, zero padding).");
   // Slot / flow-control rules of the fused ring (kernels/ring_order.h), exposed for the CPU protocol model.
   m.def("ring_src_slot", &ring_src_slot);
   m.def("ring_fwd_slot", &ring_fwd_slot);
@@ -736,7 +753,7 @@ PYBIND11_MODULE(_C, m) {
       py::arg("phases") = "allreduce", py::arg("op") = "sum",
       "Reduce-scatter + all-gather ring in one launch per rank (kernels/ring_order.h: rsag_*); "
       "phases = allreduce | reduce_scatter | all_gather; op = sum | prod | product | min | max, and on integer "
-      "types band | bor | bxor | land | lor | lxor.");
+      "types band | bor | bxor | land | lor | lxor; on the pair types maxloc | minloc only.");
   m.def(
       "allreduce_two_shot",
       [](const std::vector<uintptr_t>& va, const std::vector<uintptr_t>& vc,

@@ -25,13 +25,15 @@
 #include <type_traits>
 
 #include "../kernels/api.h"
+#include "cuda_check.h"
 
 namespace hpcp {
 
 struct DTypeInfo {
   const char* name;      // "float", "int", ... ; "bytes" for opaque types
   size_t size;           // sizeof(T)
-  bool reducible;        // has a SUM kernel in this suite
+  bool reducible;        // has reduction kernels in this suite: SUM for the arithmetic types, maxloc / minloc only
+                         // for the value-index pair types
   ElemType elem;         // valid iff reducible
   const char* torch;     // matching torch dtype name, "" if none
 };
@@ -60,6 +62,26 @@ HPCP_DTYPE(unsigned short, "unsigned short", true, ElemType::kUShort, "uint16");
 HPCP_DTYPE(unsigned char, "unsigned char", true, ElemType::kUChar, "uint8");
 HPCP_DTYPE(__nv_bfloat16, "bfloat16", true, ElemType::kBFloat16, "bfloat16");
 HPCP_DTYPE(__half, "half", true, ElemType::kHalf, "float16");
+
+// The value-index pairs of MPI_MAXLOC / MPI_MINLOC (↔ MPI_FLOAT_INT, MPI_DOUBLE_INT, MPI_LONG_INT, MPI_2INT,
+// MPI_SHORT_INT): the C struct {value; int index;} in its natural layout, the same on the host and the device.  The
+// padding (after a short value, after the index of a 16-byte pair) is zero in every pair a combine produces.
+template <typename V>
+struct LocPair {
+  using value_type = V;
+  V value;
+  int index;
+};
+static_assert(sizeof(LocPair<float>) == 8 && offsetof(LocPair<float>, index) == 4, "float_int layout");
+static_assert(sizeof(LocPair<double>) == 16 && offsetof(LocPair<double>, index) == 8, "double_int layout");
+static_assert(sizeof(LocPair<long long>) == 16 && offsetof(LocPair<long long>, index) == 8, "long_int layout");
+static_assert(sizeof(LocPair<int>) == 8 && offsetof(LocPair<int>, index) == 4, "2int layout");
+static_assert(sizeof(LocPair<short>) == 8 && offsetof(LocPair<short>, index) == 4, "short_int layout");
+HPCP_DTYPE(LocPair<float>, "float_int", true, ElemType::kFloatInt, "");
+HPCP_DTYPE(LocPair<double>, "double_int", true, ElemType::kDoubleInt, "");
+HPCP_DTYPE(LocPair<long long>, "long_int", true, ElemType::kLongInt, "");
+HPCP_DTYPE(LocPair<int>, "2int", true, ElemType::kTwoInt, "");
+HPCP_DTYPE(LocPair<short>, "short_int", true, ElemType::kShortInt, "");
 #undef HPCP_DTYPE
 
 template <typename T>
@@ -90,6 +112,8 @@ inline bool elem_type_from_name(const std::string& name, ElemType* out) {
       {"bfloat16", ElemType::kBFloat16}, {"bf16", ElemType::kBFloat16},
       {"half", ElemType::kHalf},      {"float16", ElemType::kHalf},        {"f16", ElemType::kHalf},
       {"fp16", ElemType::kHalf},
+      {"float_int", ElemType::kFloatInt}, {"double_int", ElemType::kDoubleInt}, {"long_int", ElemType::kLongInt},
+      {"2int", ElemType::kTwoInt},    {"int_int", ElemType::kTwoInt},      {"short_int", ElemType::kShortInt},
   };
   for (const Row& r : rows)
     if (name == r.name) {
@@ -111,11 +135,21 @@ inline const char* elem_type_name(ElemType t) {
     case ElemType::kUChar: return "uchar";
     case ElemType::kBFloat16: return "bfloat16";
     case ElemType::kHalf: return "half";
+    case ElemType::kFloatInt: return "float_int";
+    case ElemType::kDoubleInt: return "double_int";
+    case ElemType::kLongInt: return "long_int";
+    case ElemType::kTwoInt: return "2int";
+    case ElemType::kShortInt: return "short_int";
   }
   return "?";
 }
 
-// Run f(T{}) with the C++ type of `t`.
+inline bool elem_type_is_pair(ElemType t) {
+  return t == ElemType::kFloatInt || t == ElemType::kDoubleInt || t == ElemType::kLongInt || t == ElemType::kTwoInt ||
+         t == ElemType::kShortInt;
+}
+
+// Run f(T{}) with the C++ type of `t`, one of the eleven arithmetic types; a pair type is refused (dispatch_pair).
 template <typename F>
 void dispatch_elem(ElemType t, F&& f) {
   switch (t) {
@@ -130,6 +164,25 @@ void dispatch_elem(ElemType t, F&& f) {
     case ElemType::kUChar: f(static_cast<unsigned char>(0)); break;
     case ElemType::kBFloat16: f(__nv_bfloat16{}); break;
     case ElemType::kHalf: f(__half{}); break;
+    case ElemType::kFloatInt:
+    case ElemType::kDoubleInt:
+    case ElemType::kLongInt:
+    case ElemType::kTwoInt:
+    case ElemType::kShortInt:
+      HPCP_FAIL(std::string(elem_type_name(t)) + " is a value-index pair type: only maxloc and minloc reduce it");
+  }
+}
+
+// Run f(LocPair<V>{}) with the pair struct of `t`; an arithmetic type is refused.
+template <typename F>
+void dispatch_pair(ElemType t, F&& f) {
+  switch (t) {
+    case ElemType::kFloatInt: f(LocPair<float>{}); break;
+    case ElemType::kDoubleInt: f(LocPair<double>{}); break;
+    case ElemType::kLongInt: f(LocPair<long long>{}); break;
+    case ElemType::kTwoInt: f(LocPair<int>{}); break;
+    case ElemType::kShortInt: f(LocPair<short>{}); break;
+    default: HPCP_FAIL(std::string(elem_type_name(t)) + " is not a value-index pair type");
   }
 }
 
@@ -150,7 +203,8 @@ void dispatch_add_class(ElemType t, F&& f) {
 template <typename T>
 constexpr bool kSum16InF32 = std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value;
 
-// Reduction by name: sum, prod (or product), min, max, band, bor, bxor, land, lor, lxor; false if unknown.
+// Reduction by name: sum, prod (or product), min, max, band, bor, bxor, land, lor, lxor, maxloc, minloc; false if
+// unknown.
 inline bool reduce_op_from_name(const std::string& name, ReduceOp* out) {
   if (name == "sum") *out = ReduceOp::kSum;
   else if (name == "prod" || name == "product") *out = ReduceOp::kProd;
@@ -162,6 +216,8 @@ inline bool reduce_op_from_name(const std::string& name, ReduceOp* out) {
   else if (name == "land") *out = ReduceOp::kLAnd;
   else if (name == "lor") *out = ReduceOp::kLOr;
   else if (name == "lxor") *out = ReduceOp::kLXor;
+  else if (name == "maxloc") *out = ReduceOp::kMaxLoc;
+  else if (name == "minloc") *out = ReduceOp::kMinLoc;
   else return false;
   return true;
 }
@@ -177,6 +233,8 @@ inline const char* reduce_op_name(ReduceOp op) {
     case ReduceOp::kLAnd: return "land";
     case ReduceOp::kLOr: return "lor";
     case ReduceOp::kLXor: return "lxor";
+    case ReduceOp::kMaxLoc: return "maxloc";
+    case ReduceOp::kMinLoc: return "minloc";
   }
   return "?";
 }
@@ -187,10 +245,25 @@ inline bool reduce_op_integer_only(ReduceOp op) {
          op == ReduceOp::kLOr || op == ReduceOp::kLXor;
 }
 inline bool elem_type_is_integer(ElemType t) {
-  return t != ElemType::kFloat && t != ElemType::kDouble && t != ElemType::kBFloat16 && t != ElemType::kHalf;
+  return t != ElemType::kFloat && t != ElemType::kDouble && t != ElemType::kBFloat16 && t != ElemType::kHalf &&
+         !elem_type_is_pair(t);
 }
-// The refusal of an integer-only op on a floating type, the same words in every layer.
+// maxloc and minloc reduce the pair types only, and they are the only ops that do.
+inline bool reduce_op_on_pairs(ReduceOp op) { return op == ReduceOp::kMaxLoc || op == ReduceOp::kMinLoc; }
+// Whether `op` reduces `t`.
+inline bool reduce_op_takes(ReduceOp op, ElemType t) {
+  if (elem_type_is_pair(t) || reduce_op_on_pairs(op)) return elem_type_is_pair(t) && reduce_op_on_pairs(op);
+  return !reduce_op_integer_only(op) || elem_type_is_integer(t);
+}
+// The refusal of an op that does not reduce a type (reduce_op_takes), the same words in every layer.
 inline std::string reduce_op_type_error(ReduceOp op, ElemType t) {
+  if (elem_type_is_pair(t))
+    return std::string("op must be maxloc or minloc for ") + elem_type_name(t) + ": " + reduce_op_name(op) +
+           " reduces arithmetic types only";
+  if (reduce_op_on_pairs(op))
+    return std::string("op must be ") +
+           (elem_type_is_integer(t) ? "sum, prod, min, max, band, bor, bxor, land, lor or lxor" : "sum, prod, min or max") +
+           " for " + elem_type_name(t) + ": " + reduce_op_name(op) + " reduces value-index pair types only";
   return std::string("op must be sum, prod, min or max for ") + elem_type_name(t) + ": " + reduce_op_name(op) +
          " reduces integer types only";
 }

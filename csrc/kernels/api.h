@@ -109,12 +109,16 @@ void launch_verify_triad(const float* a, size_t n, int src_rank, float s,
 // the two's-complement add.  kBFloat16 / kHalf (↔ MPICH's MPIX_C_BF16 / MPIX_C_FLOAT16) add with one round-to-nearest-even
 // per add in the 16-bit format (rings), or accumulate in fp32 and round once (two-shot).  kFloat, kDouble, kBFloat16 and
 // kHalf are also the field types of the halo stencil below.
+// The pair types kFloatInt ... kShortInt (↔ MPI_FLOAT_INT, MPI_DOUBLE_INT, MPI_LONG_INT, MPI_2INT, MPI_SHORT_INT) are the
+// C structs {value; int index;} in their natural layout (LocPair, dtype_traits.h); only maxloc and minloc reduce them.
 enum class ElemType : int {
   kFloat = 0, kInt = 1, kUInt = 2, kDouble = 3, kLong = 4, kULong = 5, kShort = 6, kUShort = 7, kUChar = 8,
-  kBFloat16 = 9, kHalf = 10
+  kBFloat16 = 9, kHalf = 10, kFloatInt = 11, kDoubleInt = 12, kLongInt = 13, kTwoInt = 14, kShortInt = 15
 };
 constexpr size_t elem_size(ElemType t) {
-  return t == ElemType::kDouble || t == ElemType::kLong || t == ElemType::kULong ? 8
+  return t == ElemType::kDoubleInt || t == ElemType::kLongInt                                        ? 16
+         : t == ElemType::kDouble || t == ElemType::kLong || t == ElemType::kULong ||
+                   t == ElemType::kFloatInt || t == ElemType::kTwoInt || t == ElemType::kShortInt ? 8
          : t == ElemType::kShort || t == ElemType::kUShort || t == ElemType::kBFloat16 || t == ElemType::kHalf ? 2
          : t == ElemType::kUChar                                                 ? 1
                                                                                  : 4;
@@ -304,8 +308,11 @@ void launch_wait_flags(const uint32_t* flags, int count, uint32_t epoch, uint64_
 // ------------------------------------------------------ allreduce miniapp ----
 // The reduction of an allreduce (↔ MPI_SUM / MPI_PROD / MPI_MIN / MPI_MAX, and on the integer types MPI_BAND / MPI_BOR
 // / MPI_BXOR / MPI_LAND / MPI_LOR / MPI_LXOR).  kSum accumulates into VC as the reference does; the other ops overwrite
-// VC (docs/allreduce.md has their semantics per type).  NVLS is sum-only.
-enum class ReduceOp : int { kSum = 0, kProd = 1, kMin = 2, kMax = 3, kBAnd = 4, kBOr, kBXor, kLAnd, kLOr, kLXor };
+// VC (docs/allreduce.md has their semantics per type).  NVLS is sum-only.  kMaxLoc / kMinLoc (↔ MPI_MAXLOC /
+// MPI_MINLOC) reduce the pair types only, and the pair types take no other op.
+enum class ReduceOp : int {
+  kSum = 0, kProd = 1, kMin = 2, kMax = 3, kBAnd = 4, kBOr, kBXor, kLAnd, kLOr, kLXor, kMaxLoc, kMinLoc
+};
 
 // VA = a, VB = b, VC = c (↔ Initialize, allreduce-mpi-sycl.cpp:33-41). Any pointer may be null.
 void launch_init3(void* va, void* vb, void* vc, size_t n, double a, double b, double c,
@@ -316,6 +323,11 @@ void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaSt
 // Counts elements with |v - expected| >= 1e-6 (↔ the assert loop, :192-204).
 void launch_count_mismatch(const void* v, size_t n, double expected, ElemType type,
                            unsigned long long* count, cudaStream_t stream);
+// Pair types: every element of v = (value, index) with zero padding bytes; and the count of elements whose bytes differ
+// from that pair (padding included).
+void launch_init_pair(void* v, size_t n, double value, int index, ElemType type, cudaStream_t stream);
+void launch_count_pair_mismatch(const void* v, size_t n, double value, int index, ElemType type,
+                                unsigned long long* count, cudaStream_t stream);
 
 // Fused ring "rotate + accumulate" allreduce: all P-1 exchange steps and all P
 // accumulations in ONE launch per rank.  Hop t of chunk c is read once, added

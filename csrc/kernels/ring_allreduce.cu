@@ -29,6 +29,7 @@
 #include "ring_allreduce.cuh"
 
 #include <cstdlib>
+#include <cstring>
 #include <initializer_list>
 
 namespace hpcp {
@@ -74,6 +75,39 @@ __global__ void count_mismatch_kernel(const T* __restrict__ v, size_t n, double 
   }
   for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(count, bad);
+}
+
+// Pair types: W is the pair's bytes as one 8- or 16-byte word (uint2 / uint4), padding included.
+template <typename W>
+__global__ void fill_pair_kernel(W* v, size_t n, W pair) {
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) v[i] = pair;
+}
+__device__ __forceinline__ bool same_bits(uint2 a, uint2 b) { return a.x == b.x && a.y == b.y; }
+__device__ __forceinline__ bool same_bits(uint4 a, uint4 b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
+template <typename W>
+__global__ void count_pair_mismatch_kernel(const W* __restrict__ v, size_t n, W pair, unsigned long long* count) {
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  unsigned long long bad = 0;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+    bad += !same_bits(__ldcg(v + i), pair);
+  for (int off = 16; off > 0; off >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, off);
+  if ((threadIdx.x & 31) == 0 && bad) atomicAdd(count, bad);
+}
+// f(W{}, pair bits) for the pair (value, index) of `type`, padding zero.
+template <typename F>
+void with_pair_bits(ElemType type, double value, int index, F&& f) {
+  dispatch_pair(type, [&](auto tag) {
+    using P = decltype(tag);
+    using W = std::conditional_t<sizeof(P) == 16, uint4, uint2>;
+    P p;
+    std::memset(static_cast<void*>(&p), 0, sizeof p);
+    p.value = static_cast<typename P::value_type>(value);
+    p.index = index;
+    W w;
+    std::memcpy(&w, &p, sizeof w);
+    f(w);
+  });
 }
 
 // -------------------------------------------------------------------- NVLS ----
@@ -133,9 +167,11 @@ int env_choice(const char* name, std::initializer_list<int> allowed, int fallbac
   return fallback;
 }
 
-// The kernels of (type, op): the sum's are instantiated here, the other ops' in ring_allreduce_ops.cu.
+// The kernels of (type, op): the sum's are instantiated here, the other ops' in ring_allreduce_ops.cu.  The pair types
+// have no sum: refused with the words of dispatch_op.
 AllreduceKernels allreduce_kernels(ElemType type, ReduceOp op) {
   if (op != ReduceOp::kSum) return op_allreduce_kernels(type, op);
+  HPCP_REQUIRE(reduce_op_takes(op, type), reduce_op_type_error(op, type));
   AllreduceKernels k{};
   dispatch_add_class(type, [&](auto tag) { k = allreduce_kernels_of<SumOp<decltype(tag)>, false, false>(); });
   return k;
@@ -189,6 +225,7 @@ void launch_accumulate(const void* va, void* vc, size_t n, ElemType type, cudaSt
     launch_512(op_combine_kernel(type, op), ctas, stream, va_v, vc_v, nvec, va_tail, vc_tail, tail * elem_size(type));
     return;
   }
+  HPCP_REQUIRE(reduce_op_takes(op, type), reduce_op_type_error(op, type));
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     accumulate_kernel<T><<<ctas, 512, 0, stream>>>(static_cast<const uint4*>(va), static_cast<uint4*>(vc), nvec,
@@ -204,6 +241,25 @@ void launch_count_mismatch(const void* v, size_t n, double expected, ElemType ty
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     count_mismatch_kernel<T><<<ctas, 256, 0, stream>>>(static_cast<const T*>(v), n, expected, count);
+  });
+  HPCP_CUDA(cudaGetLastError());
+}
+
+void launch_init_pair(void* v, size_t n, double value, int index, ElemType type, cudaStream_t stream) {
+  const int ctas = grid_for(n, 256, 132 * 8);
+  with_pair_bits(type, value, index, [&](auto w) {
+    using W = decltype(w);
+    fill_pair_kernel<W><<<ctas, 256, 0, stream>>>(static_cast<W*>(v), n, w);
+  });
+  HPCP_CUDA(cudaGetLastError());
+}
+
+void launch_count_pair_mismatch(const void* v, size_t n, double value, int index, ElemType type,
+                                unsigned long long* count, cudaStream_t stream) {
+  const int ctas = grid_for(n, 256, 132 * 8);
+  with_pair_bits(type, value, index, [&](auto w) {
+    using W = decltype(w);
+    count_pair_mismatch_kernel<W><<<ctas, 256, 0, stream>>>(static_cast<const W*>(v), n, w, count);
   });
   HPCP_CUDA(cudaGetLastError());
 }
@@ -276,8 +332,14 @@ void launch_ring_rsag(const RingRsAgArgs& args, ElemType type, int ctas, int dev
   d.epoch_base = args.epoch_base;
   d.timeout_ns = args.timeout_ns;
   d.status = args.status;
-  // The all-gather phase only copies: every op shares the sum's kernel there.
-  const void* kernel = allreduce_kernels(type, args.phases == kRsAgAllGather ? ReduceOp::kSum : args.op).rsag;
+  // The all-gather phase only copies: every op shares the sum's kernel there, and a pair type (which has no sum) the one
+  // of int: the body moves whole 16-byte vectors whatever the type.  The op is still checked against a pair type and
+  // for maxloc / minloc, as in the other phases; the arithmetic types keep ignoring it there.
+  const bool gather = args.phases == kRsAgAllGather;
+  HPCP_REQUIRE(!gather || !(elem_type_is_pair(type) || reduce_op_on_pairs(args.op)) || reduce_op_takes(args.op, type),
+               reduce_op_type_error(args.op, type));
+  const ElemType ktype = gather && elem_type_is_pair(type) ? ElemType::kInt : type;
+  const void* kernel = allreduce_kernels(ktype, gather ? ReduceOp::kSum : args.op).rsag;
   launch_512(kernel, ring_grid(kernel, d.n_chunks, ctas, device), stream, d);
 }
 

@@ -1,6 +1,6 @@
 // Allreduce kernels for the reductions other than the sum: prod, min and max (↔ MPI_PROD / MPI_MIN / MPI_MAX), and on
 // the integer types band, bor, bxor, land, lor and lxor (↔ MPI_BAND / MPI_BOR / MPI_BXOR / MPI_LAND / MPI_LOR /
-// MPI_LXOR).
+// MPI_LXOR), and on the value-index pair types maxloc and minloc (↔ MPI_MAXLOC / MPI_MINLOC).
 //
 // They are the kernel templates of ring_allreduce.cuh, the ones the sum runs, instantiated with another combine policy:
 // the same loads, stores, arrival / ack words and barriers, in the same combine order.  Two differences on purpose:
@@ -13,6 +13,9 @@
 //               product to nearest even without FTZ; two-shot multiplies the 16-bit types in fp32 and rounds once;
 //   band / bor / bxor   &, |, ^ of the element bits, whatever the width and signedness (one kernel set for all);
 //   land / lor / lxor   an element is true iff it is nonzero over its whole width; the result is 0 or 1 of the type.
+//   maxloc / minloc     the pair whose value is largest / smallest wins; bit-equal values (or two NaNs) take the smaller
+//               signed index.  Values compare signed; floats in max / min's order (-0 < +0, a NaN value wins in both);
+//               the padding bytes of a result are zero.
 // A NaN result is the type's canonical quiet NaN (all bits set but the sign), the same bits on every rank.
 #include "ring_allreduce.cuh"
 
@@ -278,6 +281,76 @@ template <typename C> struct LAnd : LanesOf<C, LogicW<C, LAndF>> {};
 template <typename C> struct LOr : LanesOf<C, LogicW<C, LOrF>> {};
 template <typename C> struct LXor : LanesOf<C, LogicW<C, LXorF>> {};
 
+// ------------------------------------------------------- maxloc / minloc ----
+// Exact, commutative and associative: a pair's rank is (key of its value, then -index) for maxloc and (key, index) for
+// minloc, and the combine returns the better pair, so every combine order selects the same one.  key() is an unsigned
+// integer in the order of the values (a NaN value at the top for maxloc, at the bottom for minloc: it wins in both, all
+// NaNs tie); canon() is the value's bits as a result stores them (the canonical NaN; a short's upper half zero).
+template <typename V> struct LocValue;
+template <> struct LocValue<int> {
+  using W = uint32_t;
+  template <bool kMax> static __device__ __forceinline__ W key(W v) { return v ^ 0x80000000u; }
+  static __device__ __forceinline__ W canon(W v) { return v; }
+};
+template <> struct LocValue<short> {  // the low half of the word, sign-extended for the compare
+  using W = uint32_t;
+  template <bool kMax> static __device__ __forceinline__ W key(W v) { return (v & 0xffffu) ^ 0x8000u; }
+  static __device__ __forceinline__ W canon(W v) { return v & 0xffffu; }
+};
+template <> struct LocValue<long long> {
+  using W = unsigned long long;
+  template <bool kMax> static __device__ __forceinline__ W key(W v) { return v ^ 0x8000000000000000ull; }
+  static __device__ __forceinline__ W canon(W v) { return v; }
+};
+// IEEE bits -> a key in their total order (negative values reversed below the positive ones, -0 just below +0).
+template <typename W, W kSign, W kInf, W kNaN>
+struct LocFloat {
+  static __device__ __forceinline__ bool nan(W v) { return (v & ~kSign) > kInf; }
+  template <bool kMax> static __device__ __forceinline__ W key(W v) {
+    return nan(v) ? (kMax ? ~W{0} : W{0}) : (v & kSign) ? ~v : v | kSign;
+  }
+  static __device__ __forceinline__ W canon(W v) { return nan(v) ? kNaN : v; }
+};
+template <> struct LocValue<float> : LocFloat<uint32_t, 0x80000000u, 0x7f800000u, kNaN32> {
+  using W = uint32_t;
+};
+template <> struct LocValue<double>
+    : LocFloat<unsigned long long, 0x8000000000000000ull, 0x7ff0000000000000ull, kNaN64> {
+  using W = unsigned long long;
+};
+
+// a o b on one pair: true if a is the result (the better key, or the same key and the smaller or equal index).
+template <typename V, bool kMax>
+__device__ __forceinline__ bool loc_takes_a(typename LocValue<V>::W va, uint32_t ia, typename LocValue<V>::W vb,
+                                            uint32_t ib) {
+  const auto ka = LocValue<V>::template key<kMax>(va), kb = LocValue<V>::template key<kMax>(vb);
+  return (kMax ? ka > kb : ka < kb) || (ka == kb && static_cast<int>(ia) <= static_cast<int>(ib));
+}
+// The 8-byte pairs, two per vector: value in x / z, index in y / w.
+template <typename V, bool kMax>
+struct Loc8 {
+  static __device__ __forceinline__ uint4 combine(const uint4& a, const uint4& b) {
+    const bool lo = loc_takes_a<V, kMax>(a.x, a.y, b.x, b.y), hi = loc_takes_a<V, kMax>(a.z, a.w, b.z, b.w);
+    return make_uint4(LocValue<V>::canon(lo ? a.x : b.x), lo ? a.y : b.y, LocValue<V>::canon(hi ? a.z : b.z),
+                      hi ? a.w : b.w);
+  }
+};
+// The 16-byte pairs, one per vector: value in (x, y), index in z, padding in w.
+template <typename V, bool kMax>
+struct Loc16 {
+  static __device__ __forceinline__ uint4 combine(const uint4& a, const uint4& b) {
+    const bool t = loc_takes_a<V, kMax>(lane64(a.x, a.y), a.z, lane64(b.x, b.y), b.z);
+    const unsigned long long v = LocValue<V>::canon(t ? lane64(a.x, a.y) : lane64(b.x, b.y));
+    return make_uint4(static_cast<uint32_t>(v), static_cast<uint32_t>(v >> 32), t ? a.z : b.z, 0u);
+  }
+};
+template <typename P, bool kMax>
+using LocOf = std::conditional_t<sizeof(P) == 16, Loc16<typename P::value_type, kMax>,
+                                 Loc8<typename P::value_type, kMax>>;
+// P = LocPair<V> (dtype_traits.h).
+template <typename P> struct MaxLoc : LocOf<P, true> {};
+template <typename P> struct MinLoc : LocOf<P, false> {};
+
 // ---------------------------------------------------------------- kernels ----
 // VC = op(VC, VA) over whole vectors; block 0's thread 0 combines the last partial vector in registers and writes back
 // only its tail_bytes.
@@ -313,10 +386,22 @@ void dispatch_bit_op(ReduceOp op, F& f) {
   }
 }
 
-// Run f(Op{}) with the combine policy of (type, op).  The bitwise and logical ops are refused for the floating types
-// here, before any kernel is chosen, as MPI refuses them.
+// Run f(Op{}) with the combine policy of (type, op).  An op that does not reduce the type (the bitwise and logical ops
+// on the floating types, maxloc / minloc on any but the pair types, any other op on those) is refused here, before any
+// kernel is chosen, as MPI refuses it.
 template <typename F>
 void dispatch_op(ElemType type, ReduceOp op, F&& f) {
+  HPCP_REQUIRE(reduce_op_takes(op, type), reduce_op_type_error(op, type));
+  if (elem_type_is_pair(type)) {
+    dispatch_pair(type, [&](auto tag) {
+      using P = decltype(tag);
+      if (op == ReduceOp::kMaxLoc)
+        f(MaxLoc<P>{});
+      else
+        f(MinLoc<P>{});
+    });
+    return;
+  }
   dispatch_elem(type, [&](auto tag) {
     using T = decltype(tag);
     switch (op) {

@@ -32,6 +32,12 @@
 // every P >= 2: band (255 - 2^(r mod 4)) -> 256 - 2^min(P,4), bor (2^(r mod 4)) -> 2^min(P,4) - 1, bxor (128 on rank 0,
 // r elsewhere) -> 128 ^ 1 ^ ... ^ (P-1), land (r+1) -> 1, lor (2(r mod 2)) -> 1, lxor (3 on rank 0, else 0) -> 1; at
 // P = 1 VC is VA.
+// On the value-index pair types only (--type float_int|double_int|long_int|2int|short_int or allreduce.<pair type>, ↔
+// MPI_MAXLOC / MPI_MINLOC on MPI_FLOAT_INT ...): maxloc (the default op there) and minloc, same rules; any other op on a
+// pair type, and maxloc / minloc on any other type, is a usage error.  Their check is exact bytes, padding included:
+// maxloc (rank 0 holds (0, -P-10), rank r (1, 2r-3), VC starts at (7, -1000)) -> (1, -1), minloc with the values 1 and 0
+// (VC (-7, -1000)) -> (0, -1); at P = 1 VC is VA.  A tie broken towards the larger index, an unsigned index compare, a
+// selection by index alone and a kernel that reads VC each give another pair.
 #include <cuda_profiler_api.h>
 #include <getopt.h>
 
@@ -67,6 +73,7 @@ struct Config {
   AllocKind kind = AllocKind::kDevice;
   ElemType type = ElemType::kFloat;
   ReduceOp op = ReduceOp::kSum;
+  bool op_given = false;  // no --op: sum, or maxloc on a pair type
   std::string algo = "ring";
   std::string coll = "auto";
   int iters = 5;
@@ -102,7 +109,8 @@ void print_help() {
                "                       cudaProfilerStart/Stop: use with `ncu --profile-from-start off`\n"
                " -n N        ranks (one host thread + one GPU each; default: all GPUs;\n"
                "             more ranks than GPUs are placed round-robin)\n"
-               " --type T   element type: float int uint double long ulong short ushort uchar bfloat16 half\n"
+               " --type T   element type: float int uint double long ulong short ushort uchar bfloat16 half,\n"
+               "            or a value-index pair: float_int double_int long_int 2int short_int\n"
                "            (default float, or binary-name suffix)\n"
                " --algo ring|ring-unfused|ring-rsag   fused persistent ring kernel (default),\n"
                "                            separate put + accumulate kernels per step, or the\n"
@@ -110,6 +118,7 @@ void print_help() {
                " --coll auto|nvls|twoshot   collective used with -a\n"
                " --op sum|prod|min|max      reduction (default sum; nvls is sum-only, -a uses two-shot for the others)\n"
                "    |band|bor|bxor|land|lor|lxor   bitwise and logical reductions: integer types only\n"
+               "    |maxloc|minloc   value-index reductions: pair types only (their default op is maxloc)\n"
                " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
                " --ctas N --chunk N    kernel tuning (CTAs per rank, elements per ring chunk)\n"
                " --pull                fused ring, receiver-driven: every block is LOADED from the left neighbour's\n"
@@ -223,6 +232,8 @@ double op_input(ReduceOp op, int r, int P) {
     case ReduceOp::kLAnd: return r + 1;
     case ReduceOp::kLOr: return 2 * (r % 2);
     case ReduceOp::kLXor: return r == 0 ? 3 : 0;
+    case ReduceOp::kMaxLoc:
+    case ReduceOp::kMinLoc: break;  // pairs: loc_input
   }
   return 0;
 }
@@ -241,6 +252,8 @@ double op_expected(ReduceOp op, int P) {
     case ReduceOp::kLAnd: return 1;
     case ReduceOp::kLOr: return P >= 2 ? 1 : 0;
     case ReduceOp::kLXor: return P >= 2 ? 1 : 3;  // one rank: VC is VA, unnormalised
+    case ReduceOp::kMaxLoc:
+    case ReduceOp::kMinLoc: break;  // pairs: loc_expected
   }
   return 0;
 }
@@ -256,14 +269,109 @@ double op_vc_init(ReduceOp op, int P) {
     default: return 0;
   }
 }
+// The constant-data check of maxloc / minloc: (value, index) of rank r, of the result and of VC before the run.
+struct LocDatum {
+  double value;
+  int index;
+};
+LocDatum loc_input(ReduceOp op, int r, int P) {
+  const bool mx = op == ReduceOp::kMaxLoc;
+  return r == 0 ? LocDatum{mx ? 0.0 : 1.0, -P - 10} : LocDatum{mx ? 1.0 : 0.0, 2 * r - 3};
+}
+LocDatum loc_expected(ReduceOp op, int P) {
+  return P == 1 ? loc_input(op, 0, 1) : LocDatum{op == ReduceOp::kMaxLoc ? 1.0 : 0.0, -1};
+}
+LocDatum loc_vc_init(ReduceOp op) { return {op == ReduceOp::kMaxLoc ? 7.0 : -7.0, -1000}; }
+
+// The pair with padding bytes zero.
+template <typename V>
+LocPair<V> host_pair(double value, int index) {
+  LocPair<V> p;
+  std::memset(static_cast<void*>(&p), 0, sizeof p);
+  p.value = static_cast<V>(value);
+  p.index = index;
+  return p;
+}
+// maxloc / minloc with the kernels' rules: the larger (maxloc) or smaller (minloc) value wins, a NaN value wins in both,
+// -0 < +0; bit-equal values or two NaNs take the smaller signed index; the result has zero padding and a canonical NaN.
+template <typename V>
+LocPair<V> host_combine(ReduceOp op, LocPair<V> a, LocPair<V> b) {
+  const bool mx = op == ReduceOp::kMaxLoc;
+  int better = 0;  // > 0: a's value wins, < 0: b's, 0: a tie
+  if constexpr (std::is_floating_point<V>::value) {
+    const bool na = std::isnan(a.value), nb = std::isnan(b.value);
+    if (na || nb)
+      better = na == nb ? 0 : na ? 1 : -1;
+    else if (a.value != b.value || std::signbit(a.value) != std::signbit(b.value))
+      better = ((a.value > b.value || (a.value == b.value && std::signbit(b.value))) == mx) ? 1 : -1;
+  } else {
+    if (a.value != b.value) better = ((a.value > b.value) == mx) ? 1 : -1;
+  }
+  const LocPair<V>& w = better > 0 || (better == 0 && a.index <= b.index) ? a : b;
+  LocPair<V> r = host_pair<V>(0, w.index);
+  if constexpr (std::is_floating_point<V>::value)
+    r.value = std::isnan(w.value) ? host_canonical_nan<V>() : w.value;
+  else
+    r.value = w.value;
+  return r;
+}
+template <typename V>
+LocPair<V> host_add(LocPair<V>, LocPair<V>) {
+  HPCP_FAIL("the value-index pair types have no sum");
+}
+
+// The constant-data inputs and check in the host twin's element type.
+template <typename T>
+T host_input(ReduceOp op, int r, int P) {
+  return static_cast<T>(op_input(op, r, P));
+}
+template <typename T>
+T host_vc_init(ReduceOp op, int P) {
+  return static_cast<T>(op_vc_init(op, P));
+}
+template <typename T>
+bool host_is_expected(const T& v, ReduceOp op, int P) {
+  return std::abs(host_to_double(v) - host_to_double(static_cast<T>(op_expected(op, P)))) < 1e-6;
+}
+// The constant data of the host twin for a pair type (the arithmetic types: ArithHost).
+template <typename V>
+struct PairHost {
+  static LocPair<V> input(ReduceOp op, int r, int P) {
+    const LocDatum d = loc_input(op, r, P);
+    return host_pair<V>(d.value, d.index);
+  }
+  static LocPair<V> vc_init(ReduceOp op, int) {
+    const LocDatum d = loc_vc_init(op);
+    return host_pair<V>(d.value, d.index);
+  }
+  // The value's bits and the index: a struct copy need not keep padding bytes, so the host twin cannot check them.
+  static bool is_expected(const LocPair<V>& v, ReduceOp op, int P) {
+    const LocDatum d = loc_expected(op, P);
+    const V want = static_cast<V>(d.value);
+    return std::memcmp(&v.value, &want, sizeof want) == 0 && v.index == d.index;
+  }
+};
+// The bytes of the pair (value, index) with zero padding, written in place.
+template <typename V>
+void pair_bytes(double value, int index, unsigned char* out) {
+  std::memset(out, 0, sizeof(LocPair<V>));
+  const V v = static_cast<V>(value);
+  std::memcpy(out + offsetof(LocPair<V>, value), &v, sizeof v);
+  std::memcpy(out + offsetof(LocPair<V>, index), &index, sizeof index);
+}
+
 // The JSON rows carry "op" only when it is not the sum (sum rows keep their shape).
 std::string op_json(ReduceOp op) {
   return op == ReduceOp::kSum ? std::string() : std::string(",\"op\":\"") + reduce_op_name(op) + "\"";
 }
 
+// A pair type: its value.
 double first_element_as_double(const void* p, ElemType t) {
   double x = 0;
-  dispatch_elem(t, [&](auto tag) { x = host_to_double(*static_cast<const decltype(tag)*>(p)); });
+  if (elem_type_is_pair(t))
+    dispatch_pair(t, [&](auto tag) { x = static_cast<double>(static_cast<const decltype(tag)*>(p)->value); });
+  else
+    dispatch_elem(t, [&](auto tag) { x = host_to_double(*static_cast<const decltype(tag)*>(p)); });
   return x;
 }
 
@@ -282,6 +390,20 @@ unsigned long long count_mismatch_on_host(const void* p, size_t n, double expect
   dispatch_elem(t, [&](auto tag) { bad = count_mismatch_typed<decltype(tag)>(p, n, expected); });
   return bad;
 }
+// Pair types: elements whose bytes differ from the constant-data result of `op`, padding included.
+unsigned long long count_pair_mismatch_on_host(const void* p, size_t n, ReduceOp op, int P, ElemType t) {
+  unsigned long long bad = n;
+  dispatch_pair(t, [&](auto tag) {
+    using V = typename decltype(tag)::value_type;
+    const LocDatum d = loc_expected(op, P);
+    unsigned char want[sizeof(LocPair<V>)];
+    pair_bytes<V>(d.value, d.index, want);
+    const unsigned char* v = static_cast<const unsigned char*>(p);
+    bad = 0;
+    for (size_t i = 0; i < n; ++i) bad += std::memcmp(v + i * sizeof want, want, sizeof want) != 0;
+  });
+  return bad;
+}
 
 uint32_t* pad_of(const Shared& sh, int r) { return static_cast<uint32_t*>(sh.pads.ptr[r]); }
 
@@ -294,6 +416,7 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   HPCP_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   const int right = (me + 1) % P, left = (me - 1 + P) % P;
   const size_t esz = elem_size(cfg.type);
+  const bool pair = elem_type_is_pair(cfg.type);
   uint32_t* my_pad = pad_of(sh, me);
   uint32_t* status = my_pad + kPadWords + sh.pad_extra;
   std::vector<uint32_t*> pad_list;
@@ -433,9 +556,16 @@ void rank_main(RankCtx& ctx, Shared& sh) {
   for (int it = 0; it < cfg.warmup + cfg.iters; ++it) {
     NvtxRange iter_range(it < cfg.warmup ? "allreduce warm-up" : "allreduce timed");
     // (Re-)initialise outside the timed region: VA = VB = rank (the op's input), VC = 0 (sum) or a poison value.
-    const double x = op_input(cfg.op, me, P);
-    launch_init3(va, cfg.algo == "ring-unfused" && !cfg.use_collective ? sh.vb.ptr[me] : nullptr, vc,
-                 sh.n, x, x, op_vc_init(cfg.op, P), cfg.type, stream);
+    void* vb = cfg.algo == "ring-unfused" && !cfg.use_collective ? sh.vb.ptr[me] : nullptr;
+    if (pair) {
+      const LocDatum x = loc_input(cfg.op, me, P), c = loc_vc_init(cfg.op);
+      launch_init_pair(va, sh.n, x.value, x.index, cfg.type, stream);
+      if (vb) launch_init_pair(vb, sh.n, x.value, x.index, cfg.type, stream);
+      launch_init_pair(vc, sh.n, c.value, c.index, cfg.type, stream);
+    } else {
+      const double x = op_input(cfg.op, me, P);
+      launch_init3(va, vb, vc, sh.n, x, x, op_vc_init(cfg.op, P), cfg.type, stream);
+    }
     HPCP_CUDA(cudaStreamSynchronize(stream));
     ctx.barrier();
     launch_barrier_all(pad_list.data(), me, P, ++barrier_epoch, cfg.timeout_ns, status, stream);
@@ -463,12 +593,18 @@ void rank_main(RankCtx& ctx, Shared& sh) {
     // own array (:163-164) and prints "<rank> <VC[0]>" (:161).
     HPCP_CUDA(cudaMemcpyAsync(sh.host_vc[me], vc, sh.n * esz, cudaMemcpyDeviceToHost, stream));
     HPCP_CUDA(cudaStreamSynchronize(stream));
-    bad = count_mismatch_on_host(sh.host_vc[me], sh.n, want, cfg.type);
+    bad = pair ? count_pair_mismatch_on_host(sh.host_vc[me], sh.n, cfg.op, P, cfg.type)
+               : count_mismatch_on_host(sh.host_vc[me], sh.n, want, cfg.type);
   } else {
     unsigned long long* count = nullptr;
     HPCP_CUDA(cudaMalloc(&count, sizeof *count));
     HPCP_CUDA(cudaMemsetAsync(count, 0, sizeof *count, stream));
-    launch_count_mismatch(vc, sh.n, want, cfg.type, count, stream);
+    if (pair) {
+      const LocDatum w = loc_expected(cfg.op, P);
+      launch_count_pair_mismatch(vc, sh.n, w.value, w.index, cfg.type, count, stream);
+    } else {
+      launch_count_mismatch(vc, sh.n, want, cfg.type, count, stream);
+    }
     HPCP_CUDA(cudaMemcpyAsync(&bad, count, sizeof bad, cudaMemcpyDeviceToHost, stream));
     HPCP_CUDA(cudaStreamSynchronize(stream));
     (void)cudaFree(count);
@@ -516,7 +652,15 @@ void rank_main(RankCtx& ctx, Shared& sh) {
 // order, verification, output) on a machine without a device.
 // --algo ring-rsag runs the hops of ring_rsag_kernel with the same rules (ring_order.h): whole segments are memcpy'd
 // into the right neighbour's slot or VC, with a barrier between hops.
+// H supplies the constant data: input(op, r, P), vc_init(op, P) and is_expected(v, op, P).
 template <typename T>
+struct ArithHost {
+  static T input(ReduceOp op, int r, int P) { return host_input<T>(op, r, P); }
+  static T vc_init(ReduceOp op, int P) { return host_vc_init<T>(op, P); }
+  static bool is_expected(const T& v, ReduceOp op, int P) { return host_is_expected(v, op, P); }
+};
+
+template <typename T, class H>
 int run_on_host_typed(const Config& cfg) {
   const int P = cfg.ranks > 0 ? cfg.ranks : 4;
   const bool rsag = cfg.algo == "ring-rsag" && !cfg.use_collective;
@@ -530,9 +674,9 @@ int run_on_host_typed(const Config& cfg) {
   const ReduceOp op = cfg.op;
   run_ranks(P, [&](RankCtx& ctx) {
     const int me = ctx.rank, right = (me + 1) % P;
-    va[me].assign(n, static_cast<T>(op_input(op, me, P)));
-    vb[me].assign(n, static_cast<T>(op_input(op, me, P)));
-    vc[me].assign(n, static_cast<T>(op_vc_init(op, P)));
+    va[me].assign(n, H::input(op, me, P));
+    vb[me].assign(n, H::input(op, me, P));
+    vc[me].assign(n, H::vc_init(op, P));
     ctx.barrier();
     const auto t0 = std::chrono::steady_clock::now();
     if (cfg.use_collective && op != ReduceOp::kSum) {
@@ -555,11 +699,13 @@ int run_on_host_typed(const Config& cfg) {
     } else if (cfg.use_collective && kSum16InF32<T>) {
       // two-shot's 16-bit rule: element i belongs to slice s = i*P/n, whose owner s sums VA[s], VA[s+1], ... (ranks
       // mod P) in fp32 and rounds once
-      for (size_t i = 0; i < n; ++i) {
-        const int s = static_cast<int>(i * P / n);
-        float acc = static_cast<float>(host_to_double(va[s][i]));
-        for (int q = 1; q < P; ++q) acc += static_cast<float>(host_to_double(va[(s + q) % P][i]));
-        vc[me][i] = static_cast<T>(acc);
+      if constexpr (kSum16InF32<T>) {
+        for (size_t i = 0; i < n; ++i) {
+          const int s = static_cast<int>(i * P / n);
+          float acc = static_cast<float>(host_to_double(va[s][i]));
+          for (int q = 1; q < P; ++q) acc += static_cast<float>(host_to_double(va[(s + q) % P][i]));
+          vc[me][i] = static_cast<T>(acc);
+        }
       }
     } else if (cfg.use_collective) {
       for (int r = 0; r < P; ++r)
@@ -598,9 +744,8 @@ int run_on_host_typed(const Config& cfg) {
     const double ms =
         std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     const double t = ctx.max(ms);
-    const T want = static_cast<T>(op_expected(op, P));
     unsigned long long bad = 0;
-    for (size_t i = 0; i < n; ++i) bad += std::abs(host_to_double(vc[me][i]) - host_to_double(want)) >= 1e-6;
+    for (size_t i = 0; i < n; ++i) bad += !H::is_expected(vc[me][i], op, P);
     const double all_bad = ctx.sum(static_cast<double>(bad));
     if (bad == 0)
       std::cout << "Passed " << me << std::endl;
@@ -635,7 +780,13 @@ int run_on_host_typed(const Config& cfg) {
 
 int run_on_host(const Config& cfg) {
   int rc = 1;
-  dispatch_elem(cfg.type, [&](auto tag) { rc = run_on_host_typed<decltype(tag)>(cfg); });
+  if (elem_type_is_pair(cfg.type))
+    dispatch_pair(cfg.type, [&](auto tag) {
+      using T = decltype(tag);
+      rc = run_on_host_typed<T, PairHost<typename T::value_type>>(cfg);
+    });
+  else
+    dispatch_elem(cfg.type, [&](auto tag) { rc = run_on_host_typed<decltype(tag), ArithHost<decltype(tag)>>(cfg); });
   return rc;
 }
 }  // namespace
@@ -701,7 +852,9 @@ int main(int argc, char** argv) {
         case 13: cfg.profile_relaunch = true; break;
         case 14:
           if (!reduce_op_from_name(optarg, &cfg.op))
-            HPCP_FAIL(std::string("unknown --op ") + optarg + " (sum|prod|min|max|band|bor|bxor|land|lor|lxor)");
+            HPCP_FAIL(std::string("unknown --op ") + optarg +
+                      " (sum|prod|min|max|band|bor|bxor|land|lor|lxor|maxloc|minloc)");
+          cfg.op_given = true;
           break;
         case 10: cfg.slots = std::atoi(optarg); break;
         case 11: cfg.pull = true; break;
@@ -714,10 +867,14 @@ int main(int argc, char** argv) {
     HPCP_REQUIRE(cfg.slots == 0 || cfg.slots == 2, "--slots must be 2 (or omitted)");
     HPCP_REQUIRE(cfg.algo != "ring-rsag" || (cfg.slots == 0 && !cfg.pull),
                  "--slots 2 and --pull are variants of --algo ring, not of ring-rsag");
+    if (elem_type_is_pair(cfg.type) && !cfg.op_given) cfg.op = ReduceOp::kMaxLoc;
     HPCP_REQUIRE(cfg.op == ReduceOp::kSum || !cfg.use_collective || cfg.coll != "nvls",
                  std::string("--coll nvls is sum-only: --op ") + reduce_op_name(cfg.op) + " needs --coll twoshot or auto");
-    HPCP_REQUIRE(!reduce_op_integer_only(cfg.op) || elem_type_is_integer(cfg.type),
-                 reduce_op_type_error(cfg.op, cfg.type) + " (pass --type or run a typed binary such as allreduce.int)");
+    HPCP_REQUIRE(reduce_op_takes(cfg.op, cfg.type),
+                 reduce_op_type_error(cfg.op, cfg.type) +
+                     (elem_type_is_pair(cfg.type) || reduce_op_on_pairs(cfg.op)
+                          ? " (pass --type or run a typed binary such as allreduce.float_int)"
+                          : " (pass --type or run a typed binary such as allreduce.int)"));
 
     if (cfg.cpu) return run_on_host(cfg);
     const int ndev = visible_device_count();

@@ -23,6 +23,11 @@ On the integer types only (↔ MPI_BAND / MPI_BOR / MPI_BXOR / MPI_LAND / MPI_LO
 ``bxor`` act on the element bits; ``land``, ``lor``, ``lxor`` take an element as true iff it is nonzero and give 0 or 1
 (at one rank VC is VA).  A floating type is refused, as MPI does, and so is ``nccl``, which has no such reductions.
 Their checks are listed in ``op_input`` and ``expected_value``.
+On the value-index pair types only (``float_int``, ``double_int``, ``long_int``, ``2int``, ``short_int``, ↔ MPI_FLOAT_INT
+...): ``maxloc`` and ``minloc`` (↔ MPI_MAXLOC / MPI_MINLOC); the pair types take no other op.  The larger / smaller value
+wins, a NaN value wins in both, -0 < +0, ties take the smaller signed index, and a combined pair's padding is zero.
+``nccl`` has no such reductions and refuses them; ``ring-nccl`` moves the bytes and combines them in torch.  Their
+check is ``loc_input`` / ``loc_expected`` (exact bytes).
 
 The native single-process CLI twin is ``bin/allreduce`` (csrc/miniapps/allreduce.cu).
 """
@@ -35,6 +40,7 @@ from typing import List, Optional
 import torch
 
 from .. import native
+from ..ops.allreduce import LOC_LAYOUT, loc_combine, pack_loc, unpack_loc
 from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
@@ -53,6 +59,10 @@ OPS = ("sum", "prod", "min", "max") + INTEGER_OPS
 _OP_ALIASES = {"product": "prod"}
 UNSIGNED_TYPES = ("uint", "ulong", "ushort")   # torch stand-ins are signed: NCCL min/max would compare them signed
 FLOAT_TYPES = ("float", "double") + FLOAT16_TYPES
+PAIR_TYPES = tuple(LOC_LAYOUT)        # value-index pairs: maxloc / minloc only
+LOC_OPS = ("maxloc", "minloc")
+OPS = OPS + LOC_OPS
+DTYPES = tuple(_TORCH_DTYPE) + PAIR_TYPES
 
 
 def reduce_op(op: str) -> str:
@@ -64,9 +74,16 @@ def reduce_op(op: str) -> str:
 
 
 def check_op_type(op: str, dtype: str) -> None:
-    """ValueError if ``op`` does not reduce ``dtype``: the bitwise and logical ops take integer types only."""
-    if reduce_op(op) in INTEGER_OPS and dtype in FLOAT_TYPES:
-        raise ValueError(f"op must be sum, prod, min or max for {dtype}: {reduce_op(op)} reduces integer types only")
+    """ValueError if ``op`` does not reduce ``dtype``: the bitwise and logical ops take integer types only, maxloc and
+    minloc the pair types only, and the pair types no other op.  The words are the native layers'."""
+    op = reduce_op(op)
+    if dtype in PAIR_TYPES and op not in LOC_OPS:
+        raise ValueError(f"op must be maxloc or minloc for {dtype}: {op} reduces arithmetic types only")
+    if op in LOC_OPS and dtype not in PAIR_TYPES:
+        ops = "sum, prod, min or max" if dtype in FLOAT_TYPES else "sum, prod, min, max, band, bor, bxor, land, lor or lxor"
+        raise ValueError(f"op must be {ops} for {dtype}: {op} reduces value-index pair types only")
+    if op in INTEGER_OPS and dtype in FLOAT_TYPES:
+        raise ValueError(f"op must be sum, prod, min or max for {dtype}: {op} reduces integer types only")
 
 
 def expected_value(world: int, op: str = "sum") -> float:
@@ -121,6 +138,26 @@ def vc_init(op: str, world: int) -> float:
     """VC before the constant-data run: 0 for the sum, which accumulates into it; for the other ops a value that would
     change the result if a kernel read VC instead of overwriting it."""
     return {"max": float(world), "bor": 16.0, "bxor": 64.0, "lor": 3.0, "lxor": 5.0}.get(op, 0.0)
+
+
+def loc_input(op: str, rank: int, world: int):
+    """(value, index) ``rank`` holds in the constant-data run of maxloc / minloc.  The result's index -1 is held by rank
+    1 only, next to larger indices with the same value and a smaller index (rank 0's) with the losing value: a tie
+    broken towards the larger index, an unsigned index compare and a selection by index alone each give another pair."""
+    mx = op == "maxloc"
+    if rank == 0:
+        return (0.0 if mx else 1.0), -world - 10
+    return (1.0 if mx else 0.0), 2 * rank - 3
+
+
+def loc_expected(op: str, world: int):
+    """(value, index) of every element of VC after the constant-data run (VC is VA at one rank)."""
+    return loc_input(op, 0, 1) if world == 1 else ((1.0 if op == "maxloc" else 0.0), -1)
+
+
+def loc_vc_init(op: str):
+    """VC before the constant-data run: a pair that would win if a kernel read VC."""
+    return (7.0 if op == "maxloc" else -7.0), -1000
 
 
 def _nccl_op(op: str):
@@ -212,14 +249,16 @@ class AllreduceMiniapp:
         on unsigned types (their torch stand-ins are signed)."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
-        if dtype not in _TORCH_DTYPE:
-            raise ValueError(f"dtype must be one of {sorted(_TORCH_DTYPE)}")
+        if dtype not in DTYPES:
+            raise ValueError(f"dtype must be one of {sorted(DTYPES)}")
         op = reduce_op(op)
         check_op_type(op, dtype)
         if op != "sum" and algo == "nvls":
             raise ValueError(f"nvls reduces sums only: op={op} needs twoshot or a ring")
         if op in INTEGER_OPS and algo == "nccl":
             raise ValueError(f"nccl has no bitwise or logical reductions: op={op} needs twoshot or a ring")
+        if op in LOC_OPS and algo == "nccl":
+            raise ValueError(f"nccl has no maxloc or minloc: op={op} needs twoshot, a ring or ring-nccl")
         if op in ("min", "max") and algo in ("nccl", "ring-nccl") and dtype in UNSIGNED_TYPES:
             raise ValueError(f"{algo} compares {dtype} as a signed torch type: op={op} is refused")
         self.op = op
@@ -292,6 +331,13 @@ class AllreduceMiniapp:
     def initialize(self) -> None:
         va, vc = self._ptrs()
         vb = self.vb.local_ptr if self.vb is not None else 0
+        if self.dtype in PAIR_TYPES:
+            x, i = loc_input(self.op, self.rank, self.world)
+            for p in (va, vb):
+                if p:
+                    self.C.init_pair(p, self.n, x, i, self.dtype, self._stream())
+            self.C.init_pair(vc, self.n, *loc_vc_init(self.op), self.dtype, self._stream())
+            return
         x = op_input(self.op, self.rank, self.world)
         # VC: 0 for the sum, which accumulates into it; the other ops must overwrite it whatever it holds
         self.C.init3(va, vb, vc, self.n, x, x, vc_init(self.op, self.world), self.dtype, self._stream())
@@ -374,7 +420,7 @@ class AllreduceMiniapp:
         elif self.algo == "ring-nccl":
             import torch.distributed as dist
             from ..parallel.symmetric import tensor_from_ptr
-            td = _TORCH_DTYPE[self.dtype]
+            td = _TORCH_DTYPE.get(self.dtype, torch.uint8)    # pair types: their bytes
             cur = tensor_from_ptr(va, self.nbytes, self.device, td)
             other = self.vb.tensor(td)
             acc = tensor_from_ptr(vc, self.nbytes, self.device, td)
@@ -386,7 +432,9 @@ class AllreduceMiniapp:
                        "bxor": lambda: torch.bitwise_xor(acc, cur, out=acc),
                        "land": lambda: acc.copy_(torch.logical_and(acc, cur).to(td)),
                        "lor": lambda: acc.copy_(torch.logical_or(acc, cur).to(td)),
-                       "lxor": lambda: acc.copy_(torch.logical_xor(acc, cur).to(td))}
+                       "lxor": lambda: acc.copy_(torch.logical_xor(acc, cur).to(td)),
+                       "maxloc": lambda: acc.copy_(loc_combine(acc, cur, self.dtype, "maxloc")),
+                       "minloc": lambda: acc.copy_(loc_combine(acc, cur, self.dtype, "minloc"))}
             if self.op == "sum":
                 acc.add_(cur)
             else:
@@ -404,8 +452,12 @@ class AllreduceMiniapp:
     def mismatches(self) -> int:
         _, vc = self._ptrs()
         count = torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.device))
-        self.C.count_mismatch(vc, self.n, expected_value(self.world, self.op), self.dtype, count.data_ptr(),
-                              self._stream())
+        if self.dtype in PAIR_TYPES:
+            self.C.count_pair_mismatch(vc, self.n, *loc_expected(self.op, self.world), self.dtype, count.data_ptr(),
+                                       self._stream())
+        else:
+            self.C.count_mismatch(vc, self.n, expected_value(self.world, self.op), self.dtype, count.data_ptr(),
+                                  self._stream())
         torch.cuda.synchronize(self.device)
         return int(count.item())
 
@@ -487,13 +539,17 @@ class VirtualAllreduce:
         self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, vas: List[torch.Tensor]) -> None:
-        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type), VC <- 0 (the sum rings accumulate into
-        it; ring-rsag and every op other than the sum overwrite it)."""
-        td = _TORCH_DTYPE[self.dtype]
+        """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type; for a pair type a (values, indices) tuple,
+        packed by ``pack_loc``), VC <- 0 (the sum rings accumulate into it; ring-rsag and every op other than the sum
+        overwrite it)."""
         torch.cuda.synchronize(self.device)
         for app, v in zip(self.ranks, vas):
-            app.va.tensor(td).copy_(v)
-            app.vc.tensor(td).zero_()
+            if self.dtype in PAIR_TYPES:
+                app.va.tensor(torch.uint8).copy_(pack_loc(*v, dtype=self.dtype))
+                app.vc.tensor(torch.uint8).zero_()
+            else:
+                app.va.tensor(_TORCH_DTYPE[self.dtype]).copy_(v)
+                app.vc.tensor(_TORCH_DTYPE[self.dtype]).zero_()
         torch.cuda.synchronize(self.device)
 
     def run_once(self) -> None:
@@ -510,8 +566,10 @@ class VirtualAllreduce:
             app.pads.check()
 
     def results(self) -> List[torch.Tensor]:
-        """VC of every rank, on the host."""
+        """VC of every rank, on the host; for a pair type a (values, int32 indices) tuple per rank (``unpack_loc``)."""
         self.synchronize()
+        if self.dtype in PAIR_TYPES:
+            return [unpack_loc(app.vc.tensor(torch.uint8).cpu(), self.dtype) for app in self.ranks]
         return [app.vc.tensor(_TORCH_DTYPE[self.dtype]).cpu() for app in self.ranks]
 
     def close(self) -> None:
@@ -549,7 +607,7 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap = argparse.ArgumentParser(prog="allreduce", add_help=True)
     ap.add_argument("-a", action="store_true", help="use the one-launch collective (nvls, else twoshot)")
     ap.add_argument("-p", type=int, default=25, help="2^p elements (default 25)")
-    ap.add_argument("--type", default="float", choices=sorted(_TORCH_DTYPE))
+    ap.add_argument("--type", default="float", choices=sorted(DTYPES))
     ap.add_argument("--algo", default="ring", choices=ALGOS)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
@@ -559,11 +617,11 @@ def main(argv: Optional[List[str]] = None) -> int:
                          "default world-1 slots")
     ap.add_argument("--pull", action="store_true",
                     help="fused ring, receiver-driven: blocks are loaded from the left neighbour (peer loads)")
-    ap.add_argument("--op", default="sum", choices=OPS + tuple(_OP_ALIASES),
-                    help="reduction (default sum; nvls is sum-only, -a uses two-shot for the others; "
-                         "band bor bxor land lor lxor take integer types only)")
+    ap.add_argument("--op", default=None, choices=OPS + tuple(_OP_ALIASES),
+                    help="reduction (default sum, maxloc on a pair type; nvls is sum-only, -a uses two-shot for the "
+                         "others; band bor bxor land lor lxor take integer types only, maxloc minloc pair types only)")
     args = ap.parse_args(argv)
-    op = reduce_op(args.op)
+    op = reduce_op(args.op if args.op is not None else "maxloc" if args.type in PAIR_TYPES else "sum")
     check_op_type(op, args.type)
     comm = Comm()
     device = comm.device   # chosen before the process group was bound to it (Comm.pick_device)

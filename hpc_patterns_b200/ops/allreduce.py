@@ -4,6 +4,10 @@
 ``ring_allreduce`` / ``two_shot`` / ``nvls`` are the fused one-launch replacements of its
 ``SendRecvRing`` loop and ``MPI_Allreduce``.  The multi-rank drivers live in
 ``hpc_patterns_b200.models.allreduce``; these wrappers are what they (and the tests) call.
+
+The value-index pair types of maxloc / minloc (``float_int``, ``double_int``, ``long_int``, ``2int``, ``short_int``, ↔
+MPI_FLOAT_INT ...) are C structs ``{value; int index;}`` in their natural layout; ``pack_loc`` / ``unpack_loc`` convert
+between that layout (a flat uint8 tensor, padding zero) and a (values, int32 indices) pair of tensors.
 """
 from __future__ import annotations
 
@@ -22,6 +26,69 @@ def dtype_name(t: torch.Tensor) -> str:
         return _DTYPE_NAME[t.dtype]
     except KeyError:
         raise TypeError(f"allreduce kernels support float32, int32, bfloat16 and float16, not {t.dtype}") from None
+
+
+# pair type -> (torch dtype of the value, bytes per pair, byte offset of the index)
+LOC_LAYOUT = {"float_int": (torch.float32, 8, 4), "double_int": (torch.float64, 16, 8), "long_int": (torch.int64, 16, 8),
+              "2int": (torch.int32, 8, 4), "short_int": (torch.int16, 8, 4)}
+_LOC_OF_VALUE = {vt: name for name, (vt, _, _) in LOC_LAYOUT.items()}
+
+
+def pack_loc(values: torch.Tensor, indices: torch.Tensor, dtype: Optional[str] = None) -> torch.Tensor:
+    """The pairs (values[i], indices[i]) in the C layout of ``dtype`` (by default the pair type of ``values.dtype``):
+    a flat uint8 tensor on ``values``' device, padding bytes zero.  Indices are converted to int32."""
+    if dtype is None:
+        if values.dtype not in _LOC_OF_VALUE:
+            raise TypeError(f"no value-index pair type has {values.dtype} values")
+        dtype = _LOC_OF_VALUE[values.dtype]
+    if dtype not in LOC_LAYOUT:
+        raise ValueError(f"dtype must be one of {tuple(LOC_LAYOUT)}, not {dtype!r}")
+    vt, size, off = LOC_LAYOUT[dtype]
+    if values.numel() != indices.numel():
+        raise ValueError("values and indices must have the same number of elements")
+    n = values.numel()
+    buf = torch.zeros(n, size, dtype=torch.uint8, device=values.device)
+    vbytes = values.reshape(-1).to(vt).contiguous().view(torch.uint8).reshape(n, -1)
+    buf[:, :vbytes.shape[1]] = vbytes
+    buf[:, off:off + 4] = indices.reshape(-1).to(torch.int32).to(values.device).contiguous().view(torch.uint8) \
+        .reshape(n, 4)
+    return buf.reshape(-1)
+
+
+def unpack_loc(buf: torch.Tensor, dtype: str):
+    """(values, int32 indices) of the pairs of type ``dtype`` held in ``buf`` (any tensor whose bytes are the pairs)."""
+    if dtype not in LOC_LAYOUT:
+        raise ValueError(f"dtype must be one of {tuple(LOC_LAYOUT)}, not {dtype!r}")
+    vt, size, off = LOC_LAYOUT[dtype]
+    b = buf.contiguous().reshape(-1).view(torch.uint8).reshape(-1, size)
+    vbytes = torch.empty(0, dtype=vt).element_size()
+    return (b[:, :vbytes].contiguous().view(vt).reshape(-1), b[:, off:off + 4].contiguous().view(torch.int32).reshape(-1))
+
+
+def loc_combine(a: torch.Tensor, b: torch.Tensor, dtype: str, op: str) -> torch.Tensor:
+    """a o b for the packed pairs ``a`` and ``b`` (pack_loc) with the kernels' rules: the larger (maxloc) or smaller
+    (minloc) value wins, a NaN value wins in both and -0 < +0; bit-equal values or two NaNs take the smaller index; the
+    result is packed with zero padding and the canonical NaN (all bits set but the sign)."""
+    va, ia = unpack_loc(a, dtype)
+    vb, ib = unpack_loc(b, dtype)
+    mx = op == "maxloc"
+    if va.is_floating_point():
+        na, nb = torch.isnan(va), torch.isnan(vb)
+        sa, sb = torch.signbit(va), torch.signbit(vb)
+        eq = (va == vb) & (sa == sb)
+        gt = (va > vb) | ((va == vb) & sb & ~sa)       # in the order -0 < +0
+        better = (na & ~nb) | (~na & ~nb & ~eq & (gt if mx else ~gt))
+        tie = (na & nb) | (~na & ~nb & eq)
+    else:
+        better = va > vb if mx else va < vb
+        tie = va == vb
+    take_a = better | (tie & (ia <= ib))
+    v = torch.where(take_a, va, vb)
+    if v.is_floating_point():
+        bits = torch.int32 if v.dtype == torch.float32 else torch.int64
+        canon = torch.tensor(0x7FFFFFFF if bits == torch.int32 else 0x7FFFFFFFFFFFFFFF, dtype=bits).view(v.dtype)
+        v = torch.where(torch.isnan(v), canon.to(v.device), v)
+    return pack_loc(v, torch.where(take_a, ia, ib), dtype)
 
 
 def accumulate(va: torch.Tensor, vc: torch.Tensor, stream: Optional[int] = None) -> torch.Tensor:
