@@ -30,7 +30,7 @@ LIB        := $(BUILD)/libhpcp.a
 # Programs built straight from one source file depend on every header (cheap and never stale).
 HEADERS := $(shell find csrc -name '*.h' -o -name '*.hpp' -o -name '*.cuh')
 
-CLIS := bin/concurency bin/omp_con bin/peer2pear bin/topology bin/allreduce bin/halo bin/interop_torchless \
+CLIS := bin/concurency bin/omp_con bin/peer2pear bin/topology bin/allreduce bin/alltoall bin/halo bin/interop_torchless \
         bin/interop_driver bin/native_selftest
 
 .PHONY: all cli aliases ext omp_con sass sanitize test clean
@@ -84,6 +84,10 @@ bin/topology: csrc/p2p/topology.cpp csrc/p2p/topology_core.cpp $(HEADERS)
 	$(CXX) $(CXXFLAGS) -DHPCP_TOPOLOGY_WITH_CUDA $(filter %.cpp,$^) -o $@ -L/usr/local/cuda/lib64 -lcudart_static -ldl -lrt -lpthread
 
 bin/allreduce: csrc/miniapps/allreduce.cu $(LIB) $(HEADERS)
+	@mkdir -p bin
+	$(NVCC) $(NVFLAGS) $< $(LIB) -o $@ -lgomp
+
+bin/alltoall: csrc/miniapps/alltoall.cu $(LIB) $(HEADERS)
 	@mkdir -p bin
 	$(NVCC) $(NVFLAGS) $< $(LIB) -o $@ -lgomp
 

@@ -810,6 +810,42 @@ PYBIND11_MODULE(_C, m) {
       py::arg("status") = 0, py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0,
       py::arg("stream") = 0, py::arg("op") = "sum", "In-switch sum; any other op raises.");
 
+  // ------------------------------------------------------------- all-to-all ----
+  m.def(
+      "all_to_all",
+      [](const std::vector<uintptr_t>& send, const std::vector<uintptr_t>& recv, const std::vector<uintptr_t>& pads,
+         uintptr_t ticket, uint32_t ticket_base, int rank, size_t block_bytes, uint32_t barrier_epoch,
+         uint64_t timeout_ns, uintptr_t status, int ctas, int device, uintptr_t stream, bool pull) {
+        AllToAllArgs a;
+        a.world = static_cast<int>(send.size());
+        if (const char* why = all_to_all_refusal(a.world, block_bytes)) throw std::invalid_argument(why);
+        HPCP_REQUIRE(recv.size() == send.size() && pads.size() == send.size(), "all-to-all: inconsistent rank lists");
+        for (int r = 0; r < a.world; ++r) {
+          a.send[r] = as_ptr<const void>(send[r]);
+          a.recv[r] = as_ptr<void>(recv[r]);
+          a.pads[r] = as_ptr<uint32_t>(pads[r]);
+        }
+        a.ticket = as_ptr<uint32_t>(ticket);
+        a.ticket_base = ticket_base;
+        a.rank = rank;
+        a.block_bytes = block_bytes;
+        a.barrier_epoch = barrier_epoch;
+        a.timeout_ns = timeout_ns;
+        a.status = as_ptr<uint32_t>(status);
+        a.pull = pull;
+        return launch_all_to_all(a, ctas, device, as_stream(stream));
+      },
+      py::arg("send"), py::arg("recv"), py::arg("pads"), py::arg("ticket"), py::arg("ticket_base"), py::arg("rank"),
+      py::arg("block_bytes"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0, py::arg("status") = 0,
+      py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0, py::arg("pull") = false,
+      "Equal-block all-to-all in one launch: block p of my recv <- block `rank` of rank p's send (push: peer stores, "
+      "pull: peer loads), ending with the node barrier.  Returns the CTAs launched (advance the ticket by it).");
+  m.def("all_to_all_refusal", [](int world, size_t block_bytes) {
+    const char* why = all_to_all_refusal(world, block_bytes);
+    return std::string(why ? why : "");
+  });
+  m.attr("ALL_TO_ALL_OVERLAP_ERROR") = kAllToAllOverlapError;
+
   // ------------------------------------------------------------- topology ----
   m.def("topology_merge_planes", [](int n_gpus, const std::vector<std::vector<std::string>>& links) {
     std::vector<topo::LinkSet> ls;

@@ -431,4 +431,35 @@ struct NvlsArgs {
 int launch_allreduce_nvls(const NvlsArgs& args, ElemType type, int ctas, int device,
                           cudaStream_t stream);
 
+// ------------------------------------------------------------- all-to-all ----
+// (↔ MPI_Alltoall with equal blocks, ncclAllToAll.)  Every rank holds send and recv buffers of `world` blocks of
+// `block_bytes`; afterwards block p of rank r's recv is a byte copy of block r of rank p's send.  Push stores my send
+// block q into slot `rank` of rank q's recv, pull loads slot `rank` of rank p's send into my block p; one launch ends
+// with the node barrier, so completion means every peer's bytes have landed here and every peer has finished reading
+// my send buffer.  Precondition (as two-shot's): every rank's send buffer is final and no rank still reads its recv
+// (a cross-rank barrier after the producer).  Send is never written; send and recv must not overlap.
+struct AllToAllArgs {
+  const void* send[kApiMaxRanks] = {nullptr};  // peer-mapped send buffers of every rank
+  void* recv[kApiMaxRanks] = {nullptr};        // peer-mapped receive buffers of every rank
+  uint32_t* pads[kApiMaxRanks] = {nullptr};    // signal pads of every rank
+  uint32_t* ticket = nullptr;
+  uint32_t ticket_base = 0;
+  int rank = 0;
+  int world = 0;                               // 1 ... kApiMaxRanks
+  size_t block_bytes = 0;                      // a positive multiple of 16
+  uint32_t barrier_epoch = 0;
+  uint64_t timeout_ns = 0;
+  uint32_t* status = nullptr;
+  bool pull = false;
+};
+// The refusals, in the same words in every layer (CLI, bindings, Python).
+constexpr const char* kAllToAllBlockError = "all-to-all: block_bytes must be a positive multiple of 16";
+constexpr const char* kAllToAllWorldError = "all-to-all: world must be between 1 and 16 ranks";
+constexpr const char* kAllToAllOverlapError =
+    "all-to-all: the send and receive buffers must not overlap (no in-place operation)";
+// nullptr if (world, block_bytes) is accepted, else the refusal's words.
+const char* all_to_all_refusal(int world, size_t block_bytes);
+// Returns the number of CTAs launched (the caller advances its ticket counter by it).
+int launch_all_to_all(const AllToAllArgs& args, int ctas, int device, cudaStream_t stream);
+
 }  // namespace hpcp

@@ -3,6 +3,7 @@
   concurency   compute-while-copy overlap benchmark (native driver in-process)
   peer2pear    P2P bandwidth, process-per-GPU (run under torchrun for >1 GPU)
   allreduce    allreduce miniapp, process-per-GPU (run under torchrun)
+  alltoall     equal-block all-to-all miniapp (push / pull kernels, nccl baseline), process-per-GPU (torchrun)
   halo         the miniapp loop as a halo exchange fused into a slab stencil — the flagship (run under torchrun)
   tp           tensor-parallel linear layers with the collective fused into the GEMM, vs cuBLAS + NCCL (torchrun)
   topology     fabric planes / rank->GPU mapping (JSON)
@@ -18,7 +19,7 @@ from __future__ import annotations
 import os
 import sys
 
-_GPU_PROGRAMS = ("peer2pear", "allreduce", "halo", "tp", "interop")
+_GPU_PROGRAMS = ("peer2pear", "allreduce", "alltoall", "halo", "tp", "interop")
 
 
 def _no_gpu_message(prog: str):
@@ -26,7 +27,7 @@ def _no_gpu_message(prog: str):
     import torch
 
     if prog in _GPU_PROGRAMS and not torch.cuda.is_available():
-        hint = f"; bin/{prog} --cpu is the host-only plumbing run" if prog in ("peer2pear", "allreduce") else ""
+        hint = f"; bin/{prog} --cpu is the host-only plumbing run" if prog in ("peer2pear", "allreduce", "alltoall") else ""
         return f"Error: {prog}: no CUDA device (this program runs sm_90a kernels{hint})"
     return None
 
@@ -67,6 +68,9 @@ def _dispatch(prog: str, rest: list) -> int:
         return m(rest)
     if prog == "allreduce":
         from .models.allreduce import main as m
+        return m(rest)
+    if prog == "alltoall":
+        from .models.alltoall import main as m
         return m(rest)
     if prog == "halo":
         from .models.halo import main as m
