@@ -22,6 +22,7 @@
 #include "common/signal_layout.h"
 #include "concurency/bench.hpp"
 #include "concurency/driver.hpp"
+#include "kernels/alltoallv_plan.h"
 #include "kernels/api.h"
 #include "kernels/ring_order.h"
 #include "kernels/halo_columns.h"
@@ -845,6 +846,77 @@ PYBIND11_MODULE(_C, m) {
     return std::string(why ? why : "");
   });
   m.attr("ALL_TO_ALL_OVERLAP_ERROR") = kAllToAllOverlapError;
+
+  // ----------------------------------------------------------- all-to-all-v ----
+  // The plan rules (kernels/alltoallv_plan.h) on a row-major world x world count matrix.
+  const auto count_matrix = [](const std::vector<int64_t>& m, int world) {
+    HPCP_REQUIRE(world >= 1 && world <= kApiMaxRanks && m.size() == static_cast<size_t>(world) * world,
+                 "all-to-all-v: the count matrix must hold world x world counts");
+    return m.data();
+  };
+  m.def("alltoallv_verdict", [count_matrix](const std::vector<int64_t>& m, int world, int64_t send_capacity_rows,
+                                            int64_t recv_capacity_rows) {
+    return a2av_verdict(count_matrix(m, world), world, send_capacity_rows, recv_capacity_rows);
+  }, py::arg("counts"), py::arg("world"), py::arg("send_capacity_rows"), py::arg("recv_capacity_rows"));
+  m.def("alltoallv_send_offset", [count_matrix](const std::vector<int64_t>& m, int world, int p, int q) {
+    HPCP_REQUIRE(p >= 0 && p < world && q >= 0 && q < world, "all-to-all-v: rank out of range");
+    return a2av_send_offset(count_matrix(m, world), world, p, q);
+  }, py::arg("counts"), py::arg("world"), py::arg("p"), py::arg("q"));
+  m.def("alltoallv_recv_offset", [count_matrix](const std::vector<int64_t>& m, int world, int p, int r) {
+    HPCP_REQUIRE(p >= 0 && p < world && r >= 0 && r < world, "all-to-all-v: rank out of range");
+    return a2av_recv_offset(count_matrix(m, world), world, p, r);
+  }, py::arg("counts"), py::arg("world"), py::arg("p"), py::arg("r"));
+  m.def(
+      "all_to_all_v",
+      [](const std::vector<uintptr_t>& send, const std::vector<uintptr_t>& recv, const std::vector<uintptr_t>& counts,
+         uintptr_t recv_counts, uintptr_t verdict, const std::vector<uintptr_t>& pads, uintptr_t ticket,
+         uint32_t ticket_base, int rank, size_t row_bytes, int64_t send_capacity_rows, int64_t recv_capacity_rows,
+         uint32_t barrier_epoch, uint64_t timeout_ns, uintptr_t status, int ctas, int device, uintptr_t stream,
+         bool pull) {
+        AllToAllVArgs a;
+        a.world = static_cast<int>(send.size());
+        if (const char* why = all_to_all_v_refusal(a.world, row_bytes, send_capacity_rows, recv_capacity_rows))
+          throw std::invalid_argument(why);
+        HPCP_REQUIRE(recv.size() == send.size() && counts.size() == send.size() && pads.size() == send.size(),
+                     "all-to-all-v: inconsistent rank lists");
+        for (int r = 0; r < a.world; ++r) {
+          a.send[r] = as_ptr<const void>(send[r]);
+          a.recv[r] = as_ptr<void>(recv[r]);
+          a.counts[r] = as_ptr<const int64_t>(counts[r]);
+          a.pads[r] = as_ptr<uint32_t>(pads[r]);
+        }
+        a.recv_counts = as_ptr<int64_t>(recv_counts);
+        a.verdict = as_ptr<uint32_t>(verdict);
+        a.ticket = as_ptr<uint32_t>(ticket);
+        a.ticket_base = ticket_base;
+        a.rank = rank;
+        a.row_bytes = row_bytes;
+        a.send_capacity_rows = send_capacity_rows;
+        a.recv_capacity_rows = recv_capacity_rows;
+        a.barrier_epoch = barrier_epoch;
+        a.timeout_ns = timeout_ns;
+        a.status = as_ptr<uint32_t>(status);
+        a.pull = pull;
+        return launch_all_to_all_v(a, ctas, device, as_stream(stream));
+      },
+      py::arg("send"), py::arg("recv"), py::arg("counts"), py::arg("recv_counts"), py::arg("verdict"), py::arg("pads"),
+      py::arg("ticket"), py::arg("ticket_base"), py::arg("rank"), py::arg("row_bytes"), py::arg("send_capacity_rows"),
+      py::arg("recv_capacity_rows"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0, py::arg("status") = 0,
+      py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0, py::arg("pull") = false,
+      "All-to-all-v in one launch: every CTA reads every rank's int64 send counts over peer memory, the packed "
+      "segments move only if the count matrix is accepted; recv_counts and the verdict word are always written.  "
+      "Returns the CTAs launched (advance the ticket by it).");
+  m.def("all_to_all_v_refusal", [](int world, size_t row_bytes, int64_t send_capacity_rows,
+                                   int64_t recv_capacity_rows) {
+    const char* why = all_to_all_v_refusal(world, row_bytes, send_capacity_rows, recv_capacity_rows);
+    return std::string(why ? why : "");
+  });
+  m.def("all_to_all_v_verdict_words", [](uint32_t verdict) { return std::string(all_to_all_v_verdict_words(verdict)); });
+  m.attr("ALLTOALLV_ACCEPTED") = static_cast<int>(kA2avAccepted);
+  m.attr("ALLTOALLV_NEGATIVE") = static_cast<int>(kA2avNegative);
+  m.attr("ALLTOALLV_SEND_CAPACITY") = static_cast<int>(kA2avSendCapacity);
+  m.attr("ALLTOALLV_RECV_CAPACITY") = static_cast<int>(kA2avRecvCapacity);
+  m.attr("ALL_TO_ALL_V_COUNTS_OVERLAP_ERROR") = kAllToAllVCountsOverlapError;
 
   // ------------------------------------------------------------- topology ----
   m.def("topology_merge_planes", [](int n_gpus, const std::vector<std::vector<std::string>>& links) {

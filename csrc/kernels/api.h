@@ -462,4 +462,42 @@ const char* all_to_all_refusal(int world, size_t block_bytes);
 // Returns the number of CTAs launched (the caller advances its ticket counter by it).
 int launch_all_to_all(const AllToAllArgs& args, int ctas, int device, cudaStream_t stream);
 
+// ----------------------------------------------------------- all-to-all-v ----
+// (↔ MPI_Alltoallv with packed displacements, all_to_all_single with split sizes.)  Data moves in rows of row_bytes;
+// rank p's device array counts[p][0 .. world) holds the rows it sends to every rank, and every kernel reads the whole
+// world x world matrix over peer memory, so the host never learns a count.  Packed layouts and the verdict are the
+// rules of alltoallv_plan.h.  CTA 0 writes recv_counts[p] = counts[p][rank] and *verdict (0 = accepted, else the
+// broken rule's number, see all_to_all_v_verdict_words); a refused launch moves no data byte on any rank and still
+// ends with the node barrier.  Precondition as the all-to-all's, the send counts included: every rank's send buffer
+// and counts are final and no rank still reads its receive buffer or recv_counts.  Send and counts are never written.
+struct AllToAllVArgs {
+  const void* send[kApiMaxRanks] = {nullptr};       // peer-mapped send buffers of every rank
+  void* recv[kApiMaxRanks] = {nullptr};             // peer-mapped receive buffers of every rank
+  const int64_t* counts[kApiMaxRanks] = {nullptr};  // peer-mapped int64[world] send counts of every rank
+  int64_t* recv_counts = nullptr;                   // local int64[world]
+  uint32_t* verdict = nullptr;                      // local word
+  uint32_t* pads[kApiMaxRanks] = {nullptr};
+  uint32_t* ticket = nullptr;
+  uint32_t ticket_base = 0;
+  int rank = 0;
+  int world = 0;                                    // 1 ... kApiMaxRanks
+  size_t row_bytes = 0;                             // a positive multiple of 16
+  int64_t send_capacity_rows = 0;                   // rows every send buffer holds (the same on every rank)
+  int64_t recv_capacity_rows = 0;                   // rows every receive buffer holds (the same on every rank)
+  uint32_t barrier_epoch = 0;
+  uint64_t timeout_ns = 0;
+  uint32_t* status = nullptr;
+  bool pull = false;
+};
+constexpr const char* kAllToAllVRowError = "all-to-all-v: row_bytes must be a positive multiple of 16";
+constexpr const char* kAllToAllVCapacityError = "all-to-all-v: the send and receive capacities must be positive";
+constexpr const char* kAllToAllVCountsOverlapError =
+    "all-to-all-v: recv_counts must not overlap this rank's send counts";
+// nullptr if (world, row_bytes, capacities) are accepted, else the refusal's words (world: kAllToAllWorldError).
+const char* all_to_all_v_refusal(int world, size_t row_bytes, int64_t send_capacity_rows, int64_t recv_capacity_rows);
+// The words of a verdict (alltoallv_plan.h), "" for 0.
+const char* all_to_all_v_verdict_words(uint32_t verdict);
+// Returns the number of CTAs launched (the caller advances its ticket counter by it).
+int launch_all_to_all_v(const AllToAllVArgs& args, int ctas, int device, cudaStream_t stream);
+
 }  // namespace hpcp

@@ -3,6 +3,7 @@
 // the concurrency driver's pure functions.  Built as bin/native_selftest; run by tests/test_native_selftest.py
 // (the reference has no unit tests at all).
 #include <atomic>
+#include <cstdint>
 #include <cmath>
 #include <cstdio>
 #include <iostream>
@@ -15,6 +16,7 @@
 #include "../common/dtype_traits.h"
 #include "../common/rank_runtime.h"
 #include "../concurency/driver.hpp"
+#include "../kernels/alltoallv_plan.h"
 #include "../kernels/ring_order.h"
 #include "../kernels/tile_order.h"
 #include "../miniapps/devices.hpp"
@@ -228,8 +230,45 @@ void test_kernel_orderings() {
     }
 }
 
+// All-to-all-v plan: on accepted matrices the receive segments of every rank tile [0, column sum) and the send
+// segments [0, row sum) in order; the first broken rule wins.
+void test_alltoallv_plan() {
+  using namespace hpcp;
+  uint64_t x = 0x9E3779B97F4A7C15ull;
+  const auto next = [&x] { x ^= x << 13; x ^= x >> 7; x ^= x << 17; return x; };
+  for (int P = 1; P <= 16; ++P)
+    for (int trial = 0; trial < 20; ++trial) {
+      std::vector<int64_t> m(P * P);
+      for (auto& c : m) c = static_cast<int64_t>(next() % 5);
+      const int64_t cap = 4 * P;
+      CHECK(a2av_verdict(m.data(), P, cap, cap) == kA2avAccepted);
+      for (int r = 0; r < P; ++r) {
+        int64_t rows = 0, sent = 0;
+        for (int p = 0; p < P; ++p) {
+          CHECK(a2av_recv_offset(m.data(), P, p, r) == rows);
+          CHECK(a2av_send_offset(m.data(), P, r, p) == sent);
+          rows += m[p * P + r];
+          sent += m[r * P + p];
+        }
+        CHECK(rows <= cap && sent <= cap);
+      }
+      if (P > 1) {
+        m[P + 1] = cap + 1;                                                      // one count above the send capacity
+        CHECK(a2av_verdict(m.data(), P, cap, 1000 * cap) == kA2avSendCapacity);
+        CHECK(a2av_verdict(m.data(), P, 1000 * cap, cap) == kA2avRecvCapacity);
+        m[P * P - 1] = -1;                                                       // a negative beats every other rule
+        CHECK(a2av_verdict(m.data(), P, cap, cap) == kA2avNegative);
+      }
+    }
+  const int64_t big = INT64_MAX;                                                 // sums stop at the capacity: no overflow
+  const int64_t m2[4] = {big, big, big, big};
+  CHECK(a2av_verdict(m2, 2, big, big) == kA2avSendCapacity);
+  CHECK(a2av_first_rule(0) == kA2avAccepted && a2av_first_rule(0xE) == kA2avNegative && a2av_first_rule(9) == kA2avRecvCapacity);
+}
+
 int main() {
   test_kernel_orderings();
+  test_alltoallv_plan();
   test_rank_runtime();
   test_devices_and_dtypes();
   test_topology();

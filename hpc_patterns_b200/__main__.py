@@ -3,7 +3,7 @@
   concurency   compute-while-copy overlap benchmark (native driver in-process)
   peer2pear    P2P bandwidth, process-per-GPU (run under torchrun for >1 GPU)
   allreduce    allreduce miniapp, process-per-GPU (run under torchrun)
-  alltoall     equal-block all-to-all miniapp (push / pull kernels, nccl baseline), process-per-GPU (torchrun)
+  alltoall     all-to-all miniapp (push / pull kernels, nccl baseline; --counts: all-to-all-v), process-per-GPU (torchrun)
   halo         the miniapp loop as a halo exchange fused into a slab stencil — the flagship (run under torchrun)
   tp           tensor-parallel linear layers with the collective fused into the GEMM, vs cuBLAS + NCCL (torchrun)
   topology     fabric planes / rank->GPU mapping (JSON)

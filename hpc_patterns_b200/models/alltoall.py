@@ -11,6 +11,11 @@ receive buffer is block r of rank p's send buffer (↔ MPI_Alltoall, ncclAllToAl
 Check: before every iteration send block q of rank r gets the seeded pattern of (r, q) and the iteration, the receive
 buffer a poison seed no pair uses; after the last iteration every receive block p of rank r is checked against the
 seed of (p, r).  ``VirtualAlltoall`` drives ``world`` ranks from one process on one GPU.
+
+``AlltoallvMiniapp`` / ``VirtualAlltoallv`` are the all-to-all-v with device-resident counts (``bin/alltoall
+--counts``): rows of ``row_bytes``, per-peer int64 counts in peer-mapped memory, read by the kernel itself, so an
+``exchange(x, splits)`` never synchronises the host.  Its ``nccl`` algorithm is the stock MoE path: an all-to-all of
+the counts, ``.tolist()`` (a device-to-host sync), then ``all_to_all_single`` with split sizes.
 """
 from __future__ import annotations
 
@@ -21,7 +26,7 @@ from typing import List, Optional
 import torch
 
 from .. import native
-from ..ops.alltoall import all_to_all, as_blocks, check_args
+from ..ops.alltoall import (all_to_all, all_to_all_v, as_blocks, check_args, check_v_args, check_verdict)
 from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
@@ -212,6 +217,339 @@ class VirtualAlltoall:
             app.close()
 
 
+# ---------------------------------------------------------------------------------------------------- all-to-all-v ----
+V_ALGOS = ("push", "pull", "nccl")
+COUNT_KINDS = ("random", "skewed", "equal")
+TAIL_POISON_SEED = 0xC0DE0001
+_M64 = (1 << 64) - 1
+
+
+def _mix64(z: int) -> int:
+    z = (z + 0x9E3779B97F4A7C15) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def mean_rows(block_bytes: int, row_bytes: int) -> int:
+    """--block-bytes as the mean segment, rounded to rows (at least one)."""
+    return max(1, (block_bytes + row_bytes // 2) // row_bytes)
+
+
+def draw_counts(kind: str, world: int, mean: int, it: int) -> List[List[int]]:
+    """The count matrix of iteration ``it`` (M[p][q] rows from p to q), as bin/alltoall --counts draws it: ``random``
+    0 ... 2*mean per pair and one pair 0; ``skewed`` 2*mean into the hot rank it % P and at most mean/P into the others;
+    ``equal`` the mean for every pair.
+    Every matrix fits capacities of 2*P*mean rows."""
+    if kind not in COUNT_KINDS:
+        raise ValueError(f"--counts must be random, skewed or equal, not {kind}")
+    hot = it % world
+    m = [[0] * world for _ in range(world)]
+    for p in range(world):
+        for q in range(world):
+            h = _mix64((it << 16) | (p << 8) | q)
+            m[p][q] = (mean if kind == "equal" else (2 * mean if q == hot else h % (mean // world + 1))
+                       if kind == "skewed" else h % (2 * mean + 1))
+    if kind == "random":
+        i = _mix64(0xA11 ^ (it << 32)) % (world * world)
+        m[i // world][i % world] = 0
+    return m
+
+
+@dataclass
+class AlltoallvResult:
+    variant: str
+    world: int
+    block_bytes: int
+    row_bytes: int
+    counts: str
+    ms: float
+    mismatches: int
+    off_rank_bytes: float
+    max_bytes_into_a_rank: float
+    ctas: int = 0
+
+    def row(self) -> dict:
+        """One JSON row with the CLI's keys; GB/s is off-rank bytes summed over ranks / P / time."""
+        gbps = self.off_rank_bytes / self.world / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
+        return {"pattern": "alltoallv", "variant": self.variant, "ranks": self.world, "block_bytes": self.block_bytes,
+                "ms": self.ms, "GBps_sent_per_rank": gbps, "ctas": self.ctas, "mismatches": self.mismatches,
+                "counts": self.counts, "row_bytes": self.row_bytes,
+                "max_bytes_into_a_rank": self.max_bytes_into_a_rank}
+
+
+class AlltoallvMiniapp:
+    """One rank of the all-to-all-v.  ``capacity_rows`` rows of ``row_bytes`` are allocated for the send and for the
+    receive buffer and declared to the kernel (``send_capacity_rows`` / ``recv_capacity_rows``; they must be the same
+    on every rank).  ``exchange(x, splits)`` is the enqueue-only entry point; ``run()`` is the CLI's timed, checked loop."""
+
+    def __init__(self, comm: Comm, device: int, row_bytes: int, capacity_rows: int, algo: str = "push", ctas: int = 0,
+                 timeout_s: float = 30.0, _shared: Optional[dict] = None):
+        """``_shared``: buffers made by an in-process group (``VirtualAlltoallv``): ``pads``, ``send``, ``recv``,
+        ``counts``."""
+        if algo not in V_ALGOS:
+            raise ValueError(f"algo must be one of {V_ALGOS}")
+        check_v_args(comm.world, row_bytes, capacity_rows, capacity_rows)
+        if _shared is not None and algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
+        self.C = native()
+        self.comm, self.device = comm, device
+        self.rank, self.world = comm.rank, comm.world
+        self.algo, self.row_bytes, self.ctas = algo, int(row_bytes), ctas
+        self.send_capacity_rows = self.recv_capacity_rows = int(capacity_rows)
+        self.nbytes = int(capacity_rows) * self.row_bytes
+        self.launch_ctas = 0
+        self.generation = 0
+        self.matrix: List[List[int]] = []       # run(): the count matrix of the last initialised iteration
+        torch.cuda.set_device(device)
+        if _shared is not None:
+            self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
+            self.counts = _shared["counts"]
+        else:
+            self.pads = SignalPads(comm, device, timeout_s=timeout_s)
+            self.send = SymmetricBuffer(comm, self.nbytes, device, zero=False)
+            self.recv = SymmetricBuffer(comm, self.nbytes, device, zero=False)
+            self.counts = SymmetricBuffer(comm, 8 * self.world, device, zero=True)
+        dev = torch.device("cuda", device)
+        self.recv_counts = torch.zeros(self.world, dtype=torch.int64, device=dev)
+        self.verdict_word = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def rows(self, buf: SymmetricBuffer, dtype: torch.dtype = torch.uint8) -> torch.Tensor:
+        """``buf`` (send or recv) as [capacity_rows, row] of ``dtype``."""
+        return buf.tensor(dtype).view(self.nbytes // self.row_bytes, -1)
+
+    def run_once(self) -> None:
+        """Enqueue one all-to-all-v of what the send and counts buffers hold.  Precondition: every rank's send buffer
+        and counts are final and no rank still reads its receive buffer or recv_counts (``run()`` and ``exchange()``
+        put ``pads.device_barrier`` before it)."""
+        pads, st = self.pads, self._stream()
+        if self.algo == "nccl":
+            self._run_nccl()
+            return
+        pads.barrier_epoch += 1
+        self.launch_ctas = all_to_all_v(self.send.ptrs, self.recv.ptrs, self.counts.ptrs, self.recv_counts.data_ptr(),
+                                        self.verdict_word.data_ptr(), pads.buf.ptrs, pads.ticket_ptr,
+                                        pads.ticket_issued, self.rank, self.row_bytes, self.send_capacity_rows,
+                                        self.recv_capacity_rows, pads.barrier_epoch, pads.timeout_ns, pads.status_ptr,
+                                        self.ctas, self.device, st, self.algo == "pull")
+        pads.advance_tickets(self.launch_ctas)
+
+    def _run_nccl(self) -> None:
+        """The stock path: counts all-to-all, .tolist() (the host sync), all_to_all_single with split sizes."""
+        import torch.distributed as dist
+
+        send_counts = self.counts.tensor(torch.int64)
+        if self.world > 1:
+            dist.all_to_all_single(self.recv_counts, send_counts)
+        else:
+            self.recv_counts.copy_(send_counts)
+        ins, outs = send_counts.tolist(), self.recv_counts.tolist()
+        if min(ins + outs) < 0 or sum(ins) > self.send_capacity_rows or sum(outs) > self.recv_capacity_rows:
+            raise ValueError("all-to-all-v: the counts do not fit the capacities")
+        rb = self.row_bytes
+        src, dst = self.send.tensor()[: sum(ins) * rb], self.recv.tensor()[: sum(outs) * rb]
+        if self.world > 1:
+            dist.all_to_all_single(dst, src, [c * rb for c in outs], [c * rb for c in ins])
+        else:
+            dst.copy_(src)
+
+    def exchange(self, x: torch.Tensor, splits: torch.Tensor):
+        """Send the rows of ``x`` ([n, row_bytes worth of any dtype], n <= capacity) split by ``splits`` (device
+        int64[P]: rows for every rank, in rank order).  Enqueues the copies into the symmetric buffers, the device
+        barrier and the launch on the current stream and returns (received rows as [capacity, row] of x's dtype,
+        recv_counts); rows past sum(recv_counts) are not written.  Never synchronises the host; a refused count matrix
+        raises at ``check()``."""
+        if x.shape[0] > self.send_capacity_rows:
+            raise ValueError(f"all-to-all-v: x has {x.shape[0]} rows, the send capacity is {self.send_capacity_rows}")
+        xb = x.contiguous().view(torch.uint8).reshape(x.shape[0], -1)
+        if xb.shape[1] != self.row_bytes:
+            raise ValueError(f"all-to-all-v: a row of x must hold {self.row_bytes} bytes")
+        self.rows(self.send)[: x.shape[0]].copy_(xb)
+        self.counts.tensor(torch.int64).copy_(splits)
+        self.pads.device_barrier(self._stream())
+        self.run_once()
+        return self.rows(self.recv, x.dtype), self.recv_counts
+
+    def verdict(self) -> int:
+        """The verdict word of the last launch (synchronises)."""
+        torch.cuda.synchronize(self.device)
+        return int(self.verdict_word.item())
+
+    def check(self) -> None:
+        """Synchronise; RuntimeError on a failed device-side wait, ValueError with the verdict's words on a refused
+        count matrix."""
+        torch.cuda.synchronize(self.device)
+        self.pads.check()
+        if self.algo != "nccl":
+            check_verdict(self.verdict())
+
+    # ---- the CLI's seeded loop --------------------------------------------------------------------------------
+    def initialize(self, kind: str, mean: int) -> None:
+        """A new iteration: draw the count matrix, my send segments <- the pattern of (rank, q) at their packed rows,
+        the receive buffer <- the poison (past my total: the tail poison), my counts <- my row of the matrix."""
+        P, rb, st = self.world, self.row_bytes, self._stream()
+        m = self.matrix = draw_counts(kind, P, mean, self.generation)
+        total = sum(m[p][self.rank] for p in range(P))
+        cap = self.nbytes // rb
+        self.C.fill_pattern(self.recv.local_ptr + total * rb, (cap - total) * rb // 4, TAIL_POISON_SEED, st)
+        off = 0
+        for q in range(P):
+            self.C.fill_pattern(self.send.local_ptr + off * rb, m[self.rank][q] * rb // 4,
+                                pair_seed(self.generation, self.rank, q), st)
+            off += m[self.rank][q]
+        self.C.fill_pattern(self.recv.local_ptr, total * rb // 4, POISON_SEED, st)
+        self.counts.tensor(torch.int64).copy_(torch.tensor(m[self.rank], dtype=torch.int64))
+        self.recv_counts.fill_(-1)
+        self.generation += 1
+
+    def mismatches(self) -> int:
+        """Wrong words of the receive buffer against the last iteration (segment from p at its packed row, the tail
+        poison past the total), plus one per wrong recv_count and one for a non-zero verdict (kernels only)."""
+        P, rb, st, m = self.world, self.row_bytes, self._stream(), self.matrix
+        count = torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.device))
+        off = 0
+        for p in range(P):
+            self.C.verify_pattern(self.recv.local_ptr + off * rb, m[p][self.rank] * rb // 4,
+                                  pair_seed(self.generation - 1, p, self.rank), count.data_ptr(), stream=st)
+            off += m[p][self.rank]
+        self.C.verify_pattern(self.recv.local_ptr + off * rb, (self.nbytes // rb - off) * rb // 4, TAIL_POISON_SEED,
+                              count.data_ptr(), stream=st)
+        torch.cuda.synchronize(self.device)
+        bad = int(count.item())
+        bad += sum(int(a != b) for a, b in zip(self.recv_counts.tolist(), [m[p][self.rank] for p in range(P)]))
+        if self.algo != "nccl":
+            bad += int(int(self.verdict_word.item()) != 0)
+        return bad
+
+    def run(self, kind: str, block_bytes: int, iters: int = 5, warmup: int = 1) -> AlltoallvResult:
+        """``iters`` timed all-to-all-v's of freshly drawn counts with mean segments of ``block_bytes`` (rounded to
+        rows); capacity_rows must be at least 2 * P * mean."""
+        mean = mean_rows(block_bytes, self.row_bytes)
+        if 2 * self.world * mean > self.send_capacity_rows:
+            raise ValueError(f"all-to-all-v: --counts needs {2 * self.world * mean} rows of capacity")
+        stream = torch.cuda.current_stream(self.device)
+        e0 = torch.cuda.Event(enable_timing=True)
+        e1 = torch.cuda.Event(enable_timing=True)
+        best, traffic = float("inf"), (0.0, 0.0)
+        for it in range(warmup + iters):
+            self.initialize(kind, mean)
+            torch.cuda.synchronize(self.device)
+            self.comm.barrier()
+            self.pads.device_barrier(stream.cuda_stream)
+            e0.record(stream)
+            self.run_once()
+            e1.record(stream)
+            stream.synchronize()
+            self.pads.check()
+            t = self.comm.max(e0.elapsed_time(e1))
+            if it >= warmup and t < best:
+                best, traffic = t, _traffic(self.matrix, self.row_bytes)
+        bad = self.mismatches()
+        total_bad = int(self.comm.sum(bad))
+        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong words", flush=True)
+        return AlltoallvResult(self.algo, self.world, block_bytes, self.row_bytes, kind, best, total_bad, *traffic,
+                               ctas=self.launch_ctas)
+
+    def close(self) -> None:
+        torch.cuda.synchronize(self.device)
+        self.send.close()
+        self.recv.close()
+        self.counts.close()
+        self.pads.close()
+
+
+def _traffic(m: List[List[int]], row_bytes: int):
+    """(off-rank bytes of all ranks, the most bytes any rank receives)."""
+    P = len(m)
+    off = sum(m[p][q] for p in range(P) for q in range(P) if p != q) * row_bytes
+    into = max(sum(m[p][q] for p in range(P)) for q in range(P)) * row_bytes
+    return float(off), float(into)
+
+
+class VirtualAlltoallv:
+    """``world`` AlltoallvMiniapp ranks driven by ONE process on one GPU, as ``VirtualAlltoall`` does (co-resident
+    grids of at most ``sms // world`` CTAs, at most 8 ranks)."""
+
+    MAX_WORLD = 8
+
+    def __init__(self, world: int, row_bytes: int, capacity_rows: int, algo: str = "push", ctas: int = 0,
+                 device: int = 0, timeout_s: float = 10.0):
+        from ..parallel.local import LocalGroup
+
+        if not 1 <= world <= self.MAX_WORLD:
+            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
+        if algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        check_v_args(world, row_bytes, capacity_rows, capacity_rows)
+        C = native()
+        cap = max(1, C.sm_count(device) // world)
+        self.ctas = min(ctas, cap) if ctas > 0 else cap
+        self.world, self.row_bytes, self.capacity_rows, self.device = world, int(row_bytes), int(capacity_rows), device
+        self.group = LocalGroup(world, [device] * world)
+        pads = self.group.pads(timeout_s=timeout_s)
+        send = self.group.symmetric(self.capacity_rows * self.row_bytes, zero=False)
+        recv = self.group.symmetric(self.capacity_rows * self.row_bytes, zero=False)
+        counts = self.group.symmetric(8 * world, zero=True)
+        self.ranks: List[AlltoallvMiniapp] = [
+            AlltoallvMiniapp(self.group.comms[r], device, self.row_bytes, self.capacity_rows, algo, ctas=self.ctas,
+                             timeout_s=timeout_s,
+                             _shared={"pads": pads[r], "send": send[r], "recv": recv[r], "counts": counts[r]})
+            for r in range(world)]
+        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
+
+    def load(self, sends: List[torch.Tensor], counts: List) -> None:
+        """Rank r's send buffer <- ``sends[r]`` (rows of row_bytes, any dtype, at most capacity_rows) and its counts
+        <- ``counts[r]`` (P int64 values: rows for every rank).  The counts are not judged here: the kernel does."""
+        if len(sends) != self.world or len(counts) != self.world:
+            raise ValueError(f"one send tensor and one count row per rank ({self.world})")
+        torch.cuda.synchronize(self.device)
+        for app, s, c in zip(self.ranks, sends, counts):
+            b = s.contiguous().view(torch.uint8).reshape(-1)
+            if b.numel() > app.nbytes or b.numel() % self.row_bytes:
+                raise ValueError(f"a send tensor must hold whole rows of {self.row_bytes} bytes, at most "
+                                 f"{self.capacity_rows}")
+            app.send.tensor()[: b.numel()].copy_(b)
+            app.counts.tensor(torch.int64).copy_(torch.as_tensor(c, dtype=torch.int64).reshape(self.world))
+        torch.cuda.synchronize(self.device)
+
+    def run_once(self) -> None:
+        """One all-to-all-v: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one (it
+        stands in for the cross-rank barrier of the precondition)."""
+        for app, st in zip(self.ranks, self.streams):
+            with torch.cuda.device(app.device), torch.cuda.stream(st):
+                app.run_once()
+
+    def synchronize(self) -> None:
+        for st in self.streams:
+            st.synchronize()
+        for app in self.ranks:
+            app.pads.check()
+
+    def verdicts(self) -> List[int]:
+        """Every rank's verdict word of the last launch."""
+        self.synchronize()
+        return [int(app.verdict_word.item()) for app in self.ranks]
+
+    def results(self):
+        """Every rank's (received rows trimmed to its total as [total, row_bytes] uint8, recv_counts) on the host;
+        ValueError with the words of a refused count matrix."""
+        for v in self.verdicts():
+            check_verdict(v)
+        out = []
+        for app in self.ranks:
+            rc = app.recv_counts.cpu()
+            total = int(rc.sum())
+            out.append((app.rows(app.recv)[:total].cpu(), rc))
+        return out
+
+    def close(self) -> None:
+        for app in self.ranks:
+            app.close()
+
+
 def main(argv: Optional[List[str]] = None) -> int:
     """``torchrun --nproc-per-node N -m hpc_patterns_b200.models.alltoall [--block-bytes B] [--algo push|pull|nccl]``"""
     import argparse
@@ -223,8 +561,13 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--ctas", type=int, default=0)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--counts", default=None, choices=COUNT_KINDS,
+                    help="all-to-all-v with device-resident counts; --block-bytes is the mean segment")
+    ap.add_argument("--row-bytes", type=int, default=16, help="with --counts: bytes per row (default 16)")
     args = ap.parse_args(argv)
     comm = Comm()
+    if args.counts:
+        return _main_v(comm, args)
     app =AlltoallMiniapp(comm, comm.device, args.block_bytes, args.algo, ctas=args.ctas)
     res = app.run(args.iters, args.warmup)
     if comm.rank == 0:
@@ -241,3 +584,20 @@ def main(argv: Optional[List[str]] = None) -> int:
 
 if __name__ == "__main__":
     raise SystemExit(main())
+
+
+def _main_v(comm: Comm, args) -> int:
+    mean = mean_rows(args.block_bytes, args.row_bytes)
+    app = AlltoallvMiniapp(comm, comm.device, args.row_bytes, 2 * comm.world * mean, args.algo, ctas=args.ctas)
+    res = app.run(args.counts, args.block_bytes, args.iters, args.warmup)
+    if comm.rank == 0:
+        row = res.row()
+        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | alltoallv {args.algo} {args.counts} "
+              f"P={comm.world} B={args.block_bytes} R={args.row_bytes} | {row['GBps_sent_per_rank']:.1f} GB/s sent "
+              f"per rank", flush=True)
+        if args.json:
+            with open(args.json, "a") as f:
+                f.write(json.dumps(row) + "\n")
+    app.close()
+    comm.close()
+    return 0 if res.mismatches == 0 else 1
