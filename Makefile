@@ -39,6 +39,7 @@ cli: $(CLIS) aliases
 
 # Program names of the reference as links to the programs here; defaults follow the name (see each main()):
 #   <app>.<type> typed miniapps (CMakeLists.txt upstream), the three allreduce variants (allocation kind),
+#   reduce_scatter / allgather (the reduce-scatter of the allreduce miniapp, the all-gather of the alltoall miniapp),
 #   peer2pear_i / peer2pear_w (Isend/Irecv vs -DUSE_WIN builds, p2p/run.sh:4-5), sycl_con (run_sycl.sh:6),
 #   omp_host_threads / omp_nowait (one build per mode upstream, run_omp.sh:6-7; the mode is argv[1] here).
 aliases: $(CLIS)
@@ -48,6 +49,7 @@ aliases: $(CLIS)
 	          allreduce-mpi-sycl.float allreduce-mpi-sycl.int \
 	          allreduce-usm-mpi-omp-offload.float allreduce-map-mpi-omp-offload.float; do ln -sf allreduce bin/$$n; done
 	@for n in halo.float halo.double halo.bfloat16 halo.half; do ln -sf halo bin/$$n; done
+	@ln -sf allreduce bin/reduce_scatter; ln -sf alltoall bin/allgather
 	@ln -sf peer2pear bin/peer2pear_i; ln -sf peer2pear bin/peer2pear_w
 	@ln -sf concurency bin/sycl_con; ln -sf omp_con bin/omp_host_threads; ln -sf omp_con bin/omp_nowait
 

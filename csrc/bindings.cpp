@@ -847,6 +847,87 @@ PYBIND11_MODULE(_C, m) {
   });
   m.attr("ALL_TO_ALL_OVERLAP_ERROR") = kAllToAllOverlapError;
 
+  // ------------------------------------------------------- reduce-scatter ----
+  m.def(
+      "reduce_scatter",
+      [](const std::vector<uintptr_t>& send, uintptr_t recv, const std::vector<uintptr_t>& pads, uintptr_t ticket,
+         uint32_t ticket_base, int rank, size_t n, uint32_t barrier_epoch, uint64_t timeout_ns, uintptr_t status,
+         const std::string& dtype, int ctas, int device, uintptr_t stream, const std::string& op) {
+        ReduceScatterArgs a;
+        const ElemType type = elem_from(dtype);
+        a.op = op_from(op);
+        a.world = static_cast<int>(send.size());
+        if (const char* why = reduce_scatter_refusal(a.world, n, type)) throw std::invalid_argument(why);
+        if (!reduce_op_takes(a.op, type)) throw std::invalid_argument(reduce_op_type_error(a.op, type));
+        HPCP_REQUIRE(pads.size() == send.size(), "reduce-scatter: inconsistent rank lists");
+        for (int r = 0; r < a.world; ++r) {
+          a.send[r] = as_ptr<const void>(send[r]);
+          a.pads[r] = as_ptr<uint32_t>(pads[r]);
+        }
+        a.recv = as_ptr<void>(recv);
+        a.ticket = as_ptr<uint32_t>(ticket);
+        a.ticket_base = ticket_base;
+        a.rank = rank;
+        a.n = n;
+        a.barrier_epoch = barrier_epoch;
+        a.timeout_ns = timeout_ns;
+        a.status = as_ptr<uint32_t>(status);
+        return launch_reduce_scatter(a, type, ctas, device, as_stream(stream));
+      },
+      py::arg("send"), py::arg("recv"), py::arg("pads"), py::arg("ticket"), py::arg("ticket_base"), py::arg("rank"),
+      py::arg("n"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0, py::arg("status") = 0,
+      py::arg("dtype") = "float", py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0,
+      py::arg("op") = "sum",
+      "Reduce-scatter in one launch: my recv (n elements) <- op over p of segment `rank` of rank p's send buffer, "
+      "owner first; peer loads, one local store, ending with the node barrier.  Returns the CTAs launched.");
+  m.def("reduce_scatter_refusal", [](int world, size_t n, const std::string& dtype, const std::string& op) {
+    const ElemType type = elem_from(dtype);
+    if (const char* why = reduce_scatter_refusal(world, n, type)) return std::string(why);
+    const ReduceOp o = op_from(op);
+    return reduce_op_takes(o, type) ? std::string() : reduce_op_type_error(o, type);
+  }, py::arg("world"), py::arg("n"), py::arg("dtype"), py::arg("op") = "sum");
+  m.attr("REDUCE_SCATTER_COUNT_ERROR") = kReduceScatterCountError;
+  m.attr("REDUCE_SCATTER_WORLD_ERROR") = kReduceScatterWorldError;
+  m.attr("REDUCE_SCATTER_OVERLAP_ERROR") = kReduceScatterOverlapError;
+
+  // ----------------------------------------------------------- all-gather ----
+  m.def(
+      "all_gather",
+      [](const std::vector<uintptr_t>& send, const std::vector<uintptr_t>& recv, const std::vector<uintptr_t>& pads,
+         uintptr_t ticket, uint32_t ticket_base, int rank, size_t block_bytes, uint32_t barrier_epoch,
+         uint64_t timeout_ns, uintptr_t status, int ctas, int device, uintptr_t stream, bool pull) {
+        AllGatherArgs a;
+        a.world = static_cast<int>(send.size());
+        if (const char* why = all_gather_refusal(a.world, block_bytes)) throw std::invalid_argument(why);
+        HPCP_REQUIRE(recv.size() == send.size() && pads.size() == send.size(), "all-gather: inconsistent rank lists");
+        for (int r = 0; r < a.world; ++r) {
+          a.send[r] = as_ptr<const void>(send[r]);
+          a.recv[r] = as_ptr<void>(recv[r]);
+          a.pads[r] = as_ptr<uint32_t>(pads[r]);
+        }
+        a.ticket = as_ptr<uint32_t>(ticket);
+        a.ticket_base = ticket_base;
+        a.rank = rank;
+        a.block_bytes = block_bytes;
+        a.barrier_epoch = barrier_epoch;
+        a.timeout_ns = timeout_ns;
+        a.status = as_ptr<uint32_t>(status);
+        a.pull = pull;
+        return launch_all_gather(a, ctas, device, as_stream(stream));
+      },
+      py::arg("send"), py::arg("recv"), py::arg("pads"), py::arg("ticket"), py::arg("ticket_base"), py::arg("rank"),
+      py::arg("block_bytes"), py::arg("barrier_epoch"), py::arg("timeout_ns") = 0, py::arg("status") = 0,
+      py::arg("ctas") = 0, py::arg("device") = 0, py::arg("stream") = 0, py::arg("pull") = false,
+      "All-gather in one launch: block p of every recv <- rank p's send block (push: peer stores, pull: peer loads), "
+      "ending with the node barrier.  Returns the CTAs launched (advance the ticket by it).");
+  m.def("all_gather_refusal", [](int world, size_t block_bytes) {
+    const char* why = all_gather_refusal(world, block_bytes);
+    return std::string(why ? why : "");
+  });
+  m.attr("ALL_GATHER_BLOCK_ERROR") = kAllGatherBlockError;
+  m.attr("ALL_GATHER_WORLD_ERROR") = kAllGatherWorldError;
+  m.attr("ALL_GATHER_OVERLAP_ERROR") = kAllGatherOverlapError;
+
   // ----------------------------------------------------------- all-to-all-v ----
   // The plan rules (kernels/alltoallv_plan.h) on a row-major world x world count matrix.
   const auto count_matrix = [](const std::vector<int64_t>& m, int world) {

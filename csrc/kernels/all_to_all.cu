@@ -36,15 +36,22 @@ struct AllToAllDev {
   uint32_t* status;
 };
 
-template <bool kPull>
-__global__ void __launch_bounds__(512) all_to_all_kernel(const __grid_constant__ AllToAllDev a) {
+// kGather: the all-gather, the same walk with a source stride of 0.  Every rank's send buffer is ONE block, and block p
+// of every receive buffer is rank p's: push stores my block into slot `rank` of every rank's receive buffer, pull loads
+// rank p's block into my slot p.
+template <bool kPull, bool kGather>
+__device__ __forceinline__ void a2a_walk(const AllToAllDev& a) {
   constexpr int U = kA2aVectors;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t bv = a.block_vec;
   size_t off = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;  // offset in the current block
   for (int j = 0; j < a.world; ++j) {
     const int p = (a.rank + 1 + j) % a.world;
-    const uint4* src = kPull ? a.send[p] + a.rank * bv : a.send[a.rank] + p * bv;
+    const uint4* src;
+    if constexpr (kGather)
+      src = kPull ? a.send[p] : a.send[a.rank];
+    else
+      src = kPull ? a.send[p] + a.rank * bv : a.send[a.rank] + p * bv;
     uint4* dst = kPull ? a.recv[a.rank] + p * bv : a.recv[p] + a.rank * bv;
     for (; off + (U - 1) * stride < bv; off += U * stride) {
       uint4 x[U];
@@ -58,6 +65,16 @@ __global__ void __launch_bounds__(512) all_to_all_kernel(const __grid_constant__
     off -= bv;  // the same thread goes on in the next block of the walk
   }
   grid_then_node_barrier(a.ticket, a.ticket_target, a.pads, a.rank, a.world, a.barrier_epoch, a.timeout_ns, a.status);
+}
+
+template <bool kPull>
+__global__ void __launch_bounds__(512) all_to_all_kernel(const __grid_constant__ AllToAllDev a) {
+  a2a_walk<kPull, false>(a);
+}
+
+template <bool kPull>
+__global__ void __launch_bounds__(512) all_gather_kernel(const __grid_constant__ AllToAllDev a) {
+  a2a_walk<kPull, true>(a);
 }
 
 // ---------------------------------------------------------------------------------------------- all-to-all-v ----
@@ -175,6 +192,33 @@ int launch_all_to_all(const AllToAllArgs& args, int ctas, int device, cudaStream
   const int grid = grid_for(d.block_vec * args.world, 512, ctas > 0 ? ctas : sms * 2);
   d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
   const void* kernel = args.pull ? kernel_ptr(all_to_all_kernel<true>) : kernel_ptr(all_to_all_kernel<false>);
+  launch_512(kernel, grid, stream, d);
+  return grid;
+}
+
+int launch_all_gather(const AllGatherArgs& args, int ctas, int device, cudaStream_t stream) {
+  if (const char* why = all_gather_refusal(args.world, args.block_bytes)) HPCP_FAIL(why);
+  HPCP_REQUIRE(args.rank >= 0 && args.rank < args.world, "all-gather: rank out of range");
+  HPCP_REQUIRE(!byte_ranges_overlap(args.send[args.rank], args.block_bytes, args.recv[args.rank],
+                                    args.block_bytes * static_cast<size_t>(args.world)),
+               kAllGatherOverlapError);
+  AllToAllDev d{};
+  for (int p = 0; p < args.world; ++p) {
+    d.send[p] = static_cast<const uint4*>(args.send[p]);
+    d.recv[p] = static_cast<uint4*>(args.recv[p]);
+    d.pads[p] = args.pads[p];
+  }
+  d.ticket = args.ticket;
+  d.rank = args.rank;
+  d.world = args.world;
+  d.block_vec = args.block_bytes / 16;
+  d.barrier_epoch = args.barrier_epoch;
+  d.timeout_ns = args.timeout_ns;
+  d.status = args.status;
+  const int sms = device_sm_count(device);
+  const int grid = grid_for(d.block_vec * args.world, 512, ctas > 0 ? ctas : sms * 2);
+  d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
+  const void* kernel = args.pull ? kernel_ptr(all_gather_kernel<true>) : kernel_ptr(all_gather_kernel<false>);
   launch_512(kernel, grid, stream, d);
   return grid;
 }

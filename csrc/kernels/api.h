@@ -500,4 +500,80 @@ const char* all_to_all_v_verdict_words(uint32_t verdict);
 // Returns the number of CTAs launched (the caller advances its ticket counter by it).
 int launch_all_to_all_v(const AllToAllVArgs& args, int ctas, int device, cudaStream_t stream);
 
+// Whether the byte ranges [a, a + na) and [b, b + nb) share a byte (the in-place refusal of the collectives below).
+inline bool byte_ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+  const auto x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return !(x + na <= y || y + nb <= x);
+}
+
+// --------------------------------------------------------- reduce-scatter ----
+// (↔ MPI_Reduce_scatter_block, ncclReduceScatter, reduce_scatter_tensor.)  Rank p's send buffer holds `world` segments
+// of n elements; afterwards rank r's receive buffer of n elements holds op over p of segment r of rank p's send buffer,
+// combined owner first in every element, ((S_r[r] o S_{r+1}[r]) o ...) o S_{r+P-1}[r] (ranks mod P).  The 16-bit
+// floating sum and prod accumulate in fp32 and round once; NaN results are canonical; loc pairs get zero padding;
+// world 1 copies segment 0 through that fold.  Rank r loads segment r from every rank over the peer mapping and stores
+// only into its own receive buffer; one launch ends with the node barrier, so completion means my result has landed and
+// every peer has finished reading my send buffer.  Precondition as two-shot's; send is never written.
+struct ReduceScatterArgs {
+  const void* send[kApiMaxRanks] = {nullptr};  // peer-mapped send buffers of every rank (world * n elements)
+  void* recv = nullptr;                        // my receive buffer (n elements); must not overlap my send buffer
+  uint32_t* pads[kApiMaxRanks] = {nullptr};    // signal pads of every rank
+  uint32_t* ticket = nullptr;
+  uint32_t ticket_base = 0;
+  int rank = 0;
+  int world = 0;                               // 1 ... kApiMaxRanks
+  size_t n = 0;                                // elements per segment; n * elem_size a positive multiple of 16
+  uint32_t barrier_epoch = 0;
+  uint64_t timeout_ns = 0;
+  uint32_t* status = nullptr;
+  ReduceOp op = ReduceOp::kSum;                // any op the allreduce takes for the type (dispatch_op's refusals)
+};
+constexpr const char* kReduceScatterCountError =
+    "reduce-scatter: a segment must be a positive multiple of 16 bytes (n * elem_size)";
+constexpr const char* kReduceScatterWorldError = "reduce-scatter: world must be between 1 and 16 ranks";
+constexpr const char* kReduceScatterOverlapError =
+    "reduce-scatter: the send and receive buffers must not overlap (no in-place operation)";
+// nullptr if (world, n, type) are accepted, else the refusal's words.  The op is refused with dispatch_op's words
+// (reduce_op_takes / reduce_op_type_error, dtype_traits.h).
+inline const char* reduce_scatter_refusal(int world, size_t n, ElemType type) {
+  if (n == 0 || n * elem_size(type) % 16 != 0) return kReduceScatterCountError;
+  if (world < 1 || world > kApiMaxRanks) return kReduceScatterWorldError;
+  return nullptr;
+}
+// Returns the number of CTAs launched (the caller advances its ticket counter by it).
+int launch_reduce_scatter(const ReduceScatterArgs& args, ElemType type, int ctas, int device, cudaStream_t stream);
+
+// ------------------------------------------------------------- all-gather ----
+// (↔ MPI_Allgather, ncclAllGather, all_gather_into_tensor.)  Bytes, as the all-to-all moves them.  Rank p holds one
+// send block of block_bytes; afterwards block p of every rank's receive buffer (world * block_bytes) is a byte copy of
+// rank p's send block, p = r included.  The all-to-all's walk with a source stride of 0: push stores my block into
+// slot `rank` of every rank's receive buffer, pull loads rank p's block into my slot p; staggered, local block last.
+// Completion, precondition and the never-written send buffer as the all-to-all's.
+struct AllGatherArgs {
+  const void* send[kApiMaxRanks] = {nullptr};  // peer-mapped send blocks of every rank
+  void* recv[kApiMaxRanks] = {nullptr};        // peer-mapped receive buffers of every rank
+  uint32_t* pads[kApiMaxRanks] = {nullptr};
+  uint32_t* ticket = nullptr;
+  uint32_t ticket_base = 0;
+  int rank = 0;
+  int world = 0;                               // 1 ... kApiMaxRanks
+  size_t block_bytes = 0;                      // a positive multiple of 16
+  uint32_t barrier_epoch = 0;
+  uint64_t timeout_ns = 0;
+  uint32_t* status = nullptr;
+  bool pull = false;
+};
+constexpr const char* kAllGatherBlockError = "all-gather: block_bytes must be a positive multiple of 16";
+constexpr const char* kAllGatherWorldError = "all-gather: world must be between 1 and 16 ranks";
+constexpr const char* kAllGatherOverlapError =
+    "all-gather: the send and receive buffers must not overlap (no in-place operation)";
+// nullptr if (world, block_bytes) is accepted, else the refusal's words.
+inline const char* all_gather_refusal(int world, size_t block_bytes) {
+  if (block_bytes == 0 || block_bytes % 16 != 0) return kAllGatherBlockError;
+  if (world < 1 || world > kApiMaxRanks) return kAllGatherWorldError;
+  return nullptr;
+}
+// Returns the number of CTAs launched (the caller advances its ticket counter by it).
+int launch_all_gather(const AllGatherArgs& args, int ctas, int device, cudaStream_t stream);
+
 }  // namespace hpcp

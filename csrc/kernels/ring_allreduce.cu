@@ -369,6 +369,34 @@ int launch_allreduce_two_shot(const TwoShotArgs& args, ElemType type, int ctas, 
   return grid;
 }
 
+int launch_reduce_scatter(const ReduceScatterArgs& args, ElemType type, int ctas, int device, cudaStream_t stream) {
+  if (const char* why = reduce_scatter_refusal(args.world, args.n, type)) HPCP_FAIL(why);
+  HPCP_REQUIRE(args.rank >= 0 && args.rank < args.world, "reduce-scatter: rank out of range");
+  const void* kernel = allreduce_kernels(type, args.op).reduce_scatter[two_shot_shape(args.world)];  // op refusals
+  const size_t seg_bytes = args.n * elem_size(type);
+  HPCP_REQUIRE(!byte_ranges_overlap(args.send[args.rank], seg_bytes * static_cast<size_t>(args.world), args.recv,
+                                    seg_bytes),
+               kReduceScatterOverlapError);
+  TwoShotDev d{};  // two-shot's block: va = the send buffers, vc[rank] = my receive buffer (two_shot_body's kScatter)
+  for (int p = 0; p < args.world; ++p) {
+    d.va[p] = static_cast<const uint4*>(args.send[p]);
+    d.pads[p] = args.pads[p];
+  }
+  d.vc[args.rank] = static_cast<uint4*>(args.recv);
+  d.ticket = args.ticket;
+  d.rank = args.rank;
+  d.world = args.world;
+  d.slice_vec = seg_bytes / 16;
+  d.barrier_epoch = args.barrier_epoch;
+  d.timeout_ns = args.timeout_ns;
+  d.status = args.status;
+  const int sms = device_sm_count(device);
+  const int grid = grid_for(d.slice_vec, 512, ctas > 0 ? ctas : sms * 2);
+  d.ticket_target = args.ticket_base + static_cast<uint32_t>(grid);
+  launch_512(kernel, grid, stream, d);
+  return grid;
+}
+
 int launch_allreduce_nvls(const NvlsArgs& args, ElemType type, int ctas, int device,
                           cudaStream_t stream) {
   HPCP_REQUIRE(args.world >= 1 && args.world <= kApiMaxRanks, "nvls: world out of range");

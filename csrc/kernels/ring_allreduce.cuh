@@ -442,7 +442,9 @@ __device__ __forceinline__ void grid_then_node_barrier(uint32_t* ticket, uint32_
 // ((VA[s] o VA[s+1]) o ...); the tail loop does too with kOwnerFirstTail, else it goes rank 0 first.
 // kOwnerFirstTail is false for the sum only.  Its tail adding rank 0 first, unlike its main blocks, is part of the
 // sum's results (a floating sum's last bits depend on the order) and of its fingerprinted instructions.
-template <class Op, int W, int U, bool kOwnerFirstTail>
+// kScatter: the stand-alone reduce-scatter.  va[p] is rank p's send buffer and vc[rank] my receive buffer of ONE
+// segment: the result of segment `rank` is stored there only, at offset 0 (kOwnerFirstTail is true).
+template <class Op, int W, int U, bool kOwnerFirstTail, bool kScatter = false>
 __device__ __forceinline__ void two_shot_body(const TwoShotDev& a) {
   const size_t base = static_cast<size_t>(a.rank) * a.slice_vec;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -464,20 +466,28 @@ __device__ __forceinline__ void two_shot_body(const TwoShotDev& a) {
 #pragma unroll
         for (int u = 0; u < U; ++u) x[0][u] = Op::combine(x[0][u], x[q][u]);
       }
+    if constexpr (kScatter) {
 #pragma unroll
-    for (int q = 0; q < W; ++q)
-      if (q < a.world) {
-        const int p = (a.rank + q) % a.world;
+      for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[a.rank] + i + u * blockDim.x, x[0][u]);
+    } else {
 #pragma unroll
-        for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[p] + base + i + u * blockDim.x, x[0][u]);
-      }
+      for (int q = 0; q < W; ++q)
+        if (q < a.world) {
+          const int p = (a.rank + q) % a.world;
+#pragma unroll
+          for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[p] + base + i + u * blockDim.x, x[0][u]);
+        }
+    }
   }
   size_t i = n_blocks * block_vec + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   for (; i < a.slice_vec; i += stride) {
     if (kOwnerFirstTail) {
       uint4 acc = ptx::ld_peer_v4(a.va[a.rank] + base + i);
       for (int q = 1; q < a.world; ++q) acc = Op::combine(acc, ptx::ld_peer_v4(a.va[(a.rank + q) % a.world] + base + i));
-      for (int p = 0; p < a.world; ++p) ptx::st_stream_v4(a.vc[p] + base + i, acc);
+      if constexpr (kScatter)
+        ptx::st_stream_v4(a.vc[a.rank] + i, acc);
+      else
+        for (int p = 0; p < a.world; ++p) ptx::st_stream_v4(a.vc[p] + base + i, acc);
     } else {
       uint4 acc = ptx::ld_peer_v4(a.va[0] + base + i);
       for (int p = 1; p < a.world; ++p) acc = Op::combine(acc, ptx::ld_peer_v4(a.va[p] + base + i));
@@ -493,10 +503,17 @@ __global__ void __launch_bounds__(512) two_shot_kernel(const __grid_constant__ T
   two_shot_body<Op, W, U, kOwnerFirstTail>(a);
 }
 
+// The stand-alone reduce-scatter: two-shot's loads and combine order (owner first, the tail too), one store.
+template <class Op, int W, int U>
+__global__ void __launch_bounds__(512) reduce_scatter_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_body<Op, W, U, true, true>(a);
+}
+
 // Two-shot for the 16-bit floating types: same loads, stores and barrier as two_shot_body, but every lane is widened
 // to fp32 (the accumulator A, a Wide8) and the P inputs are combined owner first, ((VA[s] o VA[s+1]) o ...) o
 // VA[s+P-1] (ranks mod P), in the main blocks and in the tail loop alike; the result is rounded once to T.
-template <class A, int W, int U>
+// kScatter as in two_shot_body.
+template <class A, int W, int U, bool kScatter = false>
 __device__ __forceinline__ void two_shot_f32_body(const TwoShotDev& a) {
   const size_t base = static_cast<size_t>(a.rank) * a.slice_vec;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -521,13 +538,18 @@ __device__ __forceinline__ void two_shot_f32_body(const TwoShotDev& a) {
         if (q < a.world) s.add(x[q][u]);
       x[0][u] = s.round();
     }
+    if constexpr (kScatter) {
 #pragma unroll
-    for (int q = 0; q < W; ++q)
-      if (q < a.world) {
-        const int p = (a.rank + q) % a.world;
+      for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[a.rank] + i + u * blockDim.x, x[0][u]);
+    } else {
 #pragma unroll
-        for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[p] + base + i + u * blockDim.x, x[0][u]);
-      }
+      for (int q = 0; q < W; ++q)
+        if (q < a.world) {
+          const int p = (a.rank + q) % a.world;
+#pragma unroll
+          for (int u = 0; u < U; ++u) ptx::st_stream_v4(a.vc[p] + base + i + u * blockDim.x, x[0][u]);
+        }
+    }
   }
   size_t i = n_blocks * block_vec + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   for (; i < a.slice_vec; i += stride) {
@@ -535,7 +557,10 @@ __device__ __forceinline__ void two_shot_f32_body(const TwoShotDev& a) {
     s.set(ptx::ld_peer_v4(a.va[a.rank] + base + i));
     for (int q = 1; q < a.world; ++q) s.add(ptx::ld_peer_v4(a.va[(a.rank + q) % a.world] + base + i));
     const uint4 r = s.round();
-    for (int p = 0; p < a.world; ++p) ptx::st_stream_v4(a.vc[p] + base + i, r);
+    if constexpr (kScatter)
+      ptx::st_stream_v4(a.vc[a.rank] + i, r);
+    else
+      for (int p = 0; p < a.world; ++p) ptx::st_stream_v4(a.vc[p] + base + i, r);
   }
   grid_then_node_barrier(a.ticket, a.ticket_target, a.pads, a.rank, a.world, a.barrier_epoch,
                          a.timeout_ns, a.status);
@@ -544,6 +569,11 @@ __device__ __forceinline__ void two_shot_f32_body(const TwoShotDev& a) {
 template <class Acc, int W, int U>
 __global__ void __launch_bounds__(512) two_shot_f32_kernel(const __grid_constant__ TwoShotDev a) {
   two_shot_f32_body<Acc, W, U>(a);
+}
+
+template <class Acc, int W, int U>
+__global__ void __launch_bounds__(512) reduce_scatter_f32_kernel(const __grid_constant__ TwoShotDev a) {
+  two_shot_f32_body<Acc, W, U, true>(a);
 }
 
 // The combine policies two-shot runs through two_shot_f32_kernel, and the accumulator (a Wide8) each one uses: the sum
@@ -615,6 +645,7 @@ struct AllreduceKernels {
   const void* ring[2][2];                    // [pull][two slots]: RingDev (push) or RingPullDev (pull)
   const void* rsag;                          // RingRsAgDev
   const void* two_shot[kTwoShotShapeCount];  // [two_shot_shape(world)]: TwoShotDev
+  const void* reduce_scatter[kTwoShotShapeCount];  // [two_shot_shape(world)]: TwoShotDev, two_shot_body's kScatter
 };
 
 namespace {
@@ -633,12 +664,22 @@ const void* two_shot_kernel_of() {
     return kernel_ptr(two_shot_kernel<Op, W, U, kOwnerFirstTail>);
 }
 
+template <class Op, int I>
+const void* reduce_scatter_kernel_of() {
+  constexpr int W = kTwoShotShapes[I].w, U = kTwoShotShapes[I].u;
+  if constexpr (TwoShotInF32<Op>::value)
+    return kernel_ptr(reduce_scatter_f32_kernel<typename TwoShotInF32<Op>::acc, W, U>);
+  else
+    return kernel_ptr(reduce_scatter_kernel<Op, W, U>);
+}
+
 template <class Op, bool kOverwrite, bool kOwnerFirstTail, int... I>
 AllreduceKernels allreduce_kernels_of(std::integer_sequence<int, I...>) {
   return {{{kernel_ptr(ring_push_kernel<Op, false, kOverwrite>), kernel_ptr(ring_push_kernel<Op, true, kOverwrite>)},
            {kernel_ptr(ring_pull_kernel<Op, false, kOverwrite>), kernel_ptr(ring_pull_kernel<Op, true, kOverwrite>)}},
           kernel_ptr(ring_rsag_kernel<Op>),
-          {two_shot_kernel_of<Op, kOwnerFirstTail, I>()...}};
+          {two_shot_kernel_of<Op, kOwnerFirstTail, I>()...},
+          {reduce_scatter_kernel_of<Op, I>()...}};
 }
 // Every kernel of the combine policy Op.
 template <class Op, bool kOverwrite, bool kOwnerFirstTail>

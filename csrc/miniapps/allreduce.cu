@@ -38,6 +38,16 @@
 // maxloc (rank 0 holds (0, -P-10), rank r (1, 2r-3), VC starts at (7, -1000)) -> (1, -1), minloc with the values 1 and 0
 // (VC (-7, -1000)) -> (0, -1); at P = 1 VC is VA.  A tie broken towards the larger index, an unsigned index compare, a
 // selection by index alone and a kernel that reads VC each give another pair.
+//
+// Run as `reduce_scatter` (a program-name link to this binary) it is the stand-alone reduce-scatter (↔
+// MPI_Reduce_scatter_block, ncclReduceScatter; launch_reduce_scatter): every rank's send buffer holds P segments of n
+// elements (-p k: 2^k elements padded to P whole 16-byte segments, as -a pads) and rank r receives op over p of segment r
+// of rank p's, owner first.  Options: --type, --op, -p, -n, --iters, --warmup, --ctas, --json, --cpu; device memory
+// only, so -a, --algo, --coll, --slots, --pull, -H, -S, -R (and --chunk, --map-alias, --profile-relaunch) are usage
+// errors.  Check: the allreduce's constant data, except that for the sum segment q of rank p holds p + (q mod 8), so
+// rank r expects P(P-1)/2 + P*(r mod 8) (exact in every type up to P = 16) and a rank that reduced a neighbour's segment
+// fails; the receive buffer starts as a value no rank expects (251 for the sum, whose vc_init 0 is rank 0's result at
+// P = 1), and the send buffer is checked unchanged.  --cpu runs the same owner-first fold on host threads.
 #include <cuda_profiler_api.h>
 #include <getopt.h>
 
@@ -789,6 +799,276 @@ int run_on_host(const Config& cfg) {
     dispatch_elem(cfg.type, [&](auto tag) { rc = run_on_host_typed<decltype(tag), ArithHost<decltype(tag)>>(cfg); });
   return rc;
 }
+
+// ---------------------------------------------------------------------------------------------- reduce-scatter ----
+constexpr double kRsSumPoison = 251;  // above every rank's sum up to P = 16 (at most 232), exact in every type
+
+double rs_input(ReduceOp op, int p, int q, int P) { return op == ReduceOp::kSum ? p + q % 8 : op_input(op, p, P); }
+double rs_expected(ReduceOp op, int r, int P) {
+  return op == ReduceOp::kSum ? 0.5 * P * (P - 1) + P * (r % 8) : op_expected(op, P);
+}
+double rs_poison(ReduceOp op, int P) { return op == ReduceOp::kSum ? kRsSumPoison : op_vc_init(op, P); }
+
+// Elements per segment: 2^log2 padded to P whole 16-byte segments, divided by P.
+size_t rs_segment(const Config& cfg, int P) {
+  const size_t unit = 16 / elem_size(cfg.type) * static_cast<size_t>(P);
+  const size_t total = ((size_t{1} << cfg.log2_elems) + unit - 1) / unit * unit;
+  return total / P;
+}
+
+void rs_report(const Config& cfg, int P, size_t n, double ms, unsigned long long bad, bool host) {
+  const double sent = static_cast<double>(P - 1) * n * elem_size(cfg.type);
+  const double gbps = ms > 0 ? sent / (ms * 1e-3) * 1e-9 : 0.0;
+  const char* algo = host ? "host" : "direct";
+  std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << ms << " ms | reduce_scatter " << algo << " "
+            << elem_type_name(cfg.type) << " P=" << P << " n=" << n << " op=" << reduce_op_name(cfg.op)
+            << (host ? " host-threads" : "") << " | " << gbps << " GB/s sent per rank" << std::endl;
+  if (!cfg.json_path.empty()) {
+    if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
+      std::fprintf(f,
+                   "{\"pattern\":\"reduce_scatter\",\"algo\":\"%s\",\"type\":\"%s\",\"op\":\"%s\",\"ranks\":%d,"
+                   "\"elements\":%zu,\"ms\":%.6f,\"GBps_sent_per_rank\":%.3f,\"mismatches\":%llu}\n",
+                   algo, elem_type_name(cfg.type), reduce_op_name(cfg.op), P, n, ms, gbps, bad);
+      std::fclose(f);
+    }
+  }
+}
+
+void rs_print_verdict(int me, unsigned long long bad) {
+  const std::string line = bad == 0 ? "Passed " + std::to_string(me) + "\n"
+                                    : "FAILED " + std::to_string(me) + ": " + std::to_string(bad) + " wrong elements\n";
+  std::cout << line << std::flush;
+}
+
+struct RsShared {
+  Config cfg;
+  NodeMemory* mem = nullptr;
+  size_t n = 0;
+  SymmetricBuffer send, recv, pads;
+  double best_ms = 0;
+  unsigned long long total_bad = 0;
+};
+
+// Fill n elements at p with the constant datum of (op, rank p's value x) / (pair) on the stream.
+void rs_fill(void* p, size_t n, ReduceOp op, int rank, int P, double x, const Config& cfg, cudaStream_t st) {
+  if (elem_type_is_pair(cfg.type)) {
+    const LocDatum d = loc_input(op, rank, P);
+    launch_init_pair(p, n, d.value, d.index, cfg.type, st);
+  } else {
+    launch_init3(p, nullptr, nullptr, n, x, 0, 0, cfg.type, st);
+  }
+}
+
+void rs_rank_main(RankCtx& ctx, RsShared& sh) {
+  const Config& cfg = sh.cfg;
+  const int me = ctx.rank, P = ctx.world;
+  const int dev = sh.mem->device(me);
+  HPCP_CUDA(cudaSetDevice(dev));
+  cudaStream_t stream;
+  HPCP_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  std::vector<uint32_t*> pads;
+  for (int r = 0; r < P; ++r) pads.push_back(static_cast<uint32_t*>(sh.pads.ptr[r]));
+  uint32_t* status = pads[me] + kPadWords;
+  const size_t n = sh.n, seg = n * elem_size(cfg.type);
+  unsigned char* my_send = static_cast<unsigned char*>(sh.send.ptr[me]);
+  void* my_recv = sh.recv.ptr[me];
+  const bool pair = elem_type_is_pair(cfg.type);
+  unsigned long long* count = nullptr;
+  HPCP_CUDA(cudaMalloc(&count, sizeof *count));
+  cudaEvent_t e0, e1;
+  HPCP_CUDA(cudaEventCreate(&e0));
+  HPCP_CUDA(cudaEventCreate(&e1));
+  uint32_t barrier_epoch = 0, ticket_issued = 0;
+  double best = std::numeric_limits<double>::max();
+  for (int it = 0; it < cfg.warmup + cfg.iters; ++it) {
+    NvtxRange range(it < cfg.warmup ? "reduce_scatter warm-up" : "reduce_scatter timed");
+    for (int q = 0; q < P; ++q) rs_fill(my_send + q * seg, n, cfg.op, me, P, rs_input(cfg.op, me, q, P), cfg, stream);
+    if (pair) {
+      const LocDatum c = loc_vc_init(cfg.op);
+      launch_init_pair(my_recv, n, c.value, c.index, cfg.type, stream);
+    } else {
+      launch_init3(my_recv, nullptr, nullptr, n, rs_poison(cfg.op, P), 0, 0, cfg.type, stream);
+    }
+    HPCP_CUDA(cudaStreamSynchronize(stream));
+    ctx.barrier();
+    launch_barrier_all(pads.data(), me, P, ++barrier_epoch, cfg.timeout_ns, status, stream);
+    HPCP_CUDA(cudaEventRecord(e0, stream));
+    ReduceScatterArgs a;
+    for (int r = 0; r < P; ++r) {
+      a.send[r] = sh.send.ptr[r];
+      a.pads[r] = pads[r];
+    }
+    a.recv = my_recv;
+    a.ticket = pads[me] + kPadLocal;
+    a.ticket_base = ticket_issued;
+    a.rank = me;
+    a.world = P;
+    a.n = n;
+    a.barrier_epoch = ++barrier_epoch;
+    a.timeout_ns = cfg.timeout_ns;
+    a.status = status;
+    a.op = cfg.op;
+    ticket_issued += static_cast<uint32_t>(launch_reduce_scatter(a, cfg.type, cfg.ctas, dev, stream));
+    HPCP_CUDA(cudaEventRecord(e1, stream));
+    HPCP_CUDA(cudaStreamSynchronize(stream));
+    uint32_t st = 0;
+    HPCP_CUDA(cudaMemcpy(&st, status, sizeof st, cudaMemcpyDeviceToHost));
+    HPCP_REQUIRE(st == 0, "rank " + std::to_string(me) + ": device-side wait timed out");
+    float ms = 0;
+    HPCP_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    const double t = ctx.max(ms);
+    if (it >= cfg.warmup) best = std::min(best, t);
+  }
+  // The result, and every send segment unchanged.
+  HPCP_CUDA(cudaMemsetAsync(count, 0, sizeof *count, stream));
+  if (pair) {
+    const LocDatum w = loc_expected(cfg.op, P), x = loc_input(cfg.op, me, P);
+    launch_count_pair_mismatch(my_recv, n, w.value, w.index, cfg.type, count, stream);
+    for (int q = 0; q < P; ++q) launch_count_pair_mismatch(my_send + q * seg, n, x.value, x.index, cfg.type, count, stream);
+  } else {
+    launch_count_mismatch(my_recv, n, rs_expected(cfg.op, me, P), cfg.type, count, stream);
+    for (int q = 0; q < P; ++q)
+      launch_count_mismatch(my_send + q * seg, n, rs_input(cfg.op, me, q, P), cfg.type, count, stream);
+  }
+  unsigned long long bad = 0;
+  HPCP_CUDA(cudaMemcpyAsync(&bad, count, sizeof bad, cudaMemcpyDeviceToHost, stream));
+  HPCP_CUDA(cudaStreamSynchronize(stream));
+  const double all_bad = ctx.sum(static_cast<double>(bad));
+  rs_print_verdict(me, bad);
+  if (me == 0) {
+    sh.best_ms = best;
+    sh.total_bad = static_cast<unsigned long long>(all_bad);
+  }
+  (void)cudaFree(count);
+  (void)cudaEventDestroy(e0);
+  (void)cudaEventDestroy(e1);
+  (void)cudaStreamDestroy(stream);
+}
+
+// The host twin: rank r folds segment r of every rank owner first, ((S_r[r] o S_{r+1}[r]) o ...), the 16-bit sum and
+// prod in fp32 rounded once, as the kernel does; H supplies the pair or arithmetic constant data.
+template <typename T>
+T rs_host_datum(ReduceOp op, int p, int q, int P) {
+  if constexpr (std::is_class<T>::value && !std::is_same<T, __nv_bfloat16>::value && !std::is_same<T, __half>::value) {
+    const LocDatum d = loc_input(op, p, P);
+    return host_pair<typename T::value_type>(d.value, d.index);
+  } else {
+    return static_cast<T>(rs_input(op, p, q, P));
+  }
+}
+template <typename T>
+bool rs_host_expected(const T& v, ReduceOp op, int r, int P) {
+  if constexpr (std::is_class<T>::value && !std::is_same<T, __nv_bfloat16>::value && !std::is_same<T, __half>::value) {
+    return PairHost<typename T::value_type>::is_expected(v, op, P);
+  } else {
+    return std::abs(host_to_double(v) - host_to_double(static_cast<T>(rs_expected(op, r, P)))) < 1e-6;
+  }
+}
+
+template <typename T>
+int rs_run_on_host_typed(const Config& cfg) {
+  const int P = cfg.ranks > 0 ? cfg.ranks : 4;
+  const size_t n = rs_segment(cfg, P);
+  const ReduceOp op = cfg.op;
+  std::vector<std::vector<T>> send(P), recv(P);
+  double best = std::numeric_limits<double>::max();
+  unsigned long long total_bad = 0;
+  run_ranks(P, [&](RankCtx& ctx) {
+    const int me = ctx.rank;
+    send[me].resize(P * n);
+    recv[me].resize(n);
+    for (int it = 0; it < cfg.warmup + cfg.iters; ++it) {
+      for (int q = 0; q < P; ++q) std::fill(send[me].begin() + q * n, send[me].begin() + (q + 1) * n, rs_host_datum<T>(op, me, q, P));
+      if constexpr (std::is_class<T>::value && !std::is_same<T, __nv_bfloat16>::value && !std::is_same<T, __half>::value)
+        std::fill(recv[me].begin(), recv[me].end(), PairHost<typename T::value_type>::vc_init(op, P));
+      else
+        std::fill(recv[me].begin(), recv[me].end(), static_cast<T>(rs_poison(op, P)));
+      ctx.barrier();
+      const auto t0 = std::chrono::steady_clock::now();
+      const T* own = send[me].data() + me * n;
+      for (size_t i = 0; i < n; ++i) {
+        if constexpr (kSum16InF32<T>) {
+          if (op == ReduceOp::kSum || op == ReduceOp::kProd) {
+            float acc = static_cast<float>(host_to_double(own[i]));
+            for (int k = 1; k < P; ++k) {
+              const float x = static_cast<float>(host_to_double(send[(me + k) % P][me * n + i]));
+              acc = op == ReduceOp::kSum ? acc + x : acc * x;
+            }
+            recv[me][i] = std::isnan(acc) ? host_canonical_nan<T>() : host_from_float<T>(acc);
+            continue;
+          }
+        }
+        T acc = own[i];
+        for (int k = 1; k < P; ++k) acc = host_combine(op, acc, send[(me + k) % P][me * n + i]);
+        recv[me][i] = acc;
+      }
+      ctx.barrier();  // the node barrier: every rank has finished reading my send buffer
+      const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+      const double t = ctx.max(ms);
+      if (it >= cfg.warmup) best = std::min(best, t);
+    }
+    unsigned long long bad = 0;
+    for (size_t i = 0; i < n; ++i) bad += !rs_host_expected(recv[me][i], op, me, P);
+    for (int q = 0; q < P; ++q)
+      for (size_t i = 0; i < n; ++i) {
+        const T want = rs_host_datum<T>(op, me, q, P);
+        if constexpr (std::is_class<T>::value && !std::is_same<T, __nv_bfloat16>::value && !std::is_same<T, __half>::value)
+          bad += std::memcmp(&send[me][q * n + i].value, &want.value, sizeof want.value) != 0 ||
+                 send[me][q * n + i].index != want.index;  // a struct copy need not keep the padding bytes
+        else
+          bad += std::memcmp(&send[me][q * n + i], &want, sizeof want) != 0;
+      }
+    const double all_bad = ctx.sum(static_cast<double>(bad));
+    rs_print_verdict(me, bad);
+    if (me == 0) total_bad = static_cast<unsigned long long>(all_bad);
+  });
+  rs_report(cfg, P, n, best, total_bad, true);
+  return total_bad == 0 ? 0 : 1;
+}
+
+int run_reduce_scatter(Config cfg) {
+  if (elem_type_is_pair(cfg.type) && !cfg.op_given) cfg.op = ReduceOp::kMaxLoc;
+  HPCP_REQUIRE(reduce_op_takes(cfg.op, cfg.type), reduce_op_type_error(cfg.op, cfg.type));
+  if (cfg.cpu) {
+    const int P = cfg.ranks > 0 ? cfg.ranks : 4;
+    if (const char* why = reduce_scatter_refusal(P, rs_segment(cfg, P), cfg.type)) HPCP_FAIL(why);
+    int rc = 1;
+    if (elem_type_is_pair(cfg.type))
+      dispatch_pair(cfg.type, [&](auto tag) { rc = rs_run_on_host_typed<decltype(tag)>(cfg); });
+    else
+      dispatch_elem(cfg.type, [&](auto tag) { rc = rs_run_on_host_typed<decltype(tag)>(cfg); });
+    return rc;
+  }
+  if (cfg.ranks > 0)
+    if (const char* why = reduce_scatter_refusal(cfg.ranks, rs_segment(cfg, cfg.ranks), cfg.type)) HPCP_FAIL(why);
+  const int ndev = visible_device_count();
+  if (ndev == 0) {
+    std::cerr << "Error: No devices" << std::endl;
+    return 1;
+  }
+  if (cfg.ranks <= 0) cfg.ranks = std::min(ndev, kApiMaxRanks);
+  const int P = cfg.ranks;
+  std::vector<int> devices;
+  for (int r = 0; r < P; ++r) devices.push_back(primary_device(r, P, ndev));
+  const int ranks_per_dev = (P + ndev - 1) / ndev;
+  if (ranks_per_dev > 1 && cfg.ctas == 0)  // every rank's barrier CTA must find a slot next to its peers' grids
+    cfg.ctas = std::max(1, device_sm_count(devices[0]) / ranks_per_dev);
+  NodeMemory mem(devices);
+  RsShared sh;
+  sh.cfg = cfg;
+  sh.mem = &mem;
+  sh.n = rs_segment(cfg, P);
+  const size_t seg = sh.n * elem_size(cfg.type);
+  sh.pads = mem.alloc_pads(0);
+  sh.send = mem.alloc(seg * P, AllocKind::kDevice, /*zero=*/false);
+  sh.recv = mem.alloc(seg, AllocKind::kDevice, /*zero=*/false);
+  run_ranks(P, [&](RankCtx& ctx) { rs_rank_main(ctx, sh); });
+  mem.free(sh.send);
+  mem.free(sh.recv);
+  mem.free(sh.pads);
+  rs_report(cfg, P, sh.n, sh.best_ms, sh.total_bad, false);
+  return sh.total_bad == 0 ? 0 : 1;
+}
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -796,6 +1076,8 @@ int main(int argc, char** argv) {
   try {
     Shared sh;
     Config& cfg = sh.cfg;
+    bool reduce_scatter = false;
+    std::string rs_refused;  // the first option the reduce-scatter personality refuses
     // Type from the binary name suffix (`allreduce.int`), like upstream's `<app>.<type>` targets.
     {
       const std::string self = argv[0];
@@ -809,6 +1091,7 @@ int main(int argc, char** argv) {
       if (base.rfind("allreduce-mpi-sycl", 0) == 0) cfg.kind = AllocKind::kManaged;
       if (base.rfind("allreduce-usm-", 0) == 0) cfg.kind = AllocKind::kDevice;
       if (base.rfind("allreduce-map-", 0) == 0) cfg.kind = AllocKind::kMapped;
+      reduce_scatter = base == "reduce_scatter";
     }
     static const option long_opts[] = {{"type", required_argument, nullptr, 1},
                                        {"algo", required_argument, nullptr, 2},
@@ -828,6 +1111,22 @@ int main(int argc, char** argv) {
                                        {nullptr, 0, nullptr, 0}};
     int opt;
     while ((opt = getopt_long(argc, argv, "haHDSRp:n:", long_opts, nullptr)) != -1) {
+      if (rs_refused.empty()) {
+        switch (opt) {
+          case 'a': rs_refused = "-a"; break;
+          case 'H': rs_refused = "-H"; break;
+          case 'S': rs_refused = "-S"; break;
+          case 'R': rs_refused = "-R"; break;
+          case 2: rs_refused = "--algo"; break;
+          case 3: rs_refused = "--coll"; break;
+          case 7: rs_refused = "--chunk"; break;
+          case 10: rs_refused = "--slots"; break;
+          case 11: rs_refused = "--pull"; break;
+          case 12: rs_refused = "--map-alias"; break;
+          case 13: rs_refused = "--profile-relaunch"; break;
+          default: break;
+        }
+      }
       switch (opt) {
         case 'h': print_help(); return 1;
         case 'a': cfg.use_collective = true; break;
@@ -860,6 +1159,12 @@ int main(int argc, char** argv) {
         case 11: cfg.pull = true; break;
         default: print_help(); return 1;
       }
+    }
+    if (reduce_scatter) {
+      HPCP_REQUIRE(rs_refused.empty(), "reduce_scatter: " + rs_refused +
+                                           " is an allreduce option (the reduce-scatter runs one kernel on device memory)");
+      HPCP_REQUIRE(cfg.log2_elems >= 4 && cfg.log2_elems <= 32, "-p must be in [4,32]");
+      return run_reduce_scatter(cfg);
     }
     HPCP_REQUIRE(cfg.algo == "ring" || cfg.algo == "ring-unfused" || cfg.algo == "ring-rsag",
                  "unknown --algo " + cfg.algo);

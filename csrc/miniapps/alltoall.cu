@@ -25,6 +25,13 @@
 // and the host never tells it a count.  Check: the segments and the poison as above at their packed rows, recv_counts
 // against the host's matrix (not for --stock memcpy, whose copies are placed by the host), and the rows past each
 // rank's total still the poison.
+//
+// Run as `allgather` (a program-name link to this binary) it is the all-gather instead (↔ MPI_Allgather,
+// ncclAllGather): every rank holds ONE send block of B bytes and afterwards block p of every rank's receive buffer (P
+// blocks) is rank p's.  --pull, --stock memcpy (P-1 peer cudaMemcpyAsync copies plus the local one in the staggered
+// order, then the barrier), --sweep, --cpu and --json as above; --counts and --row-bytes are usage errors.  Check: rank
+// p's block holds the seed of (p, iteration), the receive buffer the poison; after the last iteration every receive
+// block p is checked against the seed of p, and the send block against its own seed (it is never written).
 #include <getopt.h>
 
 #include <algorithm>
@@ -66,11 +73,27 @@ struct Config {
   std::string counts;  // "" (the equal-block kernel), "random", "skewed" or "equal"
   size_t row_bytes = 16;
   bool row_given = false;
+  bool gather = false;  // program name `allgather`: the all-gather
 };
 
 constexpr size_t kSweepMaxBytes = size_t{256} << 20;
 
-void print_help() {
+void print_help(bool gather) {
+  if (gather) {
+    std::cout << "Usage: allgather [options]\n"
+                 "options:\n"
+                 " -n N               ranks (one host thread + one GPU each; default: all GPUs); 1 ... 16\n"
+                 " --block-bytes B    bytes of every rank's send block, a positive multiple of 16 (default 16 MiB);\n"
+                 "                    with --sweep the largest\n"
+                 " --pull             the kernel loads the peers' blocks instead of storing mine into their buffers\n"
+                 " --stock memcpy     stock shape: P cudaMemcpyAsync peer copies per rank, then a cross-rank barrier\n"
+                 " --sweep            block sizes 16 B ... 256 MiB (or --block-bytes) in powers of two\n"
+                 " --iters N --warmup N  timed / untimed repetitions (min is reported)\n"
+                 " --ctas N           CTAs per rank\n"
+                 " --json FILE        append one JSON row per block size\n"
+                 " --cpu              host-only plumbing run: ranks are threads, the walk is memcpy + a barrier\n";
+    return;
+  }
   std::cout << "Usage: alltoall [options]\n"
                "options:\n"
                " -n N               ranks (one host thread + one GPU each; default: all GPUs; more ranks than GPUs are\n"
@@ -96,6 +119,8 @@ uint32_t pair_seed(uint32_t it, int src, int dst) {
   return 0x40000000u | ((it & 0x3fffffu) << 8) | (static_cast<uint32_t>(src) << 4) | static_cast<uint32_t>(dst);
 }
 constexpr uint32_t kPoisonSeed = 0xC0DE0000u;
+// The all-gather's seed of rank `src`'s block in iteration `it` (bit 29 set, bits 30 and 31 clear: never the poison).
+uint32_t gather_seed(uint32_t it, int src) { return 0x20000000u | ((it & 0x3fffffu) << 4) | static_cast<uint32_t>(src); }
 constexpr uint32_t kTailPoisonSeed = 0xC0DE0001u;  // --counts: the receive rows past the total, never written
 
 const char* variant_name(const Config& cfg) {
@@ -166,16 +191,17 @@ void count_traffic(const std::vector<int64_t>& m, int P, size_t row_bytes, Row& 
 void report(const Config& cfg, int P, const Row& r) {
   const double sent = static_cast<double>(P - 1) * static_cast<double>(r.block_bytes);
   const double gbps = r.ms > 0 ? sent / (r.ms * 1e-3) * 1e-9 : 0.0;
-  const char* algo = cfg.cpu ? "host-alltoall" : variant_name(cfg);
-  std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << r.ms << " ms | alltoall " << algo
+  const char* pattern = cfg.gather ? "allgather" : "alltoall";
+  const std::string algo = cfg.cpu ? std::string("host-") + pattern : variant_name(cfg);
+  std::cout << "Elapsed (max over ranks, min of " << cfg.iters << "): " << r.ms << " ms | " << pattern << " " << algo
             << " P=" << P << " B=" << r.block_bytes << (cfg.cpu ? " host-threads" : "") << " | " << gbps
             << " GB/s sent per rank" << std::endl;
   if (!cfg.json_path.empty()) {
     if (FILE* f = std::fopen(cfg.json_path.c_str(), "a")) {
       std::fprintf(f,
-                   "{\"pattern\":\"alltoall\",\"variant\":\"%s\",\"ranks\":%d,\"block_bytes\":%zu,\"ms\":%.6f,"
+                   "{\"pattern\":\"%s\",\"variant\":\"%s\",\"ranks\":%d,\"block_bytes\":%zu,\"ms\":%.6f,"
                    "\"GBps_sent_per_rank\":%.3f,\"ctas\":%d,\"mismatches\":%llu}\n",
-                   variant_name(cfg), P, r.block_bytes, r.ms, gbps, r.ctas, r.bad);
+                   pattern, variant_name(cfg), P, r.block_bytes, r.ms, gbps, r.ctas, r.bad);
       std::fclose(f);
     }
   }
@@ -241,8 +267,11 @@ void rank_main(RankCtx& ctx, Shared& sh) {
     int ctas = 0;
     for (int it = 0; it < cfg.warmup + cfg.iters; ++it, ++it_global) {
       NvtxRange range(it < cfg.warmup ? "alltoall warm-up" : "alltoall timed");
-      for (int q = 0; q < P; ++q)
-        launch_fill_pattern(reinterpret_cast<uint32_t*>(my_send + q * B), B / 4, pair_seed(it_global, me, q), stream);
+      if (cfg.gather)
+        launch_fill_pattern(reinterpret_cast<uint32_t*>(my_send), B / 4, gather_seed(it_global, me), stream);
+      else
+        for (int q = 0; q < P; ++q)
+          launch_fill_pattern(reinterpret_cast<uint32_t*>(my_send + q * B), B / 4, pair_seed(it_global, me, q), stream);
       launch_fill_pattern(reinterpret_cast<uint32_t*>(my_recv), P * B / 4, kPoisonSeed, stream);
       HPCP_CUDA(cudaStreamSynchronize(stream));
       ctx.barrier();
@@ -251,10 +280,28 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       if (cfg.stock == "memcpy") {
         for (int j = 0; j < P; ++j) {
           const int p = (me + 1 + j) % P;
-          HPCP_CUDA(cudaMemcpyAsync(static_cast<unsigned char*>(sh.recv.ptr[p]) + me * B, my_send + p * B, B,
-                                    cudaMemcpyDefault, stream));
+          HPCP_CUDA(cudaMemcpyAsync(static_cast<unsigned char*>(sh.recv.ptr[p]) + me * B, my_send + (cfg.gather ? 0 : p * B),
+                                    B, cudaMemcpyDefault, stream));
         }
         launch_barrier_all(pads.data(), me, P, ++barrier_epoch, cfg.timeout_ns, status, stream);
+      } else if (cfg.gather) {
+        AllGatherArgs a;
+        for (int r = 0; r < P; ++r) {
+          a.send[r] = sh.send.ptr[r];
+          a.recv[r] = sh.recv.ptr[r];
+          a.pads[r] = pads[r];
+        }
+        a.ticket = my_pad + kPadLocal;
+        a.ticket_base = ticket_issued;
+        a.rank = me;
+        a.world = P;
+        a.block_bytes = B;
+        a.barrier_epoch = ++barrier_epoch;
+        a.timeout_ns = cfg.timeout_ns;
+        a.status = status;
+        a.pull = cfg.pull;
+        ctas = launch_all_gather(a, cfg.ctas, dev, stream);
+        ticket_issued += static_cast<uint32_t>(ctas);
       } else {
         AllToAllArgs a;
         for (int r = 0; r < P; ++r) {
@@ -284,11 +331,16 @@ void rank_main(RankCtx& ctx, Shared& sh) {
       const double t = ctx.max(ms);
       if (it >= cfg.warmup) best_ms = std::min(best_ms, t);
     }
-    // Every receive block p against the seed of (p, me) in the last iteration.
+    // Every receive block p against the seed of (p, me) in the last iteration (all-gather: of p, and my send block
+    // against my own seed).
     HPCP_CUDA(cudaMemsetAsync(count, 0, sizeof *count, stream));
     for (int p = 0; p < P; ++p)
-      launch_verify_pattern(reinterpret_cast<const uint32_t*>(my_recv + p * B), B / 4, pair_seed(it_global - 1, p, me),
-                            count, nullptr, nullptr, 0, 0, nullptr, stream);
+      launch_verify_pattern(reinterpret_cast<const uint32_t*>(my_recv + p * B), B / 4,
+                            cfg.gather ? gather_seed(it_global - 1, p) : pair_seed(it_global - 1, p, me), count, nullptr,
+                            nullptr, 0, 0, nullptr, stream);
+    if (cfg.gather)
+      launch_verify_pattern(reinterpret_cast<const uint32_t*>(my_send), B / 4, gather_seed(it_global - 1, me), count,
+                            nullptr, nullptr, 0, 0, nullptr, stream);
     unsigned long long bad = 0;
     HPCP_CUDA(cudaMemcpyAsync(&bad, count, sizeof bad, cudaMemcpyDeviceToHost, stream));
     HPCP_CUDA(cudaStreamSynchronize(stream));
@@ -462,21 +514,24 @@ int run_on_host(const Config& cfg) {
   std::vector<Row> rows;
   run_ranks(P, [&](RankCtx& ctx) {
     const int me = ctx.rank;
-    send[me].resize(P * top / 4);
+    send[me].resize((cfg.gather ? 1 : P) * top / 4);
     recv[me].resize(P * top / 4);
     uint32_t it_global = 0;
     for (const size_t B : sizes) {
       const size_t words = B / 4;
       double best_ms = std::numeric_limits<double>::max();
       for (int it = 0; it < cfg.warmup + cfg.iters; ++it, ++it_global) {
-        for (int q = 0; q < P; ++q)
-          for (size_t i = 0; i < words; ++i) send[me][q * words + i] = pattern_word(i, pair_seed(it_global, me, q));
+        if (cfg.gather)
+          for (size_t i = 0; i < words; ++i) send[me][i] = pattern_word(i, gather_seed(it_global, me));
+        else
+          for (int q = 0; q < P; ++q)
+            for (size_t i = 0; i < words; ++i) send[me][q * words + i] = pattern_word(i, pair_seed(it_global, me, q));
         for (size_t i = 0; i < P * words; ++i) recv[me][i] = pattern_word(i, kPoisonSeed);
         ctx.barrier();
         const auto t0 = std::chrono::steady_clock::now();
         for (int j = 0; j < P; ++j) {
           const int p = (me + 1 + j) % P;
-          std::memcpy(recv[p].data() + me * words, send[me].data() + p * words, B);
+          std::memcpy(recv[p].data() + me * words, send[me].data() + (cfg.gather ? 0 : p * words), B);
         }
         ctx.barrier();
         const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -485,9 +540,11 @@ int run_on_host(const Config& cfg) {
       }
       unsigned long long bad = 0;
       for (int p = 0; p < P; ++p) {
-        const uint32_t seed = pair_seed(it_global - 1, p, me);
+        const uint32_t seed = cfg.gather ? gather_seed(it_global - 1, p) : pair_seed(it_global - 1, p, me);
         for (size_t i = 0; i < words; ++i) bad += recv[me][p * words + i] != pattern_word(i, seed);
       }
+      if (cfg.gather)
+        for (size_t i = 0; i < words; ++i) bad += send[me][i] != pattern_word(i, gather_seed(it_global - 1, me));
       const double total_bad = ctx.sum(static_cast<double>(bad));
       print_verdict(me, bad);
       if (me == 0) rows.push_back({B, best_ms, static_cast<unsigned long long>(total_bad), 0});
@@ -580,6 +637,10 @@ int main(int argc, char** argv) {
   try {
     Shared sh;
     Config& cfg = sh.cfg;
+    {
+      const std::string prog = argv[0];
+      cfg.gather = prog.substr(prog.find_last_of('/') + 1) == "allgather";
+    }
     static const option long_opts[] = {{"block-bytes", required_argument, nullptr, 1},
                                        {"pull", no_argument, nullptr, 2},
                                        {"stock", required_argument, nullptr, 3},
@@ -596,7 +657,7 @@ int main(int argc, char** argv) {
     int opt;
     while ((opt = getopt_long(argc, argv, "hn:", long_opts, nullptr)) != -1) {
       switch (opt) {
-        case 'h': print_help(); return 0;
+        case 'h': print_help(cfg.gather); return 0;
         case 'n': cfg.ranks = std::atoi(optarg); break;
         case 1: {
           char* end = nullptr;
@@ -621,7 +682,7 @@ int main(int argc, char** argv) {
           cfg.row_given = true;
           break;
         }
-        default: print_help(); return 1;
+        default: print_help(cfg.gather); return 1;
       }
     }
     // Usage errors, before anything is allocated.
@@ -632,7 +693,13 @@ int main(int argc, char** argv) {
     HPCP_REQUIRE(cfg.counts.empty() || cfg.counts == "random" || cfg.counts == "skewed" || cfg.counts == "equal",
                  "--counts must be random, skewed or equal, not " + cfg.counts);
     HPCP_REQUIRE(!cfg.row_given || !cfg.counts.empty(), "--row-bytes needs --counts");
-    if (const char* why = all_to_all_refusal(cfg.ranks < 0 ? 1 : cfg.ranks, cfg.block_bytes)) HPCP_FAIL(why);
+    HPCP_REQUIRE(!cfg.gather || (cfg.counts.empty() && !cfg.row_given),
+                 "allgather: --counts and --row-bytes belong to the all-to-all-v (bin/alltoall)");
+    if (cfg.gather) {
+      if (const char* why = all_gather_refusal(cfg.ranks < 0 ? 1 : cfg.ranks, cfg.block_bytes)) HPCP_FAIL(why);
+    } else if (const char* why = all_to_all_refusal(cfg.ranks < 0 ? 1 : cfg.ranks, cfg.block_bytes)) {
+      HPCP_FAIL(why);
+    }
     if (!cfg.counts.empty())
       if (const char* why = all_to_all_v_refusal(cfg.ranks < 0 ? 1 : cfg.ranks, cfg.row_bytes, 1, 1)) HPCP_FAIL(why);
 
@@ -657,7 +724,7 @@ int main(int argc, char** argv) {
     const bool v = !cfg.counts.empty();
     const size_t bytes = v ? capacity_rows(P, mean_rows(top, cfg.row_bytes)) * cfg.row_bytes : top * P;
     sh.pads = mem.alloc_pads(0);
-    sh.send = mem.alloc(bytes, AllocKind::kDevice, /*zero=*/false);
+    sh.send = mem.alloc(cfg.gather ? top : bytes, AllocKind::kDevice, /*zero=*/false);
     sh.recv = mem.alloc(bytes, AllocKind::kDevice, /*zero=*/false);
     if (v) sh.counts = mem.alloc(sizeof(int64_t) * P, AllocKind::kDevice, /*zero=*/true);
     run_ranks(P, [&](RankCtx& ctx) { v ? rank_main_v(ctx, sh) : rank_main(ctx, sh); });

@@ -266,9 +266,31 @@ void test_alltoallv_plan() {
   CHECK(a2av_first_rule(0) == kA2avAccepted && a2av_first_rule(0xE) == kA2avNegative && a2av_first_rule(9) == kA2avRecvCapacity);
 }
 
+// The host refusals of the stand-alone reduce-scatter and all-gather (kernels/api.h), before any launch.
+void test_gather_scatter_refusals() {
+  using namespace hpcp;
+  CHECK(reduce_scatter_refusal(4, 4, ElemType::kFloat) == nullptr);
+  CHECK(reduce_scatter_refusal(1, 1, ElemType::kDoubleInt) == nullptr);         // one 16-byte pair is a whole vector
+  CHECK(reduce_scatter_refusal(16, 16, ElemType::kUChar) == nullptr);
+  CHECK(reduce_scatter_refusal(4, 0, ElemType::kFloat) == kReduceScatterCountError);
+  CHECK(reduce_scatter_refusal(4, 3, ElemType::kFloat) == kReduceScatterCountError);
+  CHECK(reduce_scatter_refusal(4, 4, ElemType::kBFloat16) == kReduceScatterCountError);   // 8 bytes
+  CHECK(reduce_scatter_refusal(0, 4, ElemType::kFloat) == kReduceScatterWorldError);
+  CHECK(reduce_scatter_refusal(17, 4, ElemType::kFloat) == kReduceScatterWorldError);
+  CHECK(all_gather_refusal(1, 16) == nullptr && all_gather_refusal(16, 48) == nullptr);
+  CHECK(all_gather_refusal(4, 0) == kAllGatherBlockError && all_gather_refusal(4, 24) == kAllGatherBlockError);
+  CHECK(all_gather_refusal(0, 16) == kAllGatherWorldError && all_gather_refusal(17, 16) == kAllGatherWorldError);
+  alignas(16) static unsigned char buf[256];
+  CHECK(byte_ranges_overlap(buf, 64, buf + 32, 16));                            // recv inside send (MPI_IN_PLACE)
+  CHECK(byte_ranges_overlap(buf + 32, 16, buf, 64));
+  CHECK(!byte_ranges_overlap(buf, 64, buf + 64, 64) && !byte_ranges_overlap(buf + 64, 64, buf, 64));
+  CHECK(!reduce_op_takes(ReduceOp::kBAnd, ElemType::kHalf) && reduce_op_takes(ReduceOp::kBAnd, ElemType::kUShort));
+}
+
 int main() {
   test_kernel_orderings();
   test_alltoallv_plan();
+  test_gather_scatter_refusals();
   test_rank_runtime();
   test_devices_and_dtypes();
   test_topology();

@@ -4,6 +4,8 @@
   peer2pear    P2P bandwidth, process-per-GPU (run under torchrun for >1 GPU)
   allreduce    allreduce miniapp, process-per-GPU (run under torchrun)
   alltoall     all-to-all miniapp (push / pull kernels, nccl baseline; --counts: all-to-all-v), process-per-GPU (torchrun)
+  reduce_scatter  reduce-scatter miniapp (direct kernel, nccl baseline), process-per-GPU (run under torchrun)
+  allgather    all-gather miniapp (push / pull kernels, nccl baseline), process-per-GPU (run under torchrun)
   halo         the miniapp loop as a halo exchange fused into a slab stencil — the flagship (run under torchrun)
   tp           tensor-parallel linear layers with the collective fused into the GEMM, vs cuBLAS + NCCL (torchrun)
   topology     fabric planes / rank->GPU mapping (JSON)
@@ -19,7 +21,7 @@ from __future__ import annotations
 import os
 import sys
 
-_GPU_PROGRAMS = ("peer2pear", "allreduce", "alltoall", "halo", "tp", "interop")
+_GPU_PROGRAMS = ("peer2pear", "allreduce", "alltoall", "reduce_scatter", "allgather", "halo", "tp", "interop")
 
 
 def _no_gpu_message(prog: str):
@@ -27,7 +29,7 @@ def _no_gpu_message(prog: str):
     import torch
 
     if prog in _GPU_PROGRAMS and not torch.cuda.is_available():
-        hint = f"; bin/{prog} --cpu is the host-only plumbing run" if prog in ("peer2pear", "allreduce", "alltoall") else ""
+        hint = f"; bin/{prog} --cpu is the host-only plumbing run" if prog in ("peer2pear", "allreduce", "alltoall", "reduce_scatter", "allgather") else ""
         return f"Error: {prog}: no CUDA device (this program runs sm_90a kernels{hint})"
     return None
 
@@ -71,6 +73,12 @@ def _dispatch(prog: str, rest: list) -> int:
         return m(rest)
     if prog == "alltoall":
         from .models.alltoall import main as m
+        return m(rest)
+    if prog == "reduce_scatter":
+        from .models.allreduce import main_reduce_scatter as m
+        return m(rest)
+    if prog == "allgather":
+        from .models.alltoall import main_allgather as m
         return m(rest)
     if prog == "halo":
         from .models.halo import main as m

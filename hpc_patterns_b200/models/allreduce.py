@@ -40,7 +40,8 @@ from typing import List, Optional
 import torch
 
 from .. import native
-from ..ops.allreduce import LOC_LAYOUT, loc_combine, pack_loc, unpack_loc
+from ..ops.allreduce import (LOC_LAYOUT, check_reduce_scatter_args, loc_combine, pack_loc,
+                             reduce_scatter, unpack_loc)
 from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
@@ -575,6 +576,291 @@ class VirtualAllreduce:
     def close(self) -> None:
         for app in self.ranks:
             app.close()
+
+
+# -------------------------------------------------------------------------------------------------- reduce-scatter ----
+# ``ReduceScatterMiniapp`` is the Python twin of ``bin/reduce_scatter`` (↔ MPI_Reduce_scatter_block, ncclReduceScatter):
+# rank p's send buffer holds P segments of n elements, and afterwards rank r's receive buffer holds op over p of
+# segment r of rank p's, owner first (``ops.allreduce.reduce_scatter``).  Algorithms: ``direct`` (one launch per rank,
+# peer loads, default) and ``nccl`` (torch.distributed.reduce_scatter_tensor, sum / prod / min / max, the baseline).
+RS_ALGOS = ("direct", "nccl")
+RS_SUM_POISON = 251.0       # above every rank's constant-data sum up to 16 ranks (at most 232) and exact in every type
+
+
+def rs_input(op: str, rank: int, segment: int, world: int) -> float:
+    """What segment ``segment`` of ``rank``'s send buffer holds in the constant-data run: for the sum rank + (segment
+    mod 8), so a rank that reduced another's segment gets another value; for the other ops the allreduce's
+    ``op_input``."""
+    return float(rank + segment % 8) if op == "sum" else op_input(op, rank, world)
+
+
+def rs_expected(op: str, rank: int, world: int) -> float:
+    """Every element of ``rank``'s receive buffer after the constant-data run."""
+    return world * (world - 1) / 2.0 + world * (rank % 8) if op == "sum" else expected_value(world, op)
+
+
+def rs_poison(op: str, world: int) -> float:
+    """The receive buffer before the run: a value no rank expects (vc_init's 0 is rank 0's sum at one rank)."""
+    return RS_SUM_POISON if op == "sum" else vc_init(op, world)
+
+
+@dataclass
+class ReduceScatterResult:
+    algo: str
+    dtype: str
+    world: int
+    elements: int        # per segment
+    ms: float
+    mismatches: int
+    elem_bytes: int = 4
+    op: str = "sum"
+
+    def row(self) -> dict:
+        """One JSON row; GB/s counts the (P-1) segments that leave every rank's send buffer for their owners."""
+        sent = float(self.world - 1) * self.elements * self.elem_bytes
+        gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
+        return {"pattern": "reduce_scatter", "algo": self.algo, "type": self.dtype, "op": self.op,
+                "ranks": self.world, "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
+                "mismatches": self.mismatches}
+
+
+class ReduceScatterMiniapp:
+    def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float", op: str = "sum",
+                 algo: str = "direct", ctas: int = 0, timeout_s: float = 30.0, n_elems: int = 0,
+                 _shared: Optional[dict] = None):
+        """The send buffer holds 2^log2_elems elements padded to P whole 16-byte segments (``n_elems``: exactly that
+        many per rank).  ``_shared``: buffers made by an in-process group (``VirtualReduceScatter``): ``pads``,
+        ``send``, ``recv``.  Every refusal is raised before anything is allocated."""
+        if algo not in RS_ALGOS:
+            raise ValueError(f"algo must be one of {RS_ALGOS}")
+        if dtype not in DTYPES:
+            raise ValueError(f"dtype must be one of {sorted(DTYPES)}")
+        op = reduce_op(op)
+        check_op_type(op, dtype)
+        if algo == "nccl" and (op not in ("sum", "prod", "min", "max") or dtype in PAIR_TYPES):
+            raise ValueError(f"nccl reduce-scatters sum, prod, min and max only: op={op} needs direct")
+        if algo == "nccl" and op in ("min", "max") and dtype in UNSIGNED_TYPES:
+            raise ValueError(f"nccl compares {dtype} as a signed torch type: op={op} is refused")
+        if _shared is not None and algo != "direct":
+            raise ValueError("virtual ranks run direct: nccl needs one process per GPU")
+        esz = native().elem_size(dtype)
+        total = element_count(esz, comm.world, log2_elems, n_elems)
+        check_reduce_scatter_args(comm.world, total // comm.world, dtype)
+        self.C = native()
+        self.comm, self.device = comm, device
+        self.rank, self.world = comm.rank, comm.world
+        self.algo, self.dtype, self.op, self.ctas, self.esz = algo, dtype, op, ctas, esz
+        self.n = total // self.world                 # elements per segment
+        self.seg_bytes = self.n * esz
+        self.launch_ctas = 0
+        torch.cuda.set_device(device)
+        if _shared is not None:
+            self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
+        else:
+            self.pads = SignalPads(comm, device, timeout_s=timeout_s)
+            self.send = SymmetricBuffer(comm, self.world * self.seg_bytes, device, zero=False)
+            self.recv = SymmetricBuffer(comm, self.seg_bytes, device, zero=False)   # only the local mapping is used
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _tensor(self, buf: torch.Tensor) -> torch.Tensor:
+        return buf if self.dtype in PAIR_TYPES else buf.view(_TORCH_DTYPE[self.dtype])
+
+    def initialize(self) -> None:
+        """The constant-data run's send segments and the poisoned receive buffer."""
+        st, base = self._stream(), self.send.local_ptr
+        for q in range(self.world):
+            at = base + q * self.seg_bytes
+            if self.dtype in PAIR_TYPES:
+                self.C.init_pair(at, self.n, *loc_input(self.op, self.rank, self.world), self.dtype, st)
+            else:
+                x = rs_input(self.op, self.rank, q, self.world)
+                self.C.init3(at, 0, 0, self.n, x, 0.0, 0.0, self.dtype, st)
+        if self.dtype in PAIR_TYPES:
+            self.C.init_pair(self.recv.local_ptr, self.n, *loc_vc_init(self.op), self.dtype, st)
+        else:
+            self.C.init3(self.recv.local_ptr, 0, 0, self.n, rs_poison(self.op, self.world), 0.0, 0.0, self.dtype, st)
+
+    def run_once(self) -> None:
+        """Enqueue one reduce-scatter on the current stream.  Precondition: every rank's send buffer is final and no
+        rank still reads its receive buffer (``run()`` puts ``pads.device_barrier`` before it)."""
+        pads, st = self.pads, self._stream()
+        if self.algo == "nccl":
+            import torch.distributed as dist
+            src, dst = self._tensor(self.send.tensor()), self._tensor(self.recv.tensor())
+            if self.world > 1:
+                dist.reduce_scatter_tensor(dst, src, op=_nccl_op(self.op))
+            else:
+                dst.copy_(src)
+            return
+        pads.barrier_epoch += 1
+        self.launch_ctas = reduce_scatter(self.send.ptrs, self.recv.local_ptr, pads.buf.ptrs, pads.ticket_ptr,
+                                          pads.ticket_issued, self.rank, self.n, pads.barrier_epoch, pads.timeout_ns,
+                                          pads.status_ptr, self.dtype, self.ctas, self.device, st, self.op)
+        pads.advance_tickets(self.launch_ctas)
+
+    def reduce_scatter(self, x: torch.Tensor) -> torch.Tensor:
+        """Reduce-scatter the tensor ``x`` (P*n elements of the dtype, or its packed pairs): copy it into the symmetric
+        send buffer, the device barrier and the launch, all enqueued on the current stream; returns this rank's n
+        elements as a view of the receive buffer, which the next call overwrites.  Never synchronises the host."""
+        xb = x.contiguous().view(torch.uint8).reshape(-1)
+        if xb.numel() != self.world * self.seg_bytes:
+            raise ValueError(f"reduce-scatter: x must hold {self.world} x {self.n} {self.dtype} elements")
+        self.send.tensor().copy_(xb)
+        if self.algo != "nccl":
+            self.pads.device_barrier(self._stream())
+        self.run_once()
+        return self._tensor(self.recv.tensor())
+
+    def mismatches(self) -> int:
+        """Wrong elements of the receive buffer after the constant-data run, plus those of the send buffer (which must
+        be unchanged)."""
+        count = torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.device))
+        st, c = self._stream(), count.data_ptr()
+        for q in range(self.world):
+            at = self.send.local_ptr + q * self.seg_bytes
+            if self.dtype in PAIR_TYPES:
+                self.C.count_pair_mismatch(at, self.n, *loc_input(self.op, self.rank, self.world), self.dtype, c, st)
+            else:
+                self.C.count_mismatch(at, self.n, rs_input(self.op, self.rank, q, self.world), self.dtype, c, st)
+        if self.dtype in PAIR_TYPES:
+            self.C.count_pair_mismatch(self.recv.local_ptr, self.n, *loc_expected(self.op, self.world), self.dtype,
+                                       c, st)
+        else:
+            self.C.count_mismatch(self.recv.local_ptr, self.n, rs_expected(self.op, self.rank, self.world),
+                                  self.dtype, c, st)
+        torch.cuda.synchronize(self.device)
+        return int(count.item())
+
+    def run(self, iters: int = 5, warmup: int = 1) -> ReduceScatterResult:
+        stream = torch.cuda.current_stream(self.device)
+        e0 = torch.cuda.Event(enable_timing=True)
+        e1 = torch.cuda.Event(enable_timing=True)
+        best = float("inf")
+        for it in range(warmup + iters):
+            self.initialize()
+            torch.cuda.synchronize(self.device)
+            self.comm.barrier()
+            self.pads.device_barrier(stream.cuda_stream)
+            e0.record(stream)
+            self.run_once()
+            e1.record(stream)
+            stream.synchronize()
+            self.pads.check()
+            t = self.comm.max(e0.elapsed_time(e1))
+            if it >= warmup:
+                best = min(best, t)
+        bad = self.mismatches()
+        total_bad = int(self.comm.sum(bad))
+        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong elements", flush=True)
+        return ReduceScatterResult(self.algo, self.dtype, self.world, self.n, best, total_bad, self.esz, self.op)
+
+    def close(self) -> None:
+        torch.cuda.synchronize(self.device)
+        self.send.close()
+        self.recv.close()
+        self.pads.close()
+
+
+class VirtualReduceScatter:
+    """``world`` ReduceScatterMiniapp ranks driven by ONE process on one GPU, as ``VirtualAllreduce`` does: plain peer
+    pointers, one stream per rank, every grid capped at ``sms // world`` CTAs so that the grids that end in the node
+    barrier stay co-resident, at most 8 ranks.  ``n`` is the segment, in elements."""
+
+    MAX_WORLD = 8
+
+    def __init__(self, world: int, n: int, dtype: str = "float", op: str = "sum", ctas: int = 0, device: int = 0,
+                 timeout_s: float = 10.0):
+        from ..parallel.local import LocalGroup
+
+        if not 1 <= world <= self.MAX_WORLD:
+            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
+        if dtype not in DTYPES:
+            raise ValueError(f"dtype must be one of {sorted(DTYPES)}")
+        op = reduce_op(op)
+        check_op_type(op, dtype)
+        check_reduce_scatter_args(world, n, dtype)
+        C = native()
+        cap = max(1, C.sm_count(device) // world)
+        self.ctas = min(ctas, cap) if ctas > 0 else cap
+        self.world, self.n, self.dtype, self.op, self.device = world, int(n), dtype, op, device
+        self.group = LocalGroup(world, [device] * world)
+        pads = self.group.pads(timeout_s=timeout_s)
+        send = self.group.symmetric(world * self.n * C.elem_size(dtype), zero=False)
+        recv = self.group.symmetric(self.n * C.elem_size(dtype), zero=False)
+        self.ranks: List[ReduceScatterMiniapp] = [
+            ReduceScatterMiniapp(self.group.comms[r], device, dtype=dtype, op=op, ctas=self.ctas, timeout_s=timeout_s,
+                                 n_elems=world * self.n, _shared={"pads": pads[r], "send": send[r], "recv": recv[r]})
+            for r in range(world)]
+        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
+
+    def load(self, sends: List[torch.Tensor]) -> None:
+        """Send buffer of rank r <- ``sends[r]``: P*n elements of the dtype's torch type, or any tensor of as many
+        bytes (a pair type's packed bytes)."""
+        if len(sends) != self.world:
+            raise ValueError(f"one send tensor per rank ({self.world})")
+        torch.cuda.synchronize(self.device)
+        for app, s in zip(self.ranks, sends):
+            b = s.contiguous().view(torch.uint8).reshape(-1)
+            if b.numel() != self.world * app.seg_bytes:
+                raise ValueError(f"a send tensor must hold {self.world} x {self.n} {self.dtype} elements")
+            app.send.tensor().copy_(b)
+        torch.cuda.synchronize(self.device)
+
+    def run_once(self) -> None:
+        """One reduce-scatter: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one
+        (it stands in for the cross-rank barrier of the precondition)."""
+        for app, st in zip(self.ranks, self.streams):
+            with torch.cuda.device(app.device), torch.cuda.stream(st):
+                app.run_once()
+
+    def synchronize(self) -> None:
+        for st in self.streams:
+            st.synchronize()
+        for app in self.ranks:
+            app.pads.check()
+
+    def results(self) -> List[torch.Tensor]:
+        """The receive buffer of every rank on the host (n elements; a pair type's packed bytes)."""
+        self.synchronize()
+        return [app._tensor(app.recv.tensor()).cpu() for app in self.ranks]
+
+    def close(self) -> None:
+        for app in self.ranks:
+            app.close()
+
+
+def main_reduce_scatter(argv: Optional[List[str]] = None) -> int:
+    """``torchrun --nproc-per-node N -m hpc_patterns_b200 reduce_scatter [-p K] [--type T] [--op OP]
+    [--algo direct|nccl]``"""
+    import argparse
+
+    ap = argparse.ArgumentParser(prog="reduce_scatter", add_help=True)
+    ap.add_argument("-p", "--log2-elems", type=int, default=25, help="2^K elements of send buffer per rank")
+    ap.add_argument("--type", default="float", choices=DTYPES)
+    ap.add_argument("--op", default="sum")
+    ap.add_argument("--algo", default="direct", choices=RS_ALGOS)
+    ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--ctas", type=int, default=0)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args(argv)
+    check_op_type(reduce_op(args.op), args.type)
+    comm = Comm()
+    app = ReduceScatterMiniapp(comm, comm.device, args.log2_elems, args.type, args.op, args.algo, ctas=args.ctas)
+    res = app.run(args.iters, args.warmup)
+    if comm.rank == 0:
+        row = res.row()
+        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | reduce_scatter {args.algo} "
+              f"{args.type} {app.op} P={comm.world} n={app.n} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank",
+              flush=True)
+        if args.json:
+            with open(args.json, "a") as f:
+                f.write(json.dumps(row) + "\n")
+    app.close()
+    comm.close()
+    return 0 if res.mismatches == 0 else 1
 
 
 def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int, op: str = "sum"):

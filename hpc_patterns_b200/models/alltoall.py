@@ -26,7 +26,8 @@ from typing import List, Optional
 import torch
 
 from .. import native
-from ..ops.alltoall import (all_to_all, all_to_all_v, as_blocks, check_args, check_v_args, check_verdict)
+from ..ops.alltoall import (all_gather, all_to_all, all_to_all_v, as_blocks, check_args, check_gather_args,
+                             check_v_args, check_verdict)
 from ..parallel.comm import Comm
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
 
@@ -548,6 +549,223 @@ class VirtualAlltoallv:
     def close(self) -> None:
         for app in self.ranks:
             app.close()
+
+
+# ------------------------------------------------------------------------------------------------------ all-gather ----
+# ``AllgatherMiniapp`` is the Python twin of ``bin/allgather`` (↔ MPI_Allgather, ncclAllGather): every rank holds one
+# send block of ``block_bytes``; afterwards block p of every rank's receive buffer is rank p's block
+# (``ops.alltoall.all_gather``).  Algorithms: ``push`` (default), ``pull`` and ``nccl``
+# (torch.distributed.all_gather_into_tensor, the baseline).  The check is the all-to-all's: rank p's block holds the
+# pattern seed of (p, iteration), the receive buffer the poison, and every block p is verified at its slot.
+
+
+def gather_seed(it: int, src: int) -> int:
+    """The pattern seed of rank ``src``'s send block in iteration ``it`` (never the poison)."""
+    return 0x20000000 | ((it & 0x3FFFFF) << 4) | src
+
+
+@dataclass
+class AllgatherResult(AlltoallResult):
+    def row(self) -> dict:
+        row = super().row()
+        row["pattern"] = "allgather"
+        return row
+
+
+class AllgatherMiniapp:
+    def __init__(self, comm: Comm, device: int, block_bytes: int = 16 << 20, algo: str = "push", ctas: int = 0,
+                 timeout_s: float = 30.0, _shared: Optional[dict] = None):
+        """``_shared``: buffers made by an in-process group (``VirtualAllgather``): ``pads``, ``send``, ``recv``."""
+        if algo not in ALGOS:
+            raise ValueError(f"algo must be one of {ALGOS}")
+        check_gather_args(comm.world, block_bytes)
+        if _shared is not None and algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
+        self.C = native()
+        self.comm, self.device = comm, device
+        self.rank, self.world = comm.rank, comm.world
+        self.algo, self.block_bytes, self.ctas = algo, int(block_bytes), ctas
+        self.nbytes = self.world * self.block_bytes
+        self.generation = 0
+        self.launch_ctas = 0
+        torch.cuda.set_device(device)
+        if _shared is not None:
+            self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
+        else:
+            self.pads = SignalPads(comm, device, timeout_s=timeout_s)
+            self.send = SymmetricBuffer(comm, self.block_bytes, device, zero=False)
+            self.recv = SymmetricBuffer(comm, self.nbytes, device, zero=False)
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def initialize(self) -> None:
+        """My send block <- the pattern of (rank, a new iteration); the receive buffer <- the poison."""
+        st = self._stream()
+        self.C.fill_pattern(self.send.local_ptr, self.block_bytes // 4, gather_seed(self.generation, self.rank), st)
+        self.C.fill_pattern(self.recv.local_ptr, self.nbytes // 4, POISON_SEED, st)
+        self.generation += 1
+
+    def run_once(self) -> None:
+        """Enqueue one all-gather on the current stream (precondition as ``AlltoallMiniapp.run_once``)."""
+        pads, st = self.pads, self._stream()
+        if self.algo == "nccl":
+            import torch.distributed as dist
+            src, dst = self.send.tensor(), self.recv.tensor()
+            if self.world > 1:
+                dist.all_gather_into_tensor(dst, src)
+            else:
+                dst.copy_(src)
+            return
+        pads.barrier_epoch += 1
+        self.launch_ctas = all_gather(self.send.ptrs, self.recv.ptrs, pads.buf.ptrs, pads.ticket_ptr,
+                                      pads.ticket_issued, self.rank, self.block_bytes, pads.barrier_epoch,
+                                      pads.timeout_ns, pads.status_ptr, self.ctas, self.device, st,
+                                      self.algo == "pull")
+        pads.advance_tickets(self.launch_ctas)
+
+    def all_gather(self, x: torch.Tensor) -> torch.Tensor:
+        """All-gather the tensor ``x`` (``block_bytes`` of any dtype): copy it into the symmetric send block, the device
+        barrier and the launch, all enqueued on the current stream; returns the receive buffer as a [P, *x.shape] view
+        of x's dtype, which the next call overwrites.  Never synchronises the host."""
+        xb = x.contiguous().view(torch.uint8).reshape(-1)
+        if xb.numel() != self.block_bytes:
+            raise ValueError(f"all-gather: x must hold {self.block_bytes} bytes")
+        self.send.tensor().copy_(xb)
+        if self.algo != "nccl":
+            self.pads.device_barrier(self._stream())
+        self.run_once()
+        return self.recv.tensor().view(x.dtype).reshape(self.world, *x.shape)
+
+    def mismatches(self) -> int:
+        """Wrong words of the receive buffer (block p must be rank p's) and of my send block (it must be unchanged)."""
+        count = torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.device))
+        st, B, it = self._stream(), self.block_bytes, self.generation - 1
+        for p in range(self.world):
+            self.C.verify_pattern(self.recv.local_ptr + p * B, B // 4, gather_seed(it, p), count.data_ptr(),
+                                  stream=st)
+        self.C.verify_pattern(self.send.local_ptr, B // 4, gather_seed(it, self.rank), count.data_ptr(), stream=st)
+        torch.cuda.synchronize(self.device)
+        return int(count.item())
+
+    def run(self, iters: int = 5, warmup: int = 1) -> AllgatherResult:
+        stream = torch.cuda.current_stream(self.device)
+        e0 = torch.cuda.Event(enable_timing=True)
+        e1 = torch.cuda.Event(enable_timing=True)
+        best = float("inf")
+        for it in range(warmup + iters):
+            self.initialize()
+            torch.cuda.synchronize(self.device)
+            self.comm.barrier()
+            self.pads.device_barrier(stream.cuda_stream)
+            e0.record(stream)
+            self.run_once()
+            e1.record(stream)
+            stream.synchronize()
+            self.pads.check()
+            t = self.comm.max(e0.elapsed_time(e1))
+            if it >= warmup:
+                best = min(best, t)
+        bad = self.mismatches()
+        total_bad = int(self.comm.sum(bad))
+        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong words", flush=True)
+        return AllgatherResult(self.algo, self.world, self.block_bytes, best, total_bad, self.launch_ctas)
+
+    def close(self) -> None:
+        torch.cuda.synchronize(self.device)
+        self.send.close()
+        self.recv.close()
+        self.pads.close()
+
+
+class VirtualAllgather:
+    """``world`` AllgatherMiniapp ranks driven by ONE process on one GPU, as ``VirtualAlltoall`` does."""
+
+    MAX_WORLD = 8
+
+    def __init__(self, world: int, block_bytes: int, algo: str = "push", ctas: int = 0, device: int = 0,
+                 timeout_s: float = 10.0):
+        from ..parallel.local import LocalGroup
+
+        if not 1 <= world <= self.MAX_WORLD:
+            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
+        if algo not in VIRTUAL_ALGOS:
+            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        check_gather_args(world, block_bytes)
+        C = native()
+        cap = max(1, C.sm_count(device) // world)
+        self.ctas = min(ctas, cap) if ctas > 0 else cap
+        self.world, self.block_bytes, self.device = world, int(block_bytes), device
+        self.group = LocalGroup(world, [device] * world)
+        pads = self.group.pads(timeout_s=timeout_s)
+        send = self.group.symmetric(self.block_bytes, zero=False)
+        recv = self.group.symmetric(world * self.block_bytes, zero=False)
+        self.ranks: List[AllgatherMiniapp] = [
+            AllgatherMiniapp(self.group.comms[r], device, self.block_bytes, algo, ctas=self.ctas, timeout_s=timeout_s,
+                             _shared={"pads": pads[r], "send": send[r], "recv": recv[r]})
+            for r in range(world)]
+        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
+
+    def load(self, sends: List[torch.Tensor]) -> None:
+        """Send block of rank r <- the bytes of ``sends[r]`` (``block_bytes`` of any dtype)."""
+        if len(sends) != self.world:
+            raise ValueError(f"one send tensor per rank ({self.world})")
+        torch.cuda.synchronize(self.device)
+        for app, s in zip(self.ranks, sends):
+            b = s.contiguous().view(torch.uint8).reshape(-1)
+            if b.numel() != self.block_bytes:
+                raise ValueError(f"a send tensor must hold {self.block_bytes} bytes")
+            app.send.tensor().copy_(b)
+        torch.cuda.synchronize(self.device)
+
+    def run_once(self) -> None:
+        """One all-gather: every rank's ``run_once`` on its own stream; ``synchronize`` before the next one."""
+        for app, st in zip(self.ranks, self.streams):
+            with torch.cuda.device(app.device), torch.cuda.stream(st):
+                app.run_once()
+
+    def synchronize(self) -> None:
+        for st in self.streams:
+            st.synchronize()
+        for app in self.ranks:
+            app.pads.check()
+
+    def results(self) -> List[torch.Tensor]:
+        """The receive buffer of every rank as a [P, B] uint8 tensor on the host."""
+        self.synchronize()
+        return [app.recv.tensor().cpu().reshape(self.world, self.block_bytes) for app in self.ranks]
+
+    def close(self) -> None:
+        for app in self.ranks:
+            app.close()
+
+
+def main_allgather(argv: Optional[List[str]] = None) -> int:
+    """``torchrun --nproc-per-node N -m hpc_patterns_b200 allgather [--block-bytes B] [--algo push|pull|nccl]``"""
+    import argparse
+
+    ap = argparse.ArgumentParser(prog="allgather", add_help=True)
+    ap.add_argument("--block-bytes", type=int, default=16 << 20, help="bytes per rank's block (default 16 MiB)")
+    ap.add_argument("--algo", default="push", choices=ALGOS)
+    ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--ctas", type=int, default=0)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args(argv)
+    check_gather_args(1, args.block_bytes)
+    comm = Comm()
+    app = AllgatherMiniapp(comm, comm.device, args.block_bytes, args.algo, ctas=args.ctas)
+    res = app.run(args.iters, args.warmup)
+    if comm.rank == 0:
+        row = res.row()
+        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | allgather {args.algo} "
+              f"P={comm.world} B={args.block_bytes} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank", flush=True)
+        if args.json:
+            with open(args.json, "a") as f:
+                f.write(json.dumps(row) + "\n")
+    app.close()
+    comm.close()
+    return 0 if res.mismatches == 0 else 1
 
 
 def main(argv: Optional[List[str]] = None) -> int:

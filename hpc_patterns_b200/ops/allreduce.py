@@ -122,3 +122,83 @@ def count_mismatch(v: torch.Tensor, expected: float, stream: Optional[int] = Non
                             current_stream(dev) if stream is None else stream)
     torch.cuda.synchronize(dev)
     return int(count.item())
+
+
+# -------------------------------------------------------------------------------------------------- reduce-scatter ----
+# ``reduce_scatter`` is the one-launch reduce-scatter (↔ MPI_Reduce_scatter_block, ncclReduceScatter,
+# reduce_scatter_tensor): rank p's send buffer holds P segments of n elements; afterwards rank r's receive buffer (n
+# elements) holds op over p of segment r of rank p's send buffer, owner first in every element,
+# ((S_r[r] o S_{r+1}[r]) o ...) o S_{r+P-1}[r].  Any op the allreduce takes for the type, with its refusals.
+# The refusal words and the element sizes are the native module's (csrc/kernels/api.h), read from it.
+RS_MAX_RANKS = 16
+
+
+def check_reduce_scatter_args(world: int, n: int, dtype: str) -> None:
+    """ValueError with the native words if the launcher would refuse (world, n, dtype).  An op that does not reduce the
+    type is refused by the launcher with dispatch_op's words (``models.allreduce.check_op_type`` says them first)."""
+    C = native()
+    if n <= 0 or n * C.elem_size(dtype) % 16:     # elem_size: ValueError for a name that is not a type
+        raise ValueError(C.REDUCE_SCATTER_COUNT_ERROR)
+    if not 1 <= world <= RS_MAX_RANKS:
+        raise ValueError(C.REDUCE_SCATTER_WORLD_ERROR)
+
+
+def reduce_scatter(send, recv: int, pads, ticket: int, ticket_base: int, rank: int, n: int, barrier_epoch: int,
+                   timeout_ns: int = 0, status: int = 0, dtype: str = "float", ctas: int = 0, device: int = 0,
+                   stream: int = 0, op: str = "sum") -> int:
+    """Enqueue one reduce-scatter of rank ``rank`` on ``stream``.  ``send`` / ``pads`` are every rank's peer-mapped
+    addresses, ``recv`` this rank's receive buffer of ``n`` elements.  Returns the CTAs launched (advance the ticket
+    counter by it)."""
+    world = len(send)
+    check_reduce_scatter_args(world, n, dtype)
+    if len(pads) != world:
+        raise ValueError("reduce-scatter: inconsistent rank lists")
+    if not 0 <= rank < world:
+        raise ValueError("reduce-scatter: rank out of range")
+    seg = n * native().elem_size(dtype)
+    if not (send[rank] + world * seg <= recv or recv + seg <= send[rank]):
+        raise ValueError(native().REDUCE_SCATTER_OVERLAP_ERROR)
+    return native().reduce_scatter(list(send), recv, list(pads), ticket, ticket_base & 0xFFFFFFFF, rank, n,
+                                   barrier_epoch, timeout_ns, status, dtype, ctas, device, stream, op)
+
+
+def reduce_scatter_reference(sends, op: str, dtype: str):
+    """Rank r's receive buffer for every r, computed in torch / Python from the send buffers (each P segments of n
+    elements; pair types: packed bytes), owner first: ((S_r[r] o S_{r+1}[r]) o ...).  The 16-bit floating sum and prod
+    accumulate in fp32 and round once.  torch's min / max may keep the other zero of a +0 / -0 tie and its NaNs are not
+    the kernels' canonical ones; everything else is the kernels' result bit for bit (integers wrap)."""
+    world = len(sends)
+    if dtype in LOC_LAYOUT:
+        parts = [s.contiguous().view(torch.uint8).reshape(world, -1) for s in sends]
+        out = []
+        for r in range(world):
+            acc = parts[r][r].clone()
+            for k in range(1, world):
+                acc = loc_combine(acc, parts[(r + k) % world][r], dtype, op)
+            out.append(acc)
+        return out
+    parts = [s.reshape(world, -1) for s in sends]
+    lowp = parts[0].dtype in (torch.bfloat16, torch.float16) and op in ("sum", "prod")
+    out = []
+    for r in range(world):
+        acc = parts[r][r].float() if lowp else parts[r][r].clone()
+        for k in range(1, world):
+            x = parts[(r + k) % world][r]
+            acc = _combine_ref(acc, x.float() if lowp else x, op)
+        out.append(acc.to(parts[0].dtype) if lowp else acc)
+    return out
+
+
+def _combine_ref(a: torch.Tensor, b: torch.Tensor, op: str) -> torch.Tensor:
+    if op == "sum":
+        return a + b
+    if op in ("prod", "product"):
+        return a * b
+    if op in ("min", "max"):
+        return torch.minimum(a, b) if op == "min" else torch.maximum(a, b)
+    if op in ("band", "bor", "bxor"):
+        return {"band": torch.bitwise_and, "bor": torch.bitwise_or, "bxor": torch.bitwise_xor}[op](a, b)
+    if op in ("land", "lor", "lxor"):
+        f = {"land": torch.logical_and, "lor": torch.logical_or, "lxor": torch.logical_xor}[op]
+        return f(a != 0, b != 0).to(a.dtype)
+    raise ValueError(f"unknown op {op!r}")

@@ -122,3 +122,41 @@ def all_to_all_v_reference(sends: List[torch.Tensor], counts: List, row_bytes: i
         segs = [rows[p][sum(m[p][:r]): sum(m[p][:r]) + m[p][r]] for p in range(world)]
         out.append(torch.cat(segs) if segs else torch.empty(0, row_bytes, dtype=torch.uint8))
     return out
+
+
+# ------------------------------------------------------------------------------------------------------ all-gather ----
+# ``all_gather`` is the one-launch all-gather (↔ MPI_Allgather, ncclAllGather, all_gather_into_tensor): every rank holds
+# one send block of ``block_bytes``; afterwards block p of every rank's receive buffer (P blocks) is rank p's send block.
+# It is the all-to-all's walk with a source stride of 0, push or pull, ending with the node barrier.
+# Its refusal words are the native module's (csrc/kernels/api.h), read from it.
+
+
+def check_gather_args(world: int, block_bytes: int) -> None:
+    """ValueError with the native words if the launcher would refuse (world, block_bytes)."""
+    if block_bytes <= 0 or block_bytes % 16:
+        raise ValueError(native().ALL_GATHER_BLOCK_ERROR)
+    if not 1 <= world <= MAX_RANKS:
+        raise ValueError(native().ALL_GATHER_WORLD_ERROR)
+
+
+def all_gather(send: Sequence[int], recv: Sequence[int], pads: Sequence[int], ticket: int, ticket_base: int, rank: int,
+               block_bytes: int, barrier_epoch: int, timeout_ns: int = 0, status: int = 0, ctas: int = 0,
+               device: int = 0, stream: int = 0, pull: bool = False) -> int:
+    """Enqueue one all-gather of rank ``rank`` on ``stream``.  ``send`` / ``recv`` / ``pads`` are every rank's
+    peer-mapped addresses.  Returns the CTAs launched (advance the ticket counter by it)."""
+    world = len(send)
+    check_gather_args(world, block_bytes)
+    if len(recv) != world or len(pads) != world:
+        raise ValueError("all-gather: inconsistent rank lists")
+    if not 0 <= rank < world:
+        raise ValueError("all-gather: rank out of range")
+    s, r = send[rank], recv[rank]
+    if not (s + block_bytes <= r or r + world * block_bytes <= s):
+        raise ValueError(native().ALL_GATHER_OVERLAP_ERROR)
+    return native().all_gather(list(send), list(recv), list(pads), ticket, ticket_base & 0xFFFFFFFF, rank, block_bytes,
+                               barrier_epoch, timeout_ns, status, ctas, device, stream, pull)
+
+
+def all_gather_reference(sends: List[torch.Tensor]) -> torch.Tensor:
+    """The receive buffer of every rank: the bytes of ``sends[0]``, ``sends[1]``, ... concatenated, as [P, B] uint8."""
+    return torch.stack([s.contiguous().view(torch.uint8).reshape(-1) for s in sends])

@@ -30,6 +30,8 @@ UNVALIDATED = (
     # more than 8 ranks: needs > 8 GPUs (ranks sharing one GPU's hardware queue serialise their spinning kernels)
     r"two_shot_kernel<[\w<> ]+, 16, 1, \w+>",   # every op and type
     r"two_shot_f32_kernel<[\w<>, ]+, 16, 1>",   # the 16-bit floating types' fp32 sums and products, same rank bound
+    r"reduce_scatter_kernel<[\w<> ]+, 16, 1>",   # the reduce-scatter's two-shot shapes, same rank bound
+    r"reduce_scatter_f32_kernel<[\w<>, ]+, 16, 1>",
 )
 
 
