@@ -33,7 +33,6 @@ The native single-process CLI twin is ``bin/allreduce`` (csrc/miniapps/allreduce
 """
 from __future__ import annotations
 
-import json
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -43,7 +42,9 @@ from .. import native
 from ..ops.allreduce import (LOC_LAYOUT, check_reduce_scatter_args, loc_combine, pack_loc,
                              reduce_scatter, unpack_loc)
 from ..parallel.comm import Comm
+from ..parallel.local import VirtualRanks
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
+from .collective import CollectiveMiniapp, gbps, report
 
 ALGOS = ("ring", "ring-unfused", "twoshot", "nvls", "nccl", "ring-nccl", "ring-rsag")
 VIRTUAL_ALGOS = ("ring", "ring-unfused", "twoshot", "ring-rsag")   # the ones whose peers are plain pointers (no NCCL, no multicast)
@@ -190,12 +191,10 @@ class AllreduceResult:
 
     def row(self) -> dict:
         """One JSON row; ``"op"`` only when it is not the sum (sum rows keep their shape)."""
-        nbytes = self.elements * self.elem_bytes
-        sent = bytes_sent_per_rank(self.algo, nbytes, self.world)
-        gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
+        rate = gbps(bytes_sent_per_rank(self.algo, self.elements * self.elem_bytes, self.world), self.ms)
         row = {"pattern": "allreduce", "algo": self.algo, "type": self.dtype, "ranks": self.world,
-               "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
-               "frac_of_450GBps": gbps / 450.0, "mismatches": self.mismatches}
+               "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": rate,
+               "frac_of_450GBps": rate / 450.0, "mismatches": self.mismatches}
         if self.op != "sum":
             row["op"] = self.op
         return row
@@ -235,7 +234,10 @@ def _layout(algo: str, C, n: int, esz: int, world: int, chunk_elems: int, slots_
     return (n_chunks,) + ring_layout(n * esz, n_chunks, world, slots_policy)
 
 
-class AllreduceMiniapp:
+class AllreduceMiniapp(CollectiveMiniapp):
+    PATTERN, UNIT = "allreduce", "elements"
+    BUFFERS = ("va", "vb", "vc", "slots")
+
     def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float",
                  algo: str = "ring", chunk_elems: int = 0, ctas: int = 0, timeout_s: float = 30.0,
                  slots: int = 0, pull: bool = False, n_elems: int = 0, op: str = "sum",
@@ -264,17 +266,12 @@ class AllreduceMiniapp:
             raise ValueError(f"{algo} compares {dtype} as a signed torch type: op={op} is refused")
         self.op = op
         self._op_kw = {} if op == "sum" else {"op": op}   # sum calls stay exactly as they were
-        if _shared is not None and algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
-        self.C = native()
-        self.comm, self.device = comm, device
-        self.rank, self.world = comm.rank, comm.world
-        self.algo, self.dtype, self.ctas, self.chunk_elems = algo, dtype, ctas, chunk_elems
+        super().__init__(comm, device, native(), algo, ctas, _shared, VIRTUAL_ALGOS)
+        self.dtype, self.chunk_elems = dtype, chunk_elems
         self.esz = self.C.elem_size(dtype)
         n = element_count(self.esz, self.world, log2_elems, n_elems)
         self.n, self.nbytes = n, n * self.esz
         self.right, self.left = (self.rank + 1) % self.world, (self.rank - 1) % self.world
-        torch.cuda.set_device(device)
         if slots not in (0, 2):
             raise ValueError("slots must be 0 (world-1 slots) or 2")
         self.slots_policy = slots if algo == "ring" else 0
@@ -320,9 +317,6 @@ class AllreduceMiniapp:
         self._symm = (t, hdl)
         self._va_ptr, self._vc_ptr = t.data_ptr(), t.data_ptr() + self.nbytes
         self._va_mc, self._vc_mc = mc, mc + self.nbytes
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     def _ptrs(self):
         if self.algo == "nvls":
@@ -462,68 +456,27 @@ class AllreduceMiniapp:
         torch.cuda.synchronize(self.device)
         return int(count.item())
 
-    def run(self, iters: int = 5, warmup: int = 1) -> AllreduceResult:
-        stream = torch.cuda.current_stream(self.device)
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        best = float("inf")
-        for it in range(warmup + iters):
-            self.initialize()
-            torch.cuda.synchronize(self.device)
-            self.comm.barrier()
-            self.pads.device_barrier(stream.cuda_stream)
-            torch.cuda.nvtx.range_push(f"allreduce {self.algo} {'warm-up' if it < warmup else 'timed'}")
-            e0.record(stream)
-            self.run_once()
-            e1.record(stream)
-            torch.cuda.nvtx.range_pop()
-            stream.synchronize()
-            self.pads.check()
-            t = self.comm.max(e0.elapsed_time(e1))
-            if it >= warmup:
-                best = min(best, t)
-        bad = self.mismatches()
-        total_bad = int(self.comm.sum(bad))
-        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong elements", flush=True)
-        return AllreduceResult(self.algo, self.dtype, self.world, self.n, best, total_bad, self.esz, self.op)
-
-    def close(self) -> None:
-        torch.cuda.synchronize(self.device)
-        for b in (self.va, self.vb, self.vc, self.slots):
-            if b is not None:
-                b.close()
-        self.pads.close()
+    def result(self, ms: float, mismatches: int) -> AllreduceResult:
+        return AllreduceResult(self.algo, self.dtype, self.world, self.n, ms, mismatches, self.esz, self.op)
 
 
-class VirtualAllreduce:
-    """``world`` AllreduceMiniapp ranks driven by ONE process on one GPU: virtual ranks whose peer pointers are plain
-    pointers, so the ring's arrival and ack words, the two-shot barrier and the unfused ring's rendezvous run on a
-    1-GPU box with the same ``run_once`` plumbing as one process per GPU.  ``run_once()`` enqueues one allreduce per
-    rank, each on its own stream.  The fused ring's CTAs spin per chunk on their neighbours, so every rank's grid is
-    kept co-resident: at most ``sms // world`` CTAs each.  At most 8 ranks: more streams than the device's hardware
-    queues would serialise the spinning kernels.  The unfused ring launches a kernel for the first time next to spinning
-    ones, which needs the eager module loading this package asks for when it is imported before CUDA starts."""
-
-    MAX_WORLD = 8
+class VirtualAllreduce(VirtualRanks):
+    """``world`` AllreduceMiniapp ranks on one GPU (``VirtualRanks``): the ring's arrival and ack words, the two-shot
+    barrier and the unfused ring's rendezvous run on a 1-GPU box with the same ``run_once`` plumbing as one process per
+    GPU.  The unfused ring launches a kernel for the first time next to spinning ones, which needs the eager module
+    loading this package asks for when it is imported before CUDA starts."""
 
     def __init__(self, world: int, n: int, dtype: str = "float", algo: str = "ring", slots: int = 0,
                  pull: bool = False, ctas: int = 0, chunk_elems: int = 0, device: int = 0, timeout_s: float = 10.0,
                  op: str = "sum"):
-        from ..parallel.local import LocalGroup
-
-        if not 1 <= world <= self.MAX_WORLD:
-            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
-        if algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        self.refuse(world, algo, VIRTUAL_ALGOS)
         op = reduce_op(op)
         check_op_type(op, dtype)
         C = native()
         esz = C.elem_size(dtype)
         n = element_count(esz, world, n_elems=n)
-        cap = max(1, C.sm_count(device) // world)
-        self.ctas = min(ctas, cap) if ctas > 0 else cap
-        self.dtype, self.device, self.n = dtype, device, n
-        self.group = LocalGroup(world, [device] * world)
+        super().__init__(world, device, ctas)
+        self.dtype, self.n = dtype, n
         policy = slots if algo == "ring" else 0
         _, pad_words, slot_bytes = _layout(algo, C, n, esz, world, chunk_elems, policy)
         none = [None] * world
@@ -537,7 +490,6 @@ class VirtualAllreduce:
                              ctas=self.ctas, timeout_s=timeout_s, slots=slots, pull=pull, n_elems=n, op=op,
                              _shared={"pads": pads[r], "va": va[r], "vb": vb[r], "vc": vc[r], "slots": sl[r]})
             for r in range(world)]
-        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, vas: List[torch.Tensor]) -> None:
         """VA of rank r <- ``vas[r]`` (n elements of the dtype's torch type; for a pair type a (values, indices) tuple,
@@ -553,29 +505,12 @@ class VirtualAllreduce:
                 app.vc.tensor(_TORCH_DTYPE[self.dtype]).zero_()
         torch.cuda.synchronize(self.device)
 
-    def run_once(self) -> None:
-        """One allreduce: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one (it
-        stands in for the cross-rank barrier that separates consecutive launches)."""
-        for app, st in zip(self.ranks, self.streams):
-            with torch.cuda.device(app.device), torch.cuda.stream(st):
-                app.run_once()
-
-    def synchronize(self) -> None:
-        for st in self.streams:
-            st.synchronize()
-        for app in self.ranks:
-            app.pads.check()
-
     def results(self) -> List[torch.Tensor]:
         """VC of every rank, on the host; for a pair type a (values, int32 indices) tuple per rank (``unpack_loc``)."""
         self.synchronize()
         if self.dtype in PAIR_TYPES:
             return [unpack_loc(app.vc.tensor(torch.uint8).cpu(), self.dtype) for app in self.ranks]
         return [app.vc.tensor(_TORCH_DTYPE[self.dtype]).cpu() for app in self.ranks]
-
-    def close(self) -> None:
-        for app in self.ranks:
-            app.close()
 
 
 # -------------------------------------------------------------------------------------------------- reduce-scatter ----
@@ -618,13 +553,14 @@ class ReduceScatterResult:
     def row(self) -> dict:
         """One JSON row; GB/s counts the (P-1) segments that leave every rank's send buffer for their owners."""
         sent = float(self.world - 1) * self.elements * self.elem_bytes
-        gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
         return {"pattern": "reduce_scatter", "algo": self.algo, "type": self.dtype, "op": self.op,
-                "ranks": self.world, "elements": self.elements, "ms": self.ms, "GBps_sent_per_rank": gbps,
-                "mismatches": self.mismatches}
+                "ranks": self.world, "elements": self.elements, "ms": self.ms,
+                "GBps_sent_per_rank": gbps(sent, self.ms), "mismatches": self.mismatches}
 
 
-class ReduceScatterMiniapp:
+class ReduceScatterMiniapp(CollectiveMiniapp):
+    PATTERN, UNIT = "reduce_scatter", "elements"
+
     def __init__(self, comm: Comm, device: int, log2_elems: int = 25, dtype: str = "float", op: str = "sum",
                  algo: str = "direct", ctas: int = 0, timeout_s: float = 30.0, n_elems: int = 0,
                  _shared: Optional[dict] = None):
@@ -641,28 +577,19 @@ class ReduceScatterMiniapp:
             raise ValueError(f"nccl reduce-scatters sum, prod, min and max only: op={op} needs direct")
         if algo == "nccl" and op in ("min", "max") and dtype in UNSIGNED_TYPES:
             raise ValueError(f"nccl compares {dtype} as a signed torch type: op={op} is refused")
-        if _shared is not None and algo != "direct":
-            raise ValueError("virtual ranks run direct: nccl needs one process per GPU")
-        esz = native().elem_size(dtype)
-        total = element_count(esz, comm.world, log2_elems, n_elems)
-        check_reduce_scatter_args(comm.world, total // comm.world, dtype)
-        self.C = native()
-        self.comm, self.device = comm, device
-        self.rank, self.world = comm.rank, comm.world
-        self.algo, self.dtype, self.op, self.ctas, self.esz = algo, dtype, op, ctas, esz
+        super().__init__(comm, device, native(), algo, ctas, _shared, ("direct",))
+        self.esz = self.C.elem_size(dtype)
+        total = element_count(self.esz, self.world, log2_elems, n_elems)
+        check_reduce_scatter_args(self.world, total // self.world, dtype)
+        self.dtype, self.op = dtype, op
         self.n = total // self.world                 # elements per segment
-        self.seg_bytes = self.n * esz
-        self.launch_ctas = 0
-        torch.cuda.set_device(device)
+        self.seg_bytes = self.n * self.esz
         if _shared is not None:
             self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
         else:
             self.pads = SignalPads(comm, device, timeout_s=timeout_s)
             self.send = SymmetricBuffer(comm, self.world * self.seg_bytes, device, zero=False)
             self.recv = SymmetricBuffer(comm, self.seg_bytes, device, zero=False)   # only the local mapping is used
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     def _tensor(self, buf: torch.Tensor) -> torch.Tensor:
         return buf if self.dtype in PAIR_TYPES else buf.view(_TORCH_DTYPE[self.dtype])
@@ -733,59 +660,24 @@ class ReduceScatterMiniapp:
         torch.cuda.synchronize(self.device)
         return int(count.item())
 
-    def run(self, iters: int = 5, warmup: int = 1) -> ReduceScatterResult:
-        stream = torch.cuda.current_stream(self.device)
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        best = float("inf")
-        for it in range(warmup + iters):
-            self.initialize()
-            torch.cuda.synchronize(self.device)
-            self.comm.barrier()
-            self.pads.device_barrier(stream.cuda_stream)
-            e0.record(stream)
-            self.run_once()
-            e1.record(stream)
-            stream.synchronize()
-            self.pads.check()
-            t = self.comm.max(e0.elapsed_time(e1))
-            if it >= warmup:
-                best = min(best, t)
-        bad = self.mismatches()
-        total_bad = int(self.comm.sum(bad))
-        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong elements", flush=True)
-        return ReduceScatterResult(self.algo, self.dtype, self.world, self.n, best, total_bad, self.esz, self.op)
-
-    def close(self) -> None:
-        torch.cuda.synchronize(self.device)
-        self.send.close()
-        self.recv.close()
-        self.pads.close()
+    def result(self, ms: float, mismatches: int) -> ReduceScatterResult:
+        return ReduceScatterResult(self.algo, self.dtype, self.world, self.n, ms, mismatches, self.esz, self.op)
 
 
-class VirtualReduceScatter:
-    """``world`` ReduceScatterMiniapp ranks driven by ONE process on one GPU, as ``VirtualAllreduce`` does: plain peer
-    pointers, one stream per rank, every grid capped at ``sms // world`` CTAs so that the grids that end in the node
-    barrier stay co-resident, at most 8 ranks.  ``n`` is the segment, in elements."""
-
-    MAX_WORLD = 8
+class VirtualReduceScatter(VirtualRanks):
+    """``world`` ReduceScatterMiniapp ranks on one GPU (``VirtualRanks``).  ``n`` is the segment, in elements."""
 
     def __init__(self, world: int, n: int, dtype: str = "float", op: str = "sum", ctas: int = 0, device: int = 0,
                  timeout_s: float = 10.0):
-        from ..parallel.local import LocalGroup
-
-        if not 1 <= world <= self.MAX_WORLD:
-            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
+        self.refuse(world)
         if dtype not in DTYPES:
             raise ValueError(f"dtype must be one of {sorted(DTYPES)}")
         op = reduce_op(op)
         check_op_type(op, dtype)
         check_reduce_scatter_args(world, n, dtype)
         C = native()
-        cap = max(1, C.sm_count(device) // world)
-        self.ctas = min(ctas, cap) if ctas > 0 else cap
-        self.world, self.n, self.dtype, self.op, self.device = world, int(n), dtype, op, device
-        self.group = LocalGroup(world, [device] * world)
+        super().__init__(world, device, ctas)
+        self.n, self.dtype, self.op = int(n), dtype, op
         pads = self.group.pads(timeout_s=timeout_s)
         send = self.group.symmetric(world * self.n * C.elem_size(dtype), zero=False)
         recv = self.group.symmetric(self.n * C.elem_size(dtype), zero=False)
@@ -793,7 +685,6 @@ class VirtualReduceScatter:
             ReduceScatterMiniapp(self.group.comms[r], device, dtype=dtype, op=op, ctas=self.ctas, timeout_s=timeout_s,
                                  n_elems=world * self.n, _shared={"pads": pads[r], "send": send[r], "recv": recv[r]})
             for r in range(world)]
-        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, sends: List[torch.Tensor]) -> None:
         """Send buffer of rank r <- ``sends[r]``: P*n elements of the dtype's torch type, or any tensor of as many
@@ -808,27 +699,10 @@ class VirtualReduceScatter:
             app.send.tensor().copy_(b)
         torch.cuda.synchronize(self.device)
 
-    def run_once(self) -> None:
-        """One reduce-scatter: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one
-        (it stands in for the cross-rank barrier of the precondition)."""
-        for app, st in zip(self.ranks, self.streams):
-            with torch.cuda.device(app.device), torch.cuda.stream(st):
-                app.run_once()
-
-    def synchronize(self) -> None:
-        for st in self.streams:
-            st.synchronize()
-        for app in self.ranks:
-            app.pads.check()
-
     def results(self) -> List[torch.Tensor]:
         """The receive buffer of every rank on the host (n elements; a pair type's packed bytes)."""
         self.synchronize()
         return [app._tensor(app.recv.tensor()).cpu() for app in self.ranks]
-
-    def close(self) -> None:
-        for app in self.ranks:
-            app.close()
 
 
 def main_reduce_scatter(argv: Optional[List[str]] = None) -> int:
@@ -850,17 +724,7 @@ def main_reduce_scatter(argv: Optional[List[str]] = None) -> int:
     comm = Comm()
     app = ReduceScatterMiniapp(comm, comm.device, args.log2_elems, args.type, args.op, args.algo, ctas=args.ctas)
     res = app.run(args.iters, args.warmup)
-    if comm.rank == 0:
-        row = res.row()
-        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | reduce_scatter {args.algo} "
-              f"{args.type} {app.op} P={comm.world} n={app.n} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank",
-              flush=True)
-        if args.json:
-            with open(args.json, "a") as f:
-                f.write(json.dumps(row) + "\n")
-    app.close()
-    comm.close()
-    return 0 if res.mismatches == 0 else 1
+    return report(comm, app, res, args, f"reduce_scatter {args.algo} {args.type} {app.op} P={comm.world} n={app.n}")
 
 
 def choose_collective(comm: Comm, device: int, dtype: str, log2_elems: int, op: str = "sum"):
@@ -919,18 +783,8 @@ def main(argv: Optional[List[str]] = None) -> int:
             print(f"# -a: {algo} ({why})", flush=True)
     app = AllreduceMiniapp(comm, device, args.p, args.type, algo, slots=args.slots, pull=args.pull, op=op)
     res = app.run(args.iters, args.warmup)
-    if comm.rank == 0:
-        row = res.row()
-        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | {algo} {args.type} "
-              f"P={comm.world} N={res.elements}{'' if op == 'sum' else ' op=' + op} | "
-              f"{row['GBps_sent_per_rank']:.1f} GB/s sent per rank",
-              flush=True)
-        if args.json:
-            with open(args.json, "a") as f:
-                f.write(json.dumps(row) + "\n")
-    app.close()
-    comm.close()
-    return 0 if res.mismatches == 0 else 1
+    return report(comm, app, res, args,
+                  f"{algo} {args.type} P={comm.world} N={res.elements}{'' if op == 'sum' else ' op=' + op}")
 
 
 if __name__ == "__main__":

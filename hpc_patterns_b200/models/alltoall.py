@@ -19,7 +19,6 @@ the counts, ``.tolist()`` (a device-to-host sync), then ``all_to_all_single`` wi
 """
 from __future__ import annotations
 
-import json
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -29,7 +28,9 @@ from .. import native
 from ..ops.alltoall import (all_gather, all_to_all, all_to_all_v, as_blocks, check_args, check_gather_args,
                              check_v_args, check_verdict)
 from ..parallel.comm import Comm
+from ..parallel.local import VirtualRanks
 from ..parallel.symmetric import SignalPads, SymmetricBuffer
+from .collective import CollectiveMiniapp, gbps, report
 
 ALGOS = ("push", "pull", "nccl")
 VIRTUAL_ALGOS = ("push", "pull")
@@ -53,37 +54,30 @@ class AlltoallResult:
     def row(self) -> dict:
         """One JSON row with the CLI's keys; GB/s counts the P-1 blocks that leave the rank."""
         sent = float(self.world - 1) * self.block_bytes
-        gbps = sent / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
         return {"pattern": "alltoall", "variant": self.variant, "ranks": self.world, "block_bytes": self.block_bytes,
-                "ms": self.ms, "GBps_sent_per_rank": gbps, "ctas": self.ctas, "mismatches": self.mismatches}
+                "ms": self.ms, "GBps_sent_per_rank": gbps(sent, self.ms), "ctas": self.ctas,
+                "mismatches": self.mismatches}
 
 
-class AlltoallMiniapp:
+class AlltoallMiniapp(CollectiveMiniapp):
+    PATTERN = "alltoall"
+
     def __init__(self, comm: Comm, device: int, block_bytes: int = 16 << 20, algo: str = "push", ctas: int = 0,
                  timeout_s: float = 30.0, _shared: Optional[dict] = None):
         """``_shared``: buffers made by an in-process group (``VirtualAlltoall``): ``pads``, ``send``, ``recv``."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
         check_args(comm.world, block_bytes)
-        if _shared is not None and algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
-        self.C = native()
-        self.comm, self.device = comm, device
-        self.rank, self.world = comm.rank, comm.world
-        self.algo, self.block_bytes, self.ctas = algo, int(block_bytes), ctas
+        super().__init__(comm, device, native(), algo, ctas, _shared, VIRTUAL_ALGOS)
+        self.block_bytes = int(block_bytes)
         self.nbytes = self.world * self.block_bytes
         self.generation = 0           # iterations initialised so far: the pattern seeds of the last one are checked
-        self.launch_ctas = 0
-        torch.cuda.set_device(device)
         if _shared is not None:
             self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
         else:
             self.pads = SignalPads(comm, device, timeout_s=timeout_s)
             self.send = SymmetricBuffer(comm, self.nbytes, device, zero=False)
             self.recv = SymmetricBuffer(comm, self.nbytes, device, zero=False)
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     def initialize(self) -> None:
         """Send block q <- the pattern of (rank, q) in a new iteration; the receive buffer <- the poison."""
@@ -122,58 +116,19 @@ class AlltoallMiniapp:
         torch.cuda.synchronize(self.device)
         return int(count.item())
 
-    def run(self, iters: int = 5, warmup: int = 1) -> AlltoallResult:
-        stream = torch.cuda.current_stream(self.device)
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        best = float("inf")
-        for it in range(warmup + iters):
-            self.initialize()
-            torch.cuda.synchronize(self.device)
-            self.comm.barrier()
-            self.pads.device_barrier(stream.cuda_stream)
-            e0.record(stream)
-            self.run_once()
-            e1.record(stream)
-            stream.synchronize()
-            self.pads.check()
-            t = self.comm.max(e0.elapsed_time(e1))
-            if it >= warmup:
-                best = min(best, t)
-        bad = self.mismatches()
-        total_bad = int(self.comm.sum(bad))
-        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong words", flush=True)
-        return AlltoallResult(self.algo, self.world, self.block_bytes, best, total_bad, self.launch_ctas)
-
-    def close(self) -> None:
-        torch.cuda.synchronize(self.device)
-        self.send.close()
-        self.recv.close()
-        self.pads.close()
+    def result(self, ms: float, mismatches: int) -> AlltoallResult:
+        return AlltoallResult(self.algo, self.world, self.block_bytes, ms, mismatches, self.launch_ctas)
 
 
-class VirtualAlltoall:
-    """``world`` AlltoallMiniapp ranks driven by ONE process on one GPU, as ``VirtualAllreduce`` does: the peer
-    pointers are plain pointers, and ``run_once()`` enqueues one all-to-all per rank, each on its own stream.  Every
-    rank's grid ends in the node barrier, so the grids are kept co-resident: at most ``sms // world`` CTAs each.  At
-    most 8 ranks: more streams than the device's hardware queues would serialise the spinning kernels."""
-
-    MAX_WORLD = 8
+class VirtualAlltoall(VirtualRanks):
+    """``world`` AlltoallMiniapp ranks on one GPU (``VirtualRanks``)."""
 
     def __init__(self, world: int, block_bytes: int, algo: str = "push", ctas: int = 0, device: int = 0,
                  timeout_s: float = 10.0):
-        from ..parallel.local import LocalGroup
-
-        if not 1 <= world <= self.MAX_WORLD:
-            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
-        if algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        self.refuse(world, algo, VIRTUAL_ALGOS)
         check_args(world, block_bytes)
-        C = native()
-        cap = max(1, C.sm_count(device) // world)
-        self.ctas = min(ctas, cap) if ctas > 0 else cap
-        self.world, self.block_bytes, self.device = world, int(block_bytes), device
-        self.group = LocalGroup(world, [device] * world)
+        super().__init__(world, device, ctas)
+        self.block_bytes = int(block_bytes)
         pads = self.group.pads(timeout_s=timeout_s)
         send = self.group.symmetric(world * self.block_bytes, zero=False)
         recv = self.group.symmetric(world * self.block_bytes, zero=False)
@@ -181,7 +136,6 @@ class VirtualAlltoall:
             AlltoallMiniapp(self.group.comms[r], device, self.block_bytes, algo, ctas=self.ctas, timeout_s=timeout_s,
                             _shared={"pads": pads[r], "send": send[r], "recv": recv[r]})
             for r in range(world)]
-        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, sends: List[torch.Tensor]) -> None:
         """Send buffer of rank r <- ``sends[r]``: a [P, B] uint8 tensor, or any tensor of P*B bytes (viewed as bytes)."""
@@ -195,27 +149,10 @@ class VirtualAlltoall:
             app.send.tensor().copy_(b.reshape(-1))
         torch.cuda.synchronize(self.device)
 
-    def run_once(self) -> None:
-        """One all-to-all: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one (it
-        stands in for the cross-rank barrier of the precondition)."""
-        for app, st in zip(self.ranks, self.streams):
-            with torch.cuda.device(app.device), torch.cuda.stream(st):
-                app.run_once()
-
-    def synchronize(self) -> None:
-        for st in self.streams:
-            st.synchronize()
-        for app in self.ranks:
-            app.pads.check()
-
     def results(self) -> List[torch.Tensor]:
         """The receive buffer of every rank as a [P, B] uint8 tensor on the host."""
         self.synchronize()
         return [app.recv.tensor().cpu().reshape(self.world, self.block_bytes) for app in self.ranks]
-
-    def close(self) -> None:
-        for app in self.ranks:
-            app.close()
 
 
 # ---------------------------------------------------------------------------------------------------- all-to-all-v ----
@@ -272,17 +209,20 @@ class AlltoallvResult:
 
     def row(self) -> dict:
         """One JSON row with the CLI's keys; GB/s is off-rank bytes summed over ranks / P / time."""
-        gbps = self.off_rank_bytes / self.world / (self.ms * 1e-3) / 1e9 if self.ms > 0 else 0.0
         return {"pattern": "alltoallv", "variant": self.variant, "ranks": self.world, "block_bytes": self.block_bytes,
-                "ms": self.ms, "GBps_sent_per_rank": gbps, "ctas": self.ctas, "mismatches": self.mismatches,
+                "ms": self.ms, "GBps_sent_per_rank": gbps(self.off_rank_bytes / self.world, self.ms),
+                "ctas": self.ctas, "mismatches": self.mismatches,
                 "counts": self.counts, "row_bytes": self.row_bytes,
                 "max_bytes_into_a_rank": self.max_bytes_into_a_rank}
 
 
-class AlltoallvMiniapp:
+class AlltoallvMiniapp(CollectiveMiniapp):
     """One rank of the all-to-all-v.  ``capacity_rows`` rows of ``row_bytes`` are allocated for the send and for the
     receive buffer and declared to the kernel (``send_capacity_rows`` / ``recv_capacity_rows``; they must be the same
     on every rank).  ``exchange(x, splits)`` is the enqueue-only entry point; ``run()`` is the CLI's timed, checked loop."""
+
+    PATTERN = "alltoallv"
+    BUFFERS = ("send", "recv", "counts")
 
     def __init__(self, comm: Comm, device: int, row_bytes: int, capacity_rows: int, algo: str = "push", ctas: int = 0,
                  timeout_s: float = 30.0, _shared: Optional[dict] = None):
@@ -291,18 +231,12 @@ class AlltoallvMiniapp:
         if algo not in V_ALGOS:
             raise ValueError(f"algo must be one of {V_ALGOS}")
         check_v_args(comm.world, row_bytes, capacity_rows, capacity_rows)
-        if _shared is not None and algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
-        self.C = native()
-        self.comm, self.device = comm, device
-        self.rank, self.world = comm.rank, comm.world
-        self.algo, self.row_bytes, self.ctas = algo, int(row_bytes), ctas
+        super().__init__(comm, device, native(), algo, ctas, _shared, VIRTUAL_ALGOS)
+        self.row_bytes = int(row_bytes)
         self.send_capacity_rows = self.recv_capacity_rows = int(capacity_rows)
         self.nbytes = int(capacity_rows) * self.row_bytes
-        self.launch_ctas = 0
         self.generation = 0
         self.matrix: List[List[int]] = []       # run(): the count matrix of the last initialised iteration
-        torch.cuda.set_device(device)
         if _shared is not None:
             self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
             self.counts = _shared["counts"]
@@ -314,9 +248,6 @@ class AlltoallvMiniapp:
         dev = torch.device("cuda", device)
         self.recv_counts = torch.zeros(self.world, dtype=torch.int64, device=dev)
         self.verdict_word = torch.zeros(1, dtype=torch.int32, device=dev)
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     def rows(self, buf: SymmetricBuffer, dtype: torch.dtype = torch.uint8) -> torch.Tensor:
         """``buf`` (send or recv) as [capacity_rows, row] of ``dtype``."""
@@ -431,35 +362,15 @@ class AlltoallvMiniapp:
         mean = mean_rows(block_bytes, self.row_bytes)
         if 2 * self.world * mean > self.send_capacity_rows:
             raise ValueError(f"all-to-all-v: --counts needs {2 * self.world * mean} rows of capacity")
-        stream = torch.cuda.current_stream(self.device)
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        best, traffic = float("inf"), (0.0, 0.0)
-        for it in range(warmup + iters):
-            self.initialize(kind, mean)
-            torch.cuda.synchronize(self.device)
-            self.comm.barrier()
-            self.pads.device_barrier(stream.cuda_stream)
-            e0.record(stream)
-            self.run_once()
-            e1.record(stream)
-            stream.synchronize()
-            self.pads.check()
-            t = self.comm.max(e0.elapsed_time(e1))
-            if it >= warmup and t < best:
-                best, traffic = t, _traffic(self.matrix, self.row_bytes)
-        bad = self.mismatches()
-        total_bad = int(self.comm.sum(bad))
-        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong words", flush=True)
-        return AlltoallvResult(self.algo, self.world, block_bytes, self.row_bytes, kind, best, total_bad, *traffic,
-                               ctas=self.launch_ctas)
+        self._kind, self._block_bytes, self._traffic = kind, block_bytes, (0.0, 0.0)
+        return super().run(iters, warmup, kind, mean)
 
-    def close(self) -> None:
-        torch.cuda.synchronize(self.device)
-        self.send.close()
-        self.recv.close()
-        self.counts.close()
-        self.pads.close()
+    def at_best(self) -> None:
+        self._traffic = _traffic(self.matrix, self.row_bytes)
+
+    def result(self, ms: float, mismatches: int) -> AlltoallvResult:
+        return AlltoallvResult(self.algo, self.world, self._block_bytes, self.row_bytes, self._kind, ms, mismatches,
+                               *self._traffic, ctas=self.launch_ctas)
 
 
 def _traffic(m: List[List[int]], row_bytes: int):
@@ -470,26 +381,15 @@ def _traffic(m: List[List[int]], row_bytes: int):
     return float(off), float(into)
 
 
-class VirtualAlltoallv:
-    """``world`` AlltoallvMiniapp ranks driven by ONE process on one GPU, as ``VirtualAlltoall`` does (co-resident
-    grids of at most ``sms // world`` CTAs, at most 8 ranks)."""
-
-    MAX_WORLD = 8
+class VirtualAlltoallv(VirtualRanks):
+    """``world`` AlltoallvMiniapp ranks on one GPU (``VirtualRanks``)."""
 
     def __init__(self, world: int, row_bytes: int, capacity_rows: int, algo: str = "push", ctas: int = 0,
                  device: int = 0, timeout_s: float = 10.0):
-        from ..parallel.local import LocalGroup
-
-        if not 1 <= world <= self.MAX_WORLD:
-            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
-        if algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        self.refuse(world, algo, VIRTUAL_ALGOS)
         check_v_args(world, row_bytes, capacity_rows, capacity_rows)
-        C = native()
-        cap = max(1, C.sm_count(device) // world)
-        self.ctas = min(ctas, cap) if ctas > 0 else cap
-        self.world, self.row_bytes, self.capacity_rows, self.device = world, int(row_bytes), int(capacity_rows), device
-        self.group = LocalGroup(world, [device] * world)
+        super().__init__(world, device, ctas)
+        self.row_bytes, self.capacity_rows = int(row_bytes), int(capacity_rows)
         pads = self.group.pads(timeout_s=timeout_s)
         send = self.group.symmetric(self.capacity_rows * self.row_bytes, zero=False)
         recv = self.group.symmetric(self.capacity_rows * self.row_bytes, zero=False)
@@ -499,7 +399,6 @@ class VirtualAlltoallv:
                              timeout_s=timeout_s,
                              _shared={"pads": pads[r], "send": send[r], "recv": recv[r], "counts": counts[r]})
             for r in range(world)]
-        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, sends: List[torch.Tensor], counts: List) -> None:
         """Rank r's send buffer <- ``sends[r]`` (rows of row_bytes, any dtype, at most capacity_rows) and its counts
@@ -515,19 +414,6 @@ class VirtualAlltoallv:
             app.send.tensor()[: b.numel()].copy_(b)
             app.counts.tensor(torch.int64).copy_(torch.as_tensor(c, dtype=torch.int64).reshape(self.world))
         torch.cuda.synchronize(self.device)
-
-    def run_once(self) -> None:
-        """One all-to-all-v: every rank's ``run_once`` on its own stream.  Call ``synchronize`` before the next one (it
-        stands in for the cross-rank barrier of the precondition)."""
-        for app, st in zip(self.ranks, self.streams):
-            with torch.cuda.device(app.device), torch.cuda.stream(st):
-                app.run_once()
-
-    def synchronize(self) -> None:
-        for st in self.streams:
-            st.synchronize()
-        for app in self.ranks:
-            app.pads.check()
 
     def verdicts(self) -> List[int]:
         """Every rank's verdict word of the last launch."""
@@ -545,10 +431,6 @@ class VirtualAlltoallv:
             total = int(rc.sum())
             out.append((app.rows(app.recv)[:total].cpu(), rc))
         return out
-
-    def close(self) -> None:
-        for app in self.ranks:
-            app.close()
 
 
 # ------------------------------------------------------------------------------------------------------ all-gather ----
@@ -572,32 +454,25 @@ class AllgatherResult(AlltoallResult):
         return row
 
 
-class AllgatherMiniapp:
+class AllgatherMiniapp(CollectiveMiniapp):
+    PATTERN = "allgather"
+
     def __init__(self, comm: Comm, device: int, block_bytes: int = 16 << 20, algo: str = "push", ctas: int = 0,
                  timeout_s: float = 30.0, _shared: Optional[dict] = None):
         """``_shared``: buffers made by an in-process group (``VirtualAllgather``): ``pads``, ``send``, ``recv``."""
         if algo not in ALGOS:
             raise ValueError(f"algo must be one of {ALGOS}")
         check_gather_args(comm.world, block_bytes)
-        if _shared is not None and algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}: {algo} needs one process per GPU")
-        self.C = native()
-        self.comm, self.device = comm, device
-        self.rank, self.world = comm.rank, comm.world
-        self.algo, self.block_bytes, self.ctas = algo, int(block_bytes), ctas
+        super().__init__(comm, device, native(), algo, ctas, _shared, VIRTUAL_ALGOS)
+        self.block_bytes = int(block_bytes)
         self.nbytes = self.world * self.block_bytes
         self.generation = 0
-        self.launch_ctas = 0
-        torch.cuda.set_device(device)
         if _shared is not None:
             self.pads, self.send, self.recv = _shared["pads"], _shared["send"], _shared["recv"]
         else:
             self.pads = SignalPads(comm, device, timeout_s=timeout_s)
             self.send = SymmetricBuffer(comm, self.block_bytes, device, zero=False)
             self.recv = SymmetricBuffer(comm, self.nbytes, device, zero=False)
-
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
 
     def initialize(self) -> None:
         """My send block <- the pattern of (rank, a new iteration); the receive buffer <- the poison."""
@@ -648,55 +523,19 @@ class AllgatherMiniapp:
         torch.cuda.synchronize(self.device)
         return int(count.item())
 
-    def run(self, iters: int = 5, warmup: int = 1) -> AllgatherResult:
-        stream = torch.cuda.current_stream(self.device)
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        best = float("inf")
-        for it in range(warmup + iters):
-            self.initialize()
-            torch.cuda.synchronize(self.device)
-            self.comm.barrier()
-            self.pads.device_barrier(stream.cuda_stream)
-            e0.record(stream)
-            self.run_once()
-            e1.record(stream)
-            stream.synchronize()
-            self.pads.check()
-            t = self.comm.max(e0.elapsed_time(e1))
-            if it >= warmup:
-                best = min(best, t)
-        bad = self.mismatches()
-        total_bad = int(self.comm.sum(bad))
-        print(f"Passed {self.rank}" if bad == 0 else f"FAILED {self.rank}: {bad} wrong words", flush=True)
-        return AllgatherResult(self.algo, self.world, self.block_bytes, best, total_bad, self.launch_ctas)
-
-    def close(self) -> None:
-        torch.cuda.synchronize(self.device)
-        self.send.close()
-        self.recv.close()
-        self.pads.close()
+    def result(self, ms: float, mismatches: int) -> AllgatherResult:
+        return AllgatherResult(self.algo, self.world, self.block_bytes, ms, mismatches, self.launch_ctas)
 
 
-class VirtualAllgather:
-    """``world`` AllgatherMiniapp ranks driven by ONE process on one GPU, as ``VirtualAlltoall`` does."""
-
-    MAX_WORLD = 8
+class VirtualAllgather(VirtualRanks):
+    """``world`` AllgatherMiniapp ranks on one GPU (``VirtualRanks``)."""
 
     def __init__(self, world: int, block_bytes: int, algo: str = "push", ctas: int = 0, device: int = 0,
                  timeout_s: float = 10.0):
-        from ..parallel.local import LocalGroup
-
-        if not 1 <= world <= self.MAX_WORLD:
-            raise ValueError(f"virtual ranks: 1 <= world <= {self.MAX_WORLD}")
-        if algo not in VIRTUAL_ALGOS:
-            raise ValueError(f"virtual ranks run {VIRTUAL_ALGOS}")
+        self.refuse(world, algo, VIRTUAL_ALGOS)
         check_gather_args(world, block_bytes)
-        C = native()
-        cap = max(1, C.sm_count(device) // world)
-        self.ctas = min(ctas, cap) if ctas > 0 else cap
-        self.world, self.block_bytes, self.device = world, int(block_bytes), device
-        self.group = LocalGroup(world, [device] * world)
+        super().__init__(world, device, ctas)
+        self.block_bytes = int(block_bytes)
         pads = self.group.pads(timeout_s=timeout_s)
         send = self.group.symmetric(self.block_bytes, zero=False)
         recv = self.group.symmetric(world * self.block_bytes, zero=False)
@@ -704,7 +543,6 @@ class VirtualAllgather:
             AllgatherMiniapp(self.group.comms[r], device, self.block_bytes, algo, ctas=self.ctas, timeout_s=timeout_s,
                              _shared={"pads": pads[r], "send": send[r], "recv": recv[r]})
             for r in range(world)]
-        self.streams = [torch.cuda.Stream(device) for _ in range(world)]
 
     def load(self, sends: List[torch.Tensor]) -> None:
         """Send block of rank r <- the bytes of ``sends[r]`` (``block_bytes`` of any dtype)."""
@@ -718,26 +556,10 @@ class VirtualAllgather:
             app.send.tensor().copy_(b)
         torch.cuda.synchronize(self.device)
 
-    def run_once(self) -> None:
-        """One all-gather: every rank's ``run_once`` on its own stream; ``synchronize`` before the next one."""
-        for app, st in zip(self.ranks, self.streams):
-            with torch.cuda.device(app.device), torch.cuda.stream(st):
-                app.run_once()
-
-    def synchronize(self) -> None:
-        for st in self.streams:
-            st.synchronize()
-        for app in self.ranks:
-            app.pads.check()
-
     def results(self) -> List[torch.Tensor]:
         """The receive buffer of every rank as a [P, B] uint8 tensor on the host."""
         self.synchronize()
         return [app.recv.tensor().cpu().reshape(self.world, self.block_bytes) for app in self.ranks]
-
-    def close(self) -> None:
-        for app in self.ranks:
-            app.close()
 
 
 def main_allgather(argv: Optional[List[str]] = None) -> int:
@@ -756,16 +578,7 @@ def main_allgather(argv: Optional[List[str]] = None) -> int:
     comm = Comm()
     app = AllgatherMiniapp(comm, comm.device, args.block_bytes, args.algo, ctas=args.ctas)
     res = app.run(args.iters, args.warmup)
-    if comm.rank == 0:
-        row = res.row()
-        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | allgather {args.algo} "
-              f"P={comm.world} B={args.block_bytes} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank", flush=True)
-        if args.json:
-            with open(args.json, "a") as f:
-                f.write(json.dumps(row) + "\n")
-    app.close()
-    comm.close()
-    return 0 if res.mismatches == 0 else 1
+    return report(comm, app, res, args, f"allgather {args.algo} P={comm.world} B={args.block_bytes}")
 
 
 def main(argv: Optional[List[str]] = None) -> int:
@@ -785,37 +598,16 @@ def main(argv: Optional[List[str]] = None) -> int:
     args = ap.parse_args(argv)
     comm = Comm()
     if args.counts:
-        return _main_v(comm, args)
-    app =AlltoallMiniapp(comm, comm.device, args.block_bytes, args.algo, ctas=args.ctas)
-    res = app.run(args.iters, args.warmup)
-    if comm.rank == 0:
-        row = res.row()
-        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | alltoall {args.algo} "
-              f"P={comm.world} B={args.block_bytes} | {row['GBps_sent_per_rank']:.1f} GB/s sent per rank", flush=True)
-        if args.json:
-            with open(args.json, "a") as f:
-                f.write(json.dumps(row) + "\n")
-    app.close()
-    comm.close()
-    return 0 if res.mismatches == 0 else 1
+        mean = mean_rows(args.block_bytes, args.row_bytes)
+        app = AlltoallvMiniapp(comm, comm.device, args.row_bytes, 2 * comm.world * mean, args.algo, ctas=args.ctas)
+        res = app.run(args.counts, args.block_bytes, args.iters, args.warmup)
+        what = f"alltoallv {args.algo} {args.counts} P={comm.world} B={args.block_bytes} R={args.row_bytes}"
+    else:
+        app = AlltoallMiniapp(comm, comm.device, args.block_bytes, args.algo, ctas=args.ctas)
+        res = app.run(args.iters, args.warmup)
+        what = f"alltoall {args.algo} P={comm.world} B={args.block_bytes}"
+    return report(comm, app, res, args, what)
 
 
 if __name__ == "__main__":
     raise SystemExit(main())
-
-
-def _main_v(comm: Comm, args) -> int:
-    mean = mean_rows(args.block_bytes, args.row_bytes)
-    app = AlltoallvMiniapp(comm, comm.device, args.row_bytes, 2 * comm.world * mean, args.algo, ctas=args.ctas)
-    res = app.run(args.counts, args.block_bytes, args.iters, args.warmup)
-    if comm.rank == 0:
-        row = res.row()
-        print(f"Elapsed (max over ranks, min of {args.iters}): {res.ms:.4f} ms | alltoallv {args.algo} {args.counts} "
-              f"P={comm.world} B={args.block_bytes} R={args.row_bytes} | {row['GBps_sent_per_rank']:.1f} GB/s sent "
-              f"per rank", flush=True)
-        if args.json:
-            with open(args.json, "a") as f:
-                f.write(json.dumps(row) + "\n")
-    app.close()
-    comm.close()
-    return 0 if res.mismatches == 0 else 1
