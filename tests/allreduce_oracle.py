@@ -7,11 +7,13 @@ computed operation by operation in the element type:
 
 * ``make_inputs``     one VA per rank; integers over their full range (sums wrap, carries cross every byte and 32-bit
                       boundary), floats from a normal distribution, or integer-valued floats in +-2^20 (``exact``:
-                      every sum of at most 8 of them is exact in any order);
+                      every partial sum of at most 16 of them, the most ranks a kernel takes, is exact in any order);
 * ``ring_expected``   VC of the fused ring (push and pull, both slot policies) and of the unfused ring, bit for bit:
                       rank r adds VA[r], VA[r-1], ..., VA[r-P+1] into a zeroed VC, one add at a time;
 * ``allreduce_bound`` the fp64 sum and the error bound of recursive summation in any order, for two-shot, whose
                       order differs between its main blocks (owner first) and its tail loop (rank 0 first);
+* ``two_shot_sum_pinned`` two-shot's float and double sum in exactly the kernel's order (main blocks owner first, tail
+                      vectors rank 0 first, the boundary from ``TWO_SHOT_SHAPES``), bit for bit;
 * ``mismatches`` / ``two_shot_problems`` the comparisons the GPU tests assert on.
 """
 from __future__ import annotations
@@ -28,7 +30,24 @@ TORCH_DTYPE = {"float": torch.float32, "int": torch.int32, "uint": torch.int32, 
                "long": torch.int64, "ulong": torch.int64, "short": torch.int16, "ushort": torch.int16,
                "uchar": torch.uint8}
 EXACT_RANGE = 1 << 20
+MAX_RANKS = 16              # kApiMaxRanks (csrc/kernels/api.h)
 _BITS = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+# Two-shot's <W, U> by world size (kTwoShotShapes, csrc/kernels/ring_allreduce.cuh): the first row with world <= W runs.
+# Every launch has 512 threads per CTA, and a CTA reduces 512 * U vectors per trip of the main loop.
+TWO_SHOT_SHAPES = ((2, 4), (4, 4), (8, 2), (16, 1))
+TWO_SHOT_THREADS = 512
+
+
+def two_shot_u(world: int) -> int:
+    """U of the two-shot kernel that runs at ``world`` ranks."""
+    return next(u for w, u in TWO_SHOT_SHAPES if world <= w)
+
+
+def two_shot_main_vectors(slice_vec: int, world: int, u: int = 0) -> int:
+    """Vectors of a slice of ``slice_vec`` that the main blocks reduce; the tail loop takes the rest (``u`` overrides
+    the kernel's U)."""
+    block = TWO_SHOT_THREADS * (u or two_shot_u(world))
+    return slice_vec // block * block
 
 
 def elem_bytes(dtype: str) -> int:
@@ -78,6 +97,28 @@ def allreduce_bound(vas: List[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor
     k = world - 1
     gamma = k * u / (1 - k * u) + k * 2.0 ** -53
     return x.sum(0), gamma * x.abs().sum(0)
+
+
+def two_shot_sum_pinned(vas: List[torch.Tensor], u: int = 0) -> torch.Tensor:
+    """VC of every rank after a float or double two-shot sum, in the kernel's order: within slice s, the main-block
+    vectors add owner first, ((VA[s] + VA[s+1]) + ...) + VA[s+P-1] (ranks mod P), and the tail vectors rank 0 first,
+    ((VA[0] + VA[1]) + ...) + VA[P-1], one IEEE add at a time.  ``u`` overrides the kernel's U."""
+    world, n = len(vas), vas[0].numel()
+    if vas[0].dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"the pinned order is the float and double sum's, not {vas[0].dtype}'s")
+    per, per_vec = n // world, 16 // vas[0].element_size()
+    main = two_shot_main_vectors(per // per_vec, world, u) * per_vec
+    out = []
+    for s in range(world):
+        lo = s * per
+        head = vas[s][lo:lo + main].clone()
+        for q in range(1, world):
+            head = head + vas[(s + q) % world][lo:lo + main]
+        tail = vas[0][lo + main:lo + per].clone()
+        for p in range(1, world):
+            tail = tail + vas[p][lo + main:lo + per]
+        out += [head, tail]
+    return torch.cat(out)
 
 
 def bits(t: torch.Tensor) -> torch.Tensor:

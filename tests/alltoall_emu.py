@@ -7,6 +7,8 @@ barrier.  ``fault`` plants one defect in the walk of rank ``fault_rank`` (the te
   misroute    the blocks for ranks 0 and 2 swap destinations (slot ``rank`` of the wrong rank)
   skip-local  the local block is never copied
   short-tail  the block for rank 0 loses its last 16-byte vector
+  slot-minus-8  (9 or more ranks) push stores into slot ``rank - 8`` of every receive buffer, pull loads slot
+              ``rank - 8`` of every send buffer, instead of slot ``rank``
 
 In one process the ranks run one after another, so a rank's node barrier cannot be waited for inside its launch: the
 waits are kept and checked when the status word is read (``SignalPads.check``, i.e. at the synchronize that observes
@@ -20,7 +22,7 @@ from hpc_patterns_b200.models import alltoall as alltoall_mod
 from hpc_patterns_b200.ops import alltoall as alltoall_ops
 from tests.emu_device import EmuNative, SharedEmuNative, _u32
 
-FAULTS = ("misroute", "skip-local", "short-tail")
+FAULTS = ("misroute", "skip-local", "short-tail", "slot-minus-8")
 
 
 class AlltoallEmu:
@@ -39,6 +41,7 @@ class AlltoallEmu:
         if not (send[rank] + world * B <= recv[rank] or recv[rank] + world * B <= send[rank]):
             raise RuntimeError(self.real.ALL_TO_ALL_OVERLAP_ERROR)
         faulty = self.fault is not None and rank == self.fault_rank
+        slot = rank - 8 if faulty and self.fault == "slot-minus-8" else rank
         for j in range(world):
             p = (rank + 1 + j) % world
             n = B
@@ -50,9 +53,9 @@ class AlltoallEmu:
             if faulty and self.fault == "misroute" and p in (0, 2):
                 to = 2 - p
             if pull:       # my block `to` <- slot `rank` of rank p's send
-                ctypes.memmove(recv[rank] + to * B, send[p] + rank * B, n)
+                ctypes.memmove(recv[rank] + to * B, send[p] + slot * B, n)
             else:          # slot `rank` of rank `to` <- my send block p
-                ctypes.memmove(recv[to] + rank * B, send[rank] + p * B, n)
+                ctypes.memmove(recv[to] + slot * B, send[rank] + p * B, n)
         self._node_barrier(pads, rank, barrier_epoch)
         self.launches.append(("all_to_all", rank, pull))
         return self.ctas

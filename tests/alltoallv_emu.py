@@ -11,6 +11,8 @@ emulation, not the program):
   copy-refused      a refused matrix is copied anyway
   no-recv-counts    recv_counts is never written
   short-segment     every segment loses its last 16-byte vector
+  rows-below-8      the judge reads only rows 0..7 of the matrix (a count broken in row 8 or later is accepted; what it
+                    then copies is kept inside the buffers, as with copy-refused)
 """
 import ctypes
 
@@ -21,7 +23,7 @@ from hpc_patterns_b200.models import alltoall as alltoall_mod
 from hpc_patterns_b200.ops import alltoall as alltoall_ops
 from tests.alltoall_emu import AlltoallEmu, AlltoallEmuNative, AlltoallSharedEmuNative, _u32
 
-FAULTS = ("inclusive-prefix", "row-recv-offset", "copy-refused", "no-recv-counts", "short-segment")
+FAULTS = ("inclusive-prefix", "row-recv-offset", "copy-refused", "no-recv-counts", "short-segment", "rows-below-8")
 
 
 def _i64(ptr, n):
@@ -43,10 +45,14 @@ class AlltoallvEmu(AlltoallEmu):
         m = [int(c) for p in range(P) for c in _i64(counts[p], P)]
         v = C.alltoallv_verdict(m, P, send_capacity_rows, recv_capacity_rows)
         faulty = self.fault is not None and rank == self.fault_rank
+        clamp = faulty and self.fault == "copy-refused"
+        if faulty and self.fault == "rows-below-8":
+            clamp = v != 0
+            v = C.alltoallv_verdict(m[:8 * P] + [0] * (P - 8) * P, P, send_capacity_rows, recv_capacity_rows)
         if not (faulty and self.fault == "no-recv-counts"):
             _i64(recv_counts, P)[:] = [m[p * P + rank] for p in range(P)]
         _u32(verdict).value = v
-        if v == 0 or (faulty and self.fault == "copy-refused"):
+        if v == 0 or clamp:
             for j in range(P):
                 p = (rank + 1 + j) % P
                 s, r = (p, rank) if pull else (rank, p)
@@ -62,7 +68,7 @@ class AlltoallvEmu(AlltoallEmu):
                     dst = C.alltoallv_send_offset(m, P, r, s)
                 if faulty and self.fault == "short-segment":
                     nbytes -= 16
-                if faulty and self.fault == "copy-refused":        # a kernel without the verdict stays in its buffers
+                if clamp:                  # a kernel without the (right) verdict stays in its buffers
                     src, dst = src % send_capacity_rows, dst % recv_capacity_rows
                     n = min(n, send_capacity_rows - src, recv_capacity_rows - dst)
                     nbytes = n * R

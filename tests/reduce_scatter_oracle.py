@@ -30,19 +30,25 @@ def expected(sends, r: int, op: str, dtype: str):
     world = len(sends)
     order = [(r + k) % world for k in range(world)]
     if dtype in loc.PAIR_TYPES:
-        size = loc.pair_bytes(dtype)
         seg = len(sends[0]) // world
-        parts = [loc.unpack_all(sends[p][r * seg:(r + 1) * seg], dtype) for p in order]
-        if world == 1:
-            return bytes(sends[0][r * seg:(r + 1) * seg])
+        return fold([sends[p][r * seg:(r + 1) * seg] for p in order], op, dtype)
+    return fold([_segments(sends[p], world)[r] for p in order], op, dtype)
+
+
+def fold(segs, op: str, dtype: str):
+    """((segs[0] o segs[1]) o ...) element by element, in the kernels' arithmetic (the module docstring): tensors of the
+    dtype's torch type, or bytes for a pair type.  One part comes back as it is."""
+    if dtype in loc.PAIR_TYPES:
+        if len(segs) == 1:
+            return bytes(segs[0])
+        parts = [loc.unpack_all(s, dtype) for s in segs]
         out = []
-        for k in range(seg // size):
+        for k in range(len(parts[0])):
             acc = parts[0][k]
             for part in parts[1:]:
                 acc = loc.combine(op, acc, part[k])
             out.append(loc.pack_result(acc, dtype))
         return b"".join(out)
-    segs = [_segments(sends[p], world)[r] for p in order]
     if op == "sum":
         if dtype in LOWP:
             acc = segs[0].float()

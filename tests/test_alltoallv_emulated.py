@@ -215,4 +215,5 @@ def test_refusal_words_are_the_same_in_every_layer(emu):
         VirtualAlltoallv(2, 16, 4, "nccl")
     with pytest.raises(ValueError, match="random, skewed or equal"):
         a2a.draw_counts("uniform", 2, 1, 0)
-    assert set(FAULTS) == {"inclusive-prefix", "row-recv-offset", "copy-refused", "no-recv-counts", "short-segment"}
+    assert set(FAULTS) == {"inclusive-prefix", "row-recv-offset", "copy-refused", "no-recv-counts", "short-segment",
+                           "rows-below-8"}

@@ -14,13 +14,13 @@ import torch
 
 from hpc_patterns_b200.models.alltoall import VirtualAlltoall, VirtualAlltoallv
 from hpc_patterns_b200.ops.alltoall import VERDICT_WORDS, all_to_all_v_reference
+from tests.alltoallv_oracle import PATTERNS, counts_for
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ROWS = [16, 48, 4096 + 16]
 MEAN = 24                       # mean rows per pair; every instance has capacities of 2 * P * MEAN rows
-PATTERNS = ["random", "zero", "single", "local", "column-at-capacity", "skewed"]
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -32,34 +32,6 @@ def first_launches(native):
         v.run_once()
         v.synchronize()
         v.close()
-
-
-def counts_for(pattern, P, mean, cap, launch, gen):
-    """A P x P matrix (list of lists) that fits capacities of `cap` rows; a new one for every launch."""
-    ri = lambda hi: int(torch.randint(0, hi + 1, (1,), generator=gen))
-    m = [[0] * P for _ in range(P)]
-    if pattern == "random":
-        m = [[ri(2 * mean) for _ in range(P)] for _ in range(P)]
-        for _ in range(max(1, P // 2)):
-            m[ri(P - 1)][ri(P - 1)] = 0
-    elif pattern == "single":
-        m[launch % P][(launch * 7 + 1) % P] = 1 + ri(cap - 1)
-    elif pattern == "local":
-        for p in range(P):
-            m[p][p] = 1 + ri(2 * mean)
-    elif pattern == "column-at-capacity":
-        c = launch % P
-        for p in range(P):
-            for q in range(P):
-                m[p][q] = ri(mean // P)
-        for p in range(P):
-            m[p][c] = cap // P + (cap % P if p == P - 1 else 0)
-    elif pattern == "skewed":
-        hot = launch % P
-        for p in range(P):
-            for q in range(P):
-                m[p][q] = 2 * mean if q == hot else ri(mean // P)
-    return m
 
 
 def run_and_check(v, m, gen, launch):
